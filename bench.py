@@ -6,7 +6,11 @@ Main workload (configs[1]): SD-XL base 1.0 UNet2DConditionModel, batch 8 per GPU
 denoising timestep = one UNet forward over the batch + the fused DDIM update. Metric = denoiser-forward latents/s
 (images pushed through one denoiser forward per second, whole job); finished latents/s = that / 50.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step returned on rank 0: DIR/latents.npy (the
+DDIM-updated latents) and DIR/noise_pred.npy (the UNet output), float32. Inputs and weights are seeded, so two builds
+run with the same arguments can be compared output for output.
 
 N > 1 is launched by `python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...`: one rank per GPU,
 images sharded, weights replicated, no per-step communication, one NCCL all_gather of the finished latents.
@@ -54,7 +58,7 @@ REF_STEPS, REF_WARMUP = 3, 1  # reference / cpu_baseline legs: fixed sample coun
 
 
 class ClockSampler(threading.Thread):
-    """Samples nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """Samples nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -83,15 +87,7 @@ class ClockSampler(threading.Thread):
 
 
 def igemm_traffic_per_launch():
-    """DRAM bytes (read + write) per igemm launch, averaged over the launches of one SDXL forward. NOT measured in this
-    run: it comes from a committed `ncu --metrics dram__bytes_read.sum,dram__bytes_write.sum` pass of the same forward
-    (tools/gpu_ncu.sh); returns (value, source file) or (None, None)."""
-    for name in ("r02_igemm_dram_traffic.json", "r01_igemm_dram_traffic.json"):
-        try:
-            with open(os.path.join(ROOT, "profiles", name)) as f:
-                return json.load(f)["dram_bytes_per_launch"], f"profiles/{name} (ncu pass, not measured in this run)"
-        except Exception:  # noqa: BLE001
-            continue
+    """DRAM bytes per igemm launch are not measured by this benchmark (no hardware counters on the bench machines)."""
     return None, None
 
 
@@ -100,7 +96,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d.get("bf16_tflops_sustained", 1400.0), d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json, sustained)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense bf16, HBM3), not measured"
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -257,6 +253,7 @@ def sdxl_section(c, unet, B, height, steps, warmup, with_e2e=True, sample_clocks
         eps = den(state["lat"], float(t))
         sched.step(eps, t, state["lat"], out=state["nxt"])
         state["lat"], state["nxt"] = state["nxt"], state["lat"]
+        state["eps"] = eps
 
     sampler = ClockSampler(c.local) if (sample_clocks and c.rank == 0) else None
     for i in range(warmup):
@@ -269,7 +266,9 @@ def sdxl_section(c, unet, B, height, steps, warmup, with_e2e=True, sample_clocks
     launches = ops.launches() - n0
     if sampler:
         sampler.stop_flag = True
-    res = {"ms": ms, "launches": launches, "clocks": sampler.summary() if sampler else None, "den": den, "state": s}
+    res = {"ms": ms, "launches": launches, "clocks": sampler.summary() if sampler else None, "den": den, "state": s,
+           # what the last timed step returned (later sections keep stepping the same buffers)
+           "outputs": {"latents": state["lat"].float().cpu().numpy(), "noise_pred": state["eps"].float().cpu().numpy()}}
 
     # job level: K steps + the path's only collective (all_gather of the finished latents) + D2H of the gathered result
     gathered_h = torch.empty(B * c.world, 4, H, H).pin_memory() if c.rank == 0 else None
@@ -376,7 +375,7 @@ def roofline_section(c, unet, B, height):
         a = v["work"] / (v["ms"] * 1e-3) / (1e12 if flop else 1e9)
         fam[k] = {"ms": round(v["ms"], 3), "achieved": round(a, 1), "unit": "TFLOP/s" if flop else "GB/s",
                   "frac": round(a / (peak_tf if flop else peak_gbs), 4), "launches": v["calls"]}
-    return {"kernel": "igemm_kernel (tcgen05 implicit GEMM: linear + conv3x3)", "bound": "tensor",
+    return {"kernel": "igemm_kernel (wgmma implicit GEMM: linear + conv3x3)", "bound": "tensor",
             "achieved": round(ach, 1), "peak": peak_tf, "unit": "TFLOP/s", "frac": round(ach / peak_tf, 4),
             "traffic": traffic, "traffic_source": tsrc, "peak_source": how, "launches_per_step": ig["calls"],
             "avg_launch_ms": round(ig["ms"] / ig["calls"], 4), "share_of_step": round(ig["ms"] / total_ms, 3),
@@ -479,7 +478,7 @@ def stdit2_section(c, steps, warmup, global_batch=4):
 
 def bench_qwen2vl_prefill(dev, steps=20, warmup=5):
     """Second half of BASELINE.json's metric: Qwen2-VL-7B prefill tokens/s (configs[3]: 4 x (one 448x448 image +
-    512 text tokens) = 4 x 768 tokens, bf16, 1 x B200, ViT + 28 decoder layers + lm_head over all positions)."""
+    512 text tokens) = 4 x 768 tokens, bf16, 1 GPU, ViT + 28 decoder layers + lm_head over all positions)."""
     import torch
 
     from paddlemix_b200 import ops
@@ -566,7 +565,18 @@ def parity_section(c, keep):
     return {"config": "configs[1] shape: SDXL-base UNet, latent 128x128, B=1, t=981 (GPU bf16 kernels vs CPU fp32 oracle, "
                       "same weights and inputs)", "cosine": round(cos, 6), "max_rel_err": round(err, 5),
             "tolerance": PARITY_TOL, "pass": bool(cos >= PARITY_TOL["cosine_min"] and err <= PARITY_TOL["max_rel_err"]),
-            "more": "tests/test_baseline_parity_gpu.py covers configs[1..4] shapes; profiles/ holds the recorded values"}
+            "more": "tests/test_baseline_parity_gpu.py covers configs[1..4] shapes"}
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes each array as out_dir/<name>.npy (float32), at most 64 MB in all."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    total = sum(a.astype(np.float32).nbytes for a in arrays.values())
+    if total > 64 << 20:
+        raise ValueError(f"outputs of {total} bytes exceed the 64 MB dump limit")
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 def run_b200(args):
@@ -580,6 +590,8 @@ def run_b200(args):
 
     main = sdxl_section(c, unet, B, height, args.steps, args.warmup, with_e2e=True, sample_clocks=True)
     ms, ms_e2e = main["ms"], main["e2e"]["ms"]
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, main.pop("outputs"))
     roof = roofline_section(c, unet, B, height) if rank == 0 else None
 
     extras = {}
@@ -656,7 +668,7 @@ def run_b200(args):
                    "cfg": "off (UNet rows = batch)",
                    "parallelism": f"dp{world} (images sharded, weights replicated, one all_gather of finished latents)",
                    "weights": "random init, SDXL-base architecture (2.57 B params)", "cuda_graph": True,
-                   "l2": "no explicit flush: 5.1 GB of weights + >10 GB of activations stream per step (>> 126 MB L2)"},
+                   "l2": "no explicit flush: 5.1 GB of weights + >10 GB of activations stream per step (>> 50 MB L2)"},
         "finished_latents_per_sec_50_steps": round(value / 50.0, 4),
         "model_tflops_per_sec": None if step_tflop is None else round(step_tflop * world / (ms / args.steps * 1e-3), 1),
         "clocks": clocks,
@@ -687,6 +699,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-qwen", action="store_true", help="skip the Qwen2-VL-7B prefill section")
     ap.add_argument("--no-extras", action="store_true", help="skip the strong-scaling / SD3 / STDiT2 sections")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "b200":
         args.warmup = 3

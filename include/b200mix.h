@@ -1,5 +1,5 @@
 /*
- * b200mix — C ABI of the B200-native (sm_100a) hot path that replaces, for PaddleMIX's denoiser-forward /
+ * b200mix — C ABI of the H100-native (sm_90a) hot path that replaces, for PaddleMIX's denoiser-forward /
  * ViT+LLM attention path, the arithmetic the reference delegates to paddlepaddle-gpu and to its Triton custom ops.
  *
  * Conventions (mirrors the ownership model of the reference's custom ops, paddlemix/triton_ops/triton_ops.py:641-693:
@@ -13,7 +13,7 @@
  *   - every function returns 0 on success or a negative b200mix_status and never aborts;
  *     b200mix_last_error() returns a thread-local message for the last failure;
  *   - `stream` is a cudaStream_t passed as void*.
- * There is no CPU fallback: every entry point fails with B200MIX_ERR_NO_DEVICE when no sm_100 device is present.
+ * There is no CPU fallback: every entry point fails with B200MIX_ERR_NO_DEVICE when no sm_90 device is present.
  */
 #ifndef B200MIX_H_
 #define B200MIX_H_
@@ -28,7 +28,7 @@ typedef enum b200mix_status {
   B200MIX_OK = 0,
   B200MIX_ERR_INVALID = -1,   /* bad shape / alignment / argument */
   B200MIX_ERR_CUDA = -2,      /* a CUDA runtime/driver call failed */
-  B200MIX_ERR_NO_DEVICE = -3, /* no sm_100 device visible */
+  B200MIX_ERR_NO_DEVICE = -3, /* no sm_90 device visible */
   B200MIX_ERR_UNSUPPORTED = -4
 } b200mix_status;
 
@@ -81,7 +81,7 @@ typedef struct b200mix_epilogue {
 
 const char* b200mix_last_error(void);
 const char* b200mix_version(void);
-/* Select the device for the calling thread and verify it is sm_100. Replaces paddle.set_device / the implicit
+/* Select the device for the calling thread and verify it is sm_90. Replaces paddle.set_device / the implicit
  * place of paddle::Tensor in the reference ops. */
 int b200mix_init(int device);
 int b200mix_num_sms(void);
@@ -104,7 +104,7 @@ int b200mix_comm_init(void** comm, int32_t world_size, int32_t rank, const void*
 int b200mix_allgather_latents(void* comm, const void* send, void* recv, int64_t bytes_per_rank, void* stream);
 int b200mix_comm_destroy(void* comm);
 
-/* ---- dense contractions on tcgen05 tensor cores (TMA -> smem -> tcgen05.mma -> TMEM -> fused epilogue) ------- */
+/* ---- dense contractions on wgmma tensor cores (TMA -> smem -> wgmma -> registers -> fused epilogue) ----------- */
 
 /* C[M, N(/2 if glu)] = epilogue(A[M,K] @ W[N,K]^T). Replaces F.linear (ppdiffusers/models/lora.py:453-459) and
  * 1x1 conv on NHWC (lora.py:365-377). A, W bf16; lda/ldw/ldc in elements, multiples of 8. */
@@ -141,7 +141,7 @@ int b200mix_conv3x3_up2x(const void* x, const void* w4, void* y, int64_t B, int6
 int b200mix_conv3x3_small_cin(const void* x, int32_t x_fp32, const void* w, const float* bias, void* y, int64_t B,
                               int64_t H, int64_t W, int64_t Cin, int64_t Cout, void* stream);
 
-/* Scaled dot-product attention, flash-style on tcgen05 (S=QK^T and O+=PV in TMEM, online softmax in registers).
+/* Scaled dot-product attention, flash-style on wgmma (S=QK^T and O+=PV in registers, online softmax in registers).
  * Full signature of scaled_dot_product_attention_(query, key, value, attn_mask, dropout_p=0, is_causal, scale)
  * (ppdiffusers/patches/paddle_patch.py:414-424), semantics of its `math` branch (:445-461):
  *   softmax(q k^T * scale [+ attn_mask | causal mask]) v.

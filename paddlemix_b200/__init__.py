@@ -1,4 +1,4 @@
-"""paddlemix_b200 — B200-native (sm_100a) implementation of PaddleMIX's denoiser-forward / ViT+LLM attention hot path.
+"""paddlemix_b200 — H100-native (sm_90a) implementation of PaddleMIX's denoiser-forward / ViT+LLM attention hot path.
 
 Layout: csrc/ (hand-written CUDA kernels + C ABI -> libb200mix.so), _lib.py (ctypes binding), ops.py (tensor-level
 wrappers), ppdiffusers/ (host-side mirrors of the reference's UNet2DConditionModel / schedulers / pipeline loop).

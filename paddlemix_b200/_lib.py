@@ -1,7 +1,7 @@
 """ctypes binding of libb200mix.so (the C ABI declared in include/b200mix.h).
 
 This is the only way the Python host code reaches the device. There is no fallback: if the shared library is
-missing, importing this module raises, and every entry point returns B200MIX_ERR_NO_DEVICE without an sm_100 GPU.
+missing, importing this module raises, and every entry point returns B200MIX_ERR_NO_DEVICE without an sm_90 GPU.
 """
 import ctypes
 import os
@@ -126,14 +126,8 @@ def _load():
         getattr(lib, name).argtypes = []
     lib.b200mix_debug_force_bn.argtypes = [c_int]
     lib.b200mix_debug_force_bn.restype = None
-    lib.b200mix_debug_attn_ptmem.argtypes = [c_int]
-    lib.b200mix_debug_attn_ptmem.restype = None
     lib.b200mix_debug_attn_bn64.argtypes = [c_int]
     lib.b200mix_debug_attn_bn64.restype = None
-    lib.b200mix_debug_no_shortkv.argtypes = [c_int]
-    lib.b200mix_debug_no_shortkv.restype = None
-    lib.b200mix_debug_attn_pingpong.argtypes = [c_int]
-    lib.b200mix_debug_attn_pingpong.restype = None
     lib.b200mix_debug_gemm_pair.argtypes = [c_int]
     lib.b200mix_debug_gemm_pair.restype = None
     lib.b200mix_debug_ln_register_only.argtypes = [c_int]

@@ -1,4 +1,4 @@
-"""CLIP text / vision transformers on the sm_100a kernels — host-side mirrors of
+"""CLIP text / vision transformers on the sm_90a kernels — host-side mirrors of
 ppdiffusers/ppdiffusers/transformers/clip/modeling.py (CLIPTextModel :845-897, CLIPTextModelWithProjection :1231-1304,
 CLIPVisionModel :956-1006) — the text encoders in front of the denoising loop (SURVEY.md §8 f2) and LLaVA's vision
 tower (paddlemix/models/llava/clip_model.py:945-1078, §8 a19).

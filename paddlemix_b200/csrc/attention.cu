@@ -1,14 +1,13 @@
-// Flash-style scaled-dot-product attention on tcgen05 tensor cores.
+// Flash-style scaled-dot-product attention on Hopper tensor cores (wgmma).
 //
-// One CTA = one 128-row query tile of one (batch, head). 192 threads (the two single-thread roles have the highest warp
-// ids: the sub-partition scheduler prefers the highest eligible warp id, so they are not starved by the softmax warps):
-//   warp 5     TMA producer: Q once, then K/V tiles through a shared-memory ring (128B swizzle)
-//   warp 4     TMEM owner + MMA issuer: S[j&1] = Q K_j^T (K-major x K-major), O += P_j V_j (P K-major from smem,
-//              V consumed in its natural [kv, d] layout as an MN-major B operand)
-//   warps 0-3  softmax: one query row per thread (TMEM lane == row, so row max / row sum need no shuffles),
-//              online softmax in fp32 with exp2, lazy rescale of the TMEM-resident O accumulator (only when the
-//              running max grows by more than 2^8), P written as bf16 into swizzled smem for the second MMA.
-// QK^T of tile j+1 is issued before softmax(j) finishes, so tensor cores and MUFU overlap.
+// One CTA = one 128-row query tile of one (batch, head). 288 threads:
+//   warp 8     TMA producer: Q once, then K/V tiles through a shared-memory ring (128B swizzle)
+//   warps 0-7  two consumer warpgroups; warpgroup g owns query rows [64 g, 64 g + 64): S = Q K_j^T (wgmma, both operands
+//              K-major in shared memory, fp32 accumulators in registers), online softmax in fp32 with exp2 and a lazy
+//              rescale of the register-resident O (only when the running max grows by more than 2^8), then
+//              O += P_j V_j with P taken straight from registers as the bf16 A operand and V consumed in its natural
+//              [kv, d] layout as an MN-major B operand. The two warpgroups interleave: while one exponentiates, the
+//              other's MMAs use the tensor cores.
 //
 // Semantics follow the reference's `math` SDPA (ppdiffusers/patches/paddle_patch.py:445-461): softmax(q k^T * scale
 // [+ causal]) v, [B,S,H,D] in / out; GQA per modeling_qwen2_vl.py:497-506; varlen block-diagonal per :354-381.
@@ -37,23 +36,6 @@ struct AttnParams {
   float inv_scale;  // 1 / scale: the bias is folded into the raw score as s + mask * inv_scale
 };
 
-// Adds the mask bias of keys [k0, k0 + 32) of one query row to a 32-column chunk of raw scores (columns at or beyond
-// `sk` are left alone: the caller masks them through its visible-column limit).
-__device__ __forceinline__ void add_mask_chunk(uint32_t (&sv)[32], const AttnParams& p, long long row_off, int k0) {
-  if (p.mask_fp32) {
-    const float* mrow = reinterpret_cast<const float*>(p.mask) + row_off + k0;
-#pragma unroll
-    for (int i = 0; i < 32; ++i)
-      if (k0 + i < p.Sk) sv[i] = __float_as_uint(fmaf(__ldg(mrow + i), p.inv_scale, __uint_as_float(sv[i])));
-  } else {
-    const __nv_bfloat16* mrow = reinterpret_cast<const __nv_bfloat16*>(p.mask) + row_off + k0;
-#pragma unroll
-    for (int i = 0; i < 32; ++i)
-      if (k0 + i < p.Sk)
-        sv[i] = __float_as_uint(fmaf(__bfloat162float(mrow[i]), p.inv_scale, __uint_as_float(sv[i])));
-  }
-}
-
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -70,42 +52,30 @@ __device__ __forceinline__ void tma_load_rows(void* dst, const CUtensorMap* m, u
   tma_load_4d(dst, m, bar, c[0], c[1], c[2], c[3]);
 }
 
-// Per-head-dim configuration. D = 64 (the SD / SDXL / SD3 case) is limited by the exponential (MUFU) rate, not by the
-// tensor cores, so it runs TWO CTAs per SM (single S buffer, 2-deep K/V ring, 256 TMEM columns): while one CTA's
-// softmax warps exponentiate, the other CTA's MMAs use the tensor cores. D >= 128 keeps one CTA per SM with a
-// double-buffered S so QK^T(j+1) overlaps softmax(j) inside the CTA.
-// BN = keys per K/V block. D = 64 with BN = 64 needs only 64 (S) + 64 (O) TMEM columns and 64 KB of shared memory, so
-// three CTAs could share an SM; measured slower than BN = 128 with two CTAs (see g_attn_bn64), so it is not the default.
-template <int D, int BN, bool PTM = false>
-struct AttnCfg {
-  static constexpr int SB = (D == 64) ? 1 : 2;                      // S accumulator buffers in TMEM
-  static constexpr int KS = (D == 192) ? 1 : 2;                     // K/V ring depth
-  // Optional variant: P (bf16, two keys per 32-bit column) stays in TMEM and feeds the PV MMA as its A operand (no
-  // shared-memory round trip, half of exp(j) runs before PV(j-1) completes, 118 registers); S is then read from TMEM
-  // twice and released later, which costs more than it saves on long sequences. Parity-tested, not the default.
-  // (b200mix_debug_attn_ptmem; measured with tools/attn_probe.py: 659 vs 680 TFLOP/s at S = 4096, 531 vs 524 at S = 1024)
-  static constexpr bool P_TMEM = PTM && (BN == 128);
-  // SB*BN (S) + BN/2 (P, if in TMEM) + D (O) <= 256 / 512 columns
-  static constexpr int TMEM_COLS = (D == 64) ? (BN == 64 ? 128 : 256) : 512;
-  static constexpr int MIN_CTAS = (D == 64) ? (BN == 64 ? 3 : 2) : 1;
-  // dynamic smem is declared __align__(1024) (128B-swizzle atoms), so no alignment slack
-  static constexpr int SMEM = 128 * D * 2 + 2 * KS * BN * D * 2 + (P_TMEM ? 0 : 128 * BN * 2) + 256;
-};
+__device__ __forceinline__ float mask_value(const AttnParams& p, long long row_off, int k) {
+  return p.mask_fp32 ? __ldg(reinterpret_cast<const float*>(p.mask) + row_off + k)
+                     : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.mask)[row_off + k]);
+}
 
-template <int D, int BN, bool PTM>
-__global__ void __launch_bounds__(192, AttnCfg<D, BN, PTM>::MIN_CTAS)
+// BN = keys per K/V block; KS = K/V ring depth. The register budget of a consumer thread (S: BN / 2, O: D / 2, P: BN / 4
+// fp32 / bf16x2 registers) sets BN: 128 keys for D = 64, 64 keys for D = 128 and 192.
+template <int D, int BN>
+struct AttnCfg {
+  static constexpr int KS = 2;
+  // dynamic smem is declared __align__(1024) (128B-swizzle atoms), so no alignment slack
+  static constexpr int SMEM = 128 * D * 2 + 2 * KS * BN * D * 2 + 256;
+};
+constexpr int ATTN_THREADS = 288;
+
+template <int D, int BN>
+__global__ void __launch_bounds__(ATTN_THREADS, 1)
     attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ AttnParams p) {
   constexpr int DC = D / 64;               // 64-wide head-dim chunks (one 128B swizzle atom each)
   constexpr int TILE_BYTES = 128 * D * 2;  // the 128-row Q tile
   constexpr int KV_BYTES = BN * D * 2;     // one BN-row tile of K / V
   constexpr int KV_PANEL = BN * 128;       // one 64-wide head-dim panel of it
-  constexpr int KS = AttnCfg<D, BN, PTM>::KS;
-  constexpr int SB = AttnCfg<D, BN, PTM>::SB;
-  constexpr bool PT = AttnCfg<D, BN, PTM>::P_TMEM;
-  constexpr int P_BYTES = PT ? 0 : 128 * BN * 2;
-  constexpr uint32_t TM_S = 0, TM_P = SB * BN, TM_O = TM_P + (PT ? BN / 2 : 0);
-  static_assert(TM_O + D <= AttnCfg<D, BN, PTM>::TMEM_COLS, "TMEM budget");
+  constexpr int KS = AttnCfg<D, BN>::KS;
 
   // cu_seqlens / kv_lens are read right away: if they are given, wait for the previous kernel first
   if (p.cu || p.kv_lens) pdl_wait();
@@ -150,1142 +120,178 @@ __global__ void __launch_bounds__(192, AttnCfg<D, BN, PTM>::MIN_CTAS)
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + TILE_BYTES;
   uint8_t* sV = sK + KS * KV_BYTES;
-  uint8_t* sP = sV + KS * KV_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + P_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + KS * KV_BYTES);
   uint64_t* q_full = bars;            // 1
   uint64_t* k_full = bars + 1;        // KS
   uint64_t* k_empty = k_full + KS;    // KS
   uint64_t* v_full = k_empty + KS;    // KS
   uint64_t* v_empty = v_full + KS;    // KS
-  uint64_t* s_full = v_empty + KS;    // 2
-  uint64_t* p_full = s_full + 2;      // 1
-  uint64_t* pv_done = p_full + 1;     // 1
-  uint64_t* s_empty = pv_done + 1;    // 1 (used when SB == 1: softmax has drained S into registers)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(s_empty + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
     for (int s = 0; s < KS; ++s) {
       mbar_init(&k_full[s], 1);
-      mbar_init(&k_empty[s], 1);
+      mbar_init(&k_empty[s], 8);  // every consumer warp
       mbar_init(&v_full[s], 1);
-      mbar_init(&v_empty[s], 1);
-    }
-    mbar_init(&s_full[0], 1);
-    mbar_init(&s_full[1], 1);
-    mbar_init(p_full, 128);
-    mbar_init(pv_done, 1);
-    mbar_init(s_empty, 128);
-    fence_barrier_init();
-    prefetch_tmap(&tmQ);
-    prefetch_tmap(&tmK);
-    prefetch_tmap(&tmV);
-  }
-  if (warp == 4) tmem_alloc<AttnCfg<D, BN, PTM>::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();
-  pdl_launch_dependents();
-
-  // The two single-thread roles run their loops with the whole (converged) warp and issue under elect_one_sync():
-  // see ptx.cuh (an `if (lane == 0)` region makes the compiler wrap every TMA / MMA instruction in an election loop).
-  if (warp == 5) {
-    {
-      // ===== TMA producer =====
-      if (elect_one_sync()) {
-        mbar_expect_tx(q_full, TILE_BYTES);
-#pragma unroll
-        for (int dc = 0; dc < DC; ++dc) tma_load_rows(sQ + dc * 16384, &tmQ, q_full, p.q_pos, dc * 64, q_begin, h, b);
-      }
-      __syncwarp();
-      int st = 0;
-      uint32_t ph = 0;
-      for (int j = 0; j < n_tiles; ++j) {
-        const int row0 = kv_begin + j * BN;
-        mbar_wait(&k_empty[st], ph ^ 1);
-        if (elect_one_sync()) {
-          mbar_expect_tx(&k_full[st], KV_BYTES);
-#pragma unroll
-          for (int dc = 0; dc < DC; ++dc)
-            tma_load_rows(sK + st * KV_BYTES + dc * KV_PANEL, &tmK, &k_full[st], p.k_pos, dc * 64, row0, hk, b);
-        }
-        __syncwarp();
-        mbar_wait(&v_empty[st], ph ^ 1);
-        if (elect_one_sync()) {
-          mbar_expect_tx(&v_full[st], KV_BYTES);
-#pragma unroll
-          for (int dc = 0; dc < DC; ++dc)
-            tma_load_rows(sV + st * KV_BYTES + dc * KV_PANEL, &tmV, &v_full[st], p.v_pos, dc * 64, row0, hk, b);
-        }
-        __syncwarp();
-        if (++st == KS) st = 0, ph ^= 1;
-      }
-    }
-  } else if (warp == 4) {
-    {
-      // ===== MMA issuer =====
-      constexpr uint32_t idesc_qk = make_idesc_bf16(128, BN, 0, 0);
-      constexpr uint32_t idesc_pv = make_idesc_bf16(128, D, 0, 1);  // B (= V) is MN-major
-      const uint32_t q_addr = smem_u32(sQ), p_addr = smem_u32(sP);
-      auto issue_qk = [&](int j, int st) {
-        const uint32_t k_addr = smem_u32(sK + st * KV_BYTES);
-        const uint32_t d_tmem = tmem_base + TM_S + (j % SB) * BN;
-#pragma unroll
-        for (int k = 0; k < D / 16; ++k) {
-          const uint32_t q_off = (k >> 2) * 16384 + (k & 3) * 32;
-          const uint32_t k_off = (k >> 2) * KV_PANEL + (k & 3) * 32;
-          umma_bf16_ss(d_tmem, make_smem_desc_sw128(q_addr + q_off, 16, 1024),
-                       make_smem_desc_sw128(k_addr + k_off, 16, 1024), idesc_qk, k != 0 ? 1u : 0u);
-        }
-      };
-      mbar_wait(q_full, 0);
-      int kst = 0;
-      uint32_t kph = 0;  // K ring position of the NEXT QK^T to issue
-      int vst = 0;
-      uint32_t vph = 0;  // V ring position of the next PV
-      if (n_tiles > 0) {  // no visible key (kv_lens[b] == 0): the producer loads no K, nothing to multiply
-        mbar_wait(&k_full[0], 0);
-        tc_fence_after();
-        if (elect_one_sync()) {
-          issue_qk(0, 0);
-          umma_commit(&k_empty[0]);
-          umma_commit(&s_full[0]);
-        }
-        __syncwarp();
-        if (++kst == KS) kst = 0, kph ^= 1;
-      }
-      for (int j = 0; j < n_tiles; ++j) {
-        if (j + 1 < n_tiles) {
-          mbar_wait(&k_full[kst], kph);
-          if (SB == 1) mbar_wait(s_empty, j & 1);  // softmax(j) has copied S out of TMEM
-          tc_fence_after();
-          if (elect_one_sync()) {
-            issue_qk(j + 1, kst);
-            umma_commit(&k_empty[kst]);
-            umma_commit(&s_full[(j + 1) % SB]);
-          }
-          __syncwarp();
-          if (++kst == KS) kst = 0, kph ^= 1;
-        }
-        mbar_wait(p_full, j & 1);
-        mbar_wait(&v_full[vst], vph);
-        tc_fence_after();
-        const uint32_t v_addr = smem_u32(sV + vst * KV_BYTES);
-        if (elect_one_sync()) {
-#pragma unroll
-          for (int k = 0; k < BN / 16; ++k) {
-            const uint64_t bd = make_smem_desc_sw128(v_addr + k * 2048, KV_PANEL, 1024);
-            if (PT) {
-              umma_bf16_ts(tmem_base + TM_O, tmem_base + TM_P + k * 8, bd, idesc_pv, (j | k) != 0 ? 1u : 0u);
-            } else {
-              const uint64_t ad = make_smem_desc_sw128(p_addr + (k >> 2) * 16384 + (k & 3) * 32, 16, 1024);
-              umma_bf16_ss(tmem_base + TM_O, ad, bd, idesc_pv, (j | k) != 0 ? 1u : 0u);
-            }
-          }
-          umma_commit(&v_empty[vst]);
-          umma_commit(pv_done);
-        }
-        __syncwarp();
-        if (++vst == KS) vst = 0, vph ^= 1;
-      }
-    }
-  } else {
-    // ===== softmax warps: one query row per thread =====
-    const int qd = warp & 3;
-    const int row = qd * 32 + lane;
-    const uint32_t lane_base = tmem_base + (static_cast<uint32_t>(qd * 32) << 16);
-    const int row_limit_base = p.causal ? (q_rel0 + row + causal_off + 1) : kv_len;
-    float m = -INFINITY, l = 0.0f;
-    uint8_t* p_row = sP + row * 128;
-    const int sw = row & 7;
-    // additive mask row of this query (rows past the end of the sequence read row Sq - 1: in bounds, never stored)
-    const long long mask_row = static_cast<long long>(b) * p.m_sb + static_cast<long long>(h) * p.m_sh +
-                               static_cast<long long>(min(q_begin + row, p.Sq - 1)) * p.m_sq;
-
-    if constexpr (PT) {
-      // ---- P in TMEM: S is read from TMEM twice (row max, then exponentials) in 32-column chunks, the next chunk's
-      // load in flight while the current one is processed, so a thread holds 64 S values instead of 128 and the
-      // compiler has registers left to overlap the FFMA -> ex2 -> FADD chains. The packed P words go back to TMEM.
-      for (int j = 0; j < n_tiles; ++j) {
-        mbar_wait(&s_full[j % SB], (j / SB) & 1);
-        tc_fence_after();
-        const uint32_t s_addr = lane_base + TM_S + (j % SB) * BN;
-        const int limit = min(kv_len, row_limit_base) - j * BN;  // columns [0, limit) of this tile are visible
-        const bool full = limit >= BN;
-        uint32_t ch[2][32];
-        tmem_ld_32x32b_x32(s_addr, ch[0]);
-        tmem_wait_ld();
-        float mx = -INFINITY;
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          // next chunk (or chunk 0 again for the second pass) is fetched while this one is reduced
-          tmem_ld_32x32b_x32(s_addr + ((c + 1) & 3) * 32, ch[(c + 1) & 1]);
-          if (full) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) mx = fmaxf(mx, __uint_as_float(ch[c & 1][i]));
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (c * 32 + i < limit) mx = fmaxf(mx, __uint_as_float(ch[c & 1][i]));
-          }
-          tmem_wait_ld();
-        }
-        const float m_cand = fmaxf(m, mx);
-        const bool grow = (m_cand - m) * p.scale_log2 > 8.0f;  // also true for the first finite tile (m = -inf)
-        float alpha = 1.0f;
-        if (grow) {
-          alpha = fast_exp2((m - m_cand) * p.scale_log2);
-          m = m_cand;
-          l *= alpha;
-        }
-        const float m_scaled = (m == -INFINITY) ? 0.0f : m * p.scale_log2;
-        float sum = 0.0f;
-        uint32_t pk[32];
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          if (c < 3) tmem_ld_32x32b_x32(s_addr + (c + 1) * 32, ch[(c + 1) & 1]);
-#pragma unroll
-          for (int t = 0; t < 16; ++t) {
-            float s0 = __uint_as_float(ch[c & 1][2 * t]), s1 = __uint_as_float(ch[c & 1][2 * t + 1]);
-            if (!full) {
-              s0 = (c * 32 + 2 * t < limit) ? s0 : -INFINITY;
-              s1 = (c * 32 + 2 * t + 1 < limit) ? s1 : -INFINITY;
-            }
-            const float e0 = fast_exp2(fmaf(s0, p.scale_log2, -m_scaled));
-            const float e1 = fast_exp2(fmaf(s1, p.scale_log2, -m_scaled));
-            sum += e0 + e1;
-            pk[16 * (c & 1) + t] = pack_bf16x2(e0, e1);
-          }
-          if (c < 3) tmem_wait_ld();
-          if (c == 2 && SB == 1) {  // the last S chunk is in registers: QK^T of the next block may overwrite S
-            tc_fence_before();
-            mbar_arrive(s_empty);
-          }
-          if (c == 1 || c == 3) {
-            if (c == 1 && j > 0) {
-              // O and the P columns are free once PV_{j-1} has completed; the lazy rescale of O happens here too, i.e.
-              // AFTER half of this block's exponentials: they overlap the previous block's second MMA
-              mbar_wait(pv_done, (j - 1) & 1);
-              tc_fence_after();
-              if (__any_sync(0xffffffffu, grow)) {
-#pragma unroll 1
-                for (int oc = 0; oc < D / 32; ++oc) {
-                  uint32_t o[32];
-                  tmem_ld_32x32b_x32(lane_base + TM_O + oc * 32, o);
-                  tmem_wait_ld();
-#pragma unroll
-                  for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-                  tmem_st_32x32b_x32(lane_base + TM_O + oc * 32, o);
-                }
-              }
-            }
-            tmem_st_32x32b_x32(lane_base + TM_P + (c >> 1) * 32, pk);
-          }
-        }
-        l += sum;
-        tmem_wait_st();
-        tc_fence_before();
-        mbar_arrive(p_full);
-      }
-    } else {
-    for (int j = 0; j < n_tiles; ++j) {
-      mbar_wait(&s_full[j % SB], (j / SB) & 1);
-      tc_fence_after();
-      uint32_t sv[BN / 32][32];
-#pragma unroll
-      for (int c = 0; c < BN / 32; ++c) tmem_ld_32x32b_x32(lane_base + TM_S + (j % SB) * BN + c * 32, sv[c]);
-      tmem_wait_ld();
-      if (SB == 1) {
-        tc_fence_before();
-        mbar_arrive(s_empty);
-      }
-      if (p.mask) {
-#pragma unroll
-        for (int c = 0; c < BN / 32; ++c) add_mask_chunk(sv[c], p, mask_row, kv_begin + j * BN + c * 32);
-      }
-
-      const int limit = min(kv_len, row_limit_base) - j * BN;  // columns [0, limit) of this tile are visible
-      float mx = -INFINITY;
-      if (limit >= BN) {
-#pragma unroll
-        for (int c = 0; c < BN / 32; ++c)
-#pragma unroll
-          for (int i = 0; i < 32; ++i) mx = fmaxf(mx, __uint_as_float(sv[c][i]));
-      } else {
-#pragma unroll
-        for (int c = 0; c < BN / 32; ++c)
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            float s = (c * 32 + i < limit) ? __uint_as_float(sv[c][i]) : -INFINITY;
-            sv[c][i] = __float_as_uint(s);
-            mx = fmaxf(mx, s);
-          }
-      }
-      const float m_cand = fmaxf(m, mx);
-      const bool grow = (m_cand - m) * p.scale_log2 > 8.0f;  // also true for the first finite tile (m = -inf)
-      float alpha = 1.0f;
-      if (grow) {
-        alpha = fast_exp2((m - m_cand) * p.scale_log2);
-        m = m_cand;
-        l *= alpha;
-      }
-      const float m_scaled = (m == -INFINITY) ? 0.0f : m * p.scale_log2;
-
-      if (j > 0) {
-        // O (and the single P buffer) are free once PV_{j-1} has completed
-        mbar_wait(pv_done, (j - 1) & 1);
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, grow)) {
-#pragma unroll 1
-          for (int c = 0; c < D / 32; ++c) {
-            uint32_t o[32];
-            tmem_ld_32x32b_x32(lane_base + TM_O + c * 32, o);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st_32x32b_x32(lane_base + TM_O + c * 32, o);
-          }
-          tmem_wait_st();
-        }
-      }
-      float sum = 0.0f;
-      // exponentiate (row sum in fp32), pack P to bf16 and stream it into the K-major SW128 layout the second MMA
-      // expects (16-byte unit u of row r lives at u ^ (r & 7)); 8 columns at a time keeps the register footprint low
-#pragma unroll
-      for (int g8 = 0; g8 < BN / 8; ++g8) {
-        uint32_t w[4];
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          const int col = g8 * 8 + t * 2;
-          const float e0 = fast_exp2(fmaf(__uint_as_float(sv[col >> 5][col & 31]), p.scale_log2, -m_scaled));
-          const float e1 = fast_exp2(fmaf(__uint_as_float(sv[col >> 5][(col & 31) + 1]), p.scale_log2, -m_scaled));
-          sum += e0 + e1;
-          w[t] = pack_bf16x2(e0, e1);
-        }
-        const int chunk = g8 >> 3, u = g8 & 7;
-        *reinterpret_cast<uint4*>(p_row + chunk * 16384 + ((u ^ sw) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
-      }
-      l += sum;
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(p_full);
-    }
-    }
-
-    // ---- epilogue: O / l -> global (a row without any visible key gets zeros: O was never written) ----
-    if (n_tiles > 0) {
-      mbar_wait(pv_done, (n_tiles - 1) & 1);
-      tc_fence_after();
-    }
-    const float inv_l = (l > 0.0f) ? 1.0f / l : 0.0f;
-    const int q_abs = q_begin + row;
-    const bool valid = q_abs < q_end;
-    __nv_bfloat16* dst = p.o + static_cast<long long>(b) * p.o_sb + static_cast<long long>(q_abs) * p.o_ss +
-                         static_cast<long long>(h) * p.o_sh;
-#pragma unroll 1
-    for (int c = 0; c < D / 32; ++c) {
-      uint32_t o[32];
-      if (n_tiles > 0) {
-        tmem_ld_32x32b_x32(lane_base + TM_O + c * 32, o);
-        tmem_wait_ld();
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o[i] = 0u;
-      }
-      if (valid) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          uint4 w;
-          w.x = pack_bf16x2(__uint_as_float(o[8 * i + 0]) * inv_l, __uint_as_float(o[8 * i + 1]) * inv_l);
-          w.y = pack_bf16x2(__uint_as_float(o[8 * i + 2]) * inv_l, __uint_as_float(o[8 * i + 3]) * inv_l);
-          w.z = pack_bf16x2(__uint_as_float(o[8 * i + 4]) * inv_l, __uint_as_float(o[8 * i + 5]) * inv_l);
-          w.w = pack_bf16x2(__uint_as_float(o[8 * i + 6]) * inv_l, __uint_as_float(o[8 * i + 7]) * inv_l);
-          reinterpret_cast<uint4*>(dst + c * 32)[i] = w;
-        }
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc<AttnCfg<D, BN, PTM>::TMEM_COLS>(tmem_base);
-  }
-}
-
-
-// ------------------------------------------------------------------------------------------------------------
-// Short-KV attention (cross-attention against <= 128 keys, e.g. the 77 text tokens of SD / SDXL): one K/V block, so a
-// query tile is a single QK^T -> softmax -> PV chain of ~2 us whose cost is all latency. Instead of one CTA per tile
-// (barrier / TMEM / K,V set-up paid 1280 times, Q load latency exposed every time) the grid is persistent: each CTA owns
-// a contiguous range of the flattened (batch, head, q-tile) space, keeps K / V of the current (batch, head) in shared
-// memory, prefetches the next Q tile through a 2-deep ring while the current one is in softmax, skips the key chunks
-// beyond kv_len, and writes O through the (idle) P buffer so global stores are full 128-byte lines.
-// ------------------------------------------------------------------------------------------------------------
-constexpr int SKV_SMEM = 2 * 16384 /*Q ring*/ + 16384 /*K*/ + 16384 /*V*/ + 32768 /*P, O staging*/ + 256;
-
-__global__ void __launch_bounds__(192, 2)
-    attn_shortkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                        const __grid_constant__ CUtensorMap tmV, const __grid_constant__ AttnParams p, int nq,
-                        int total_tiles) {
-  constexpr int D = 64;
-  constexpr int TILE_BYTES = 128 * D * 2;
-  constexpr uint32_t TM_S = 0, TM_O = 128;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* sQ = smem;                   // 2 x 16 KB
-  uint8_t* sK = sQ + 2 * TILE_BYTES;
-  uint8_t* sV = sK + TILE_BYTES;
-  uint8_t* sP = sV + TILE_BYTES;        // 32 KB: P (bf16 128x128, two 64-column SW128 panels), then O staging
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 32768);
-  uint64_t* q_full = bars;        // 2
-  uint64_t* q_empty = bars + 2;   // 2
-  uint64_t* kv_full = bars + 4;
-  uint64_t* kv_empty = bars + 5;
-  uint64_t* s_full = bars + 6;
-  uint64_t* s_empty = bars + 7;   // 128
-  uint64_t* p_full = bars + 8;    // 128
-  uint64_t* pv_done = bars + 9;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 10);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    mbar_init(&q_full[0], 1), mbar_init(&q_full[1], 1);
-    mbar_init(&q_empty[0], 1), mbar_init(&q_empty[1], 1);
-    mbar_init(kv_full, 1), mbar_init(kv_empty, 1);
-    mbar_init(s_full, 1), mbar_init(s_empty, 128);
-    mbar_init(p_full, 128), mbar_init(pv_done, 1);
-    fence_barrier_init();
-    prefetch_tmap(&tmQ);
-    prefetch_tmap(&tmK);
-    prefetch_tmap(&tmV);
-  }
-  if (warp == 4) tmem_alloc<256>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();
-  pdl_launch_dependents();
-
-  // my contiguous slice of the flattened (batch, head, q-tile) space
-  const int f0 = static_cast<int>(static_cast<long long>(blockIdx.x) * total_tiles / gridDim.x);
-  const int f1 = static_cast<int>(static_cast<long long>(blockIdx.x + 1) * total_tiles / gridDim.x);
-  const int rep = p.Hq / p.Hkv;
-
-  if (warp == 5) {
-    {
-      // ===== TMA producer (converged warp, elected lane issues) =====
-      int g_prev = -1, kvn = 0;
-      for (int f = f0, i = 0; f < f1; ++f, ++i) {
-        const int grp = f / nq, qt = f - grp * nq;
-        const int b = grp / p.Hq, h = grp - b * p.Hq;
-        if (grp != g_prev) {
-          if (kvn > 0) mbar_wait(kv_empty, (kvn - 1) & 1);  // every MMA on the previous K / V has completed
-          if (elect_one_sync()) {
-            mbar_expect_tx(kv_full, 2 * TILE_BYTES);
-            tma_load_rows(sK, &tmK, kv_full, p.k_pos, 0, 0, h / rep, b);  // rows >= Sk are zero-filled
-            tma_load_rows(sV, &tmV, kv_full, p.v_pos, 0, 0, h / rep, b);
-          }
-          __syncwarp();
-          ++kvn;
-          g_prev = grp;
-        }
-        const int s = i & 1;
-        mbar_wait(&q_empty[s], ((i >> 1) & 1) ^ 1);
-        if (elect_one_sync()) {
-          mbar_expect_tx(&q_full[s], TILE_BYTES);
-          tma_load_rows(sQ + s * TILE_BYTES, &tmQ, &q_full[s], p.q_pos, 0, qt * 128, h, b);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp == 4) {
-    {
-      // ===== MMA issuer (converged warp, elected lane issues) =====
-      constexpr uint32_t idesc_qk = make_idesc_bf16(128, 128, 0, 0);
-      constexpr uint32_t idesc_pv = make_idesc_bf16(128, D, 0, 1);  // B (= V) is MN-major
-      const uint32_t k_addr = smem_u32(sK), v_addr = smem_u32(sV), p_addr = smem_u32(sP);
-      int g_prev = -1, kvn = 0;
-      for (int f = f0, i = 0; f < f1; ++f, ++i) {
-        const int grp = f / nq;
-        const int b = grp / p.Hq;
-        if (grp != g_prev) {
-          mbar_wait(kv_full, kvn & 1);
-          ++kvn;
-          g_prev = grp;
-        }
-        const int kv_len = p.kv_lens ? min(p.Sk, p.kv_lens[b]) : p.Sk;
-        const int s = i & 1;
-        mbar_wait(&q_full[s], (i >> 1) & 1);
-        if (i > 0) mbar_wait(s_empty, (i - 1) & 1);  // softmax(i-1) has copied S out of TMEM
-        tc_fence_after();
-        const uint32_t q_addr = smem_u32(sQ + s * TILE_BYTES);
-        if (elect_one_sync()) {
-#pragma unroll
-          for (int k = 0; k < D / 16; ++k)
-            umma_bf16_ss(tmem_base + TM_S, make_smem_desc_sw128(q_addr + k * 32, 16, 1024),
-                         make_smem_desc_sw128(k_addr + k * 32, 16, 1024), idesc_qk, k != 0 ? 1u : 0u);
-          umma_commit(&q_empty[s]);
-          umma_commit(s_full);
-        }
-        __syncwarp();
-        mbar_wait(p_full, i & 1);  // P(i) is in smem; the same threads finished reading O(i-1) before writing it
-        tc_fence_after();
-        const int ksteps = (kv_len + 15) >> 4;  // P columns beyond kv_len are never read
-        if (elect_one_sync()) {
-          for (int k = 0; k < ksteps; ++k) {
-            const uint64_t ad = make_smem_desc_sw128(p_addr + (k >> 2) * 16384 + (k & 3) * 32, 16, 1024);
-            const uint64_t bd = make_smem_desc_sw128(v_addr + k * 2048, 16384, 1024);
-            umma_bf16_ss(tmem_base + TM_O, ad, bd, idesc_pv, k != 0 ? 1u : 0u);
-          }
-          umma_commit(pv_done);
-          if (f + 1 == f1 || (f + 1) / nq != grp) umma_commit(kv_empty);  // last use of this K / V
-        }
-        __syncwarp();
-      }
-    }
-  } else {
-    // ===== softmax + output: one query row per thread =====
-    const int qd = warp & 3;
-    const int row = qd * 32 + lane;
-    const uint32_t lane_base = tmem_base + (static_cast<uint32_t>(qd * 32) << 16);
-    uint8_t* p_row = sP + row * 128;
-    const int sw = row & 7;
-    uint8_t* o_stage = sP + qd * 4096;  // this warp's 32 rows x 128 B of O (P is dead once PV has completed)
-    for (int f = f0, i = 0; f < f1; ++f, ++i) {
-      const int grp = f / nq, qt = f - grp * nq;
-      const int b = grp / p.Hq, h = grp - b * p.Hq;
-      const int kv_len = p.kv_lens ? min(p.Sk, p.kv_lens[b]) : p.Sk;
-      const int nch = (kv_len + 31) >> 5;  // 32-column chunks of S that hold visible keys (1..4)
-      mbar_wait(s_full, i & 1);
-      tc_fence_after();
-      uint32_t sv[4][32];
-#pragma unroll
-      for (int c = 0; c < 4; ++c)
-        if (c < nch) tmem_ld_32x32b_x32(lane_base + TM_S + c * 32, sv[c]);
-      tmem_wait_ld();
-      tc_fence_before();
-      mbar_arrive(s_empty);
-      if (p.mask) {
-        const long long mask_row = static_cast<long long>(b) * p.m_sb + static_cast<long long>(h) * p.m_sh +
-                                   static_cast<long long>(min(qt * 128 + row, p.Sq - 1)) * p.m_sq;
-#pragma unroll
-        for (int c = 0; c < 4; ++c)
-          if (c < nch) add_mask_chunk(sv[c], p, mask_row, c * 32);
-      }
-
-      // only the chunk that holds the boundary needs per-column masking; row max with 3-input max on four chains, the
-      // scale-subtract and the row sum on packed fp32 pairs (FFMA2 / FADD2): the kernel is issue-bound, not MUFU-bound
-      float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-      for (int c = 0; c < 4; ++c)
-        if (c < nch) {
-          if (kv_len < (c + 1) * 32) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (c * 32 + j >= kv_len) sv[c][j] = 0xff800000u;  // -inf
-          }
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-            mx4[j & 3] = fmax3(mx4[j & 3], __uint_as_float(sv[c][2 * j]), __uint_as_float(sv[c][2 * j + 1]));
-        }
-      const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-      const float m_scaled = (mx == -INFINITY) ? 0.0f : mx * p.scale_log2;
-      const uint64_t sc2 = pack_f32x2(p.scale_log2, p.scale_log2), nm2 = pack_f32x2(-m_scaled, -m_scaled);
-      uint64_t sum2[2] = {0ull, 0ull};
-#pragma unroll
-      for (int g8 = 0; g8 < 16; ++g8) {
-        if ((g8 >> 2) < nch) {
-          uint32_t w[4];
-#pragma unroll
-          for (int t = 0; t < 4; ++t) {
-            const int col = g8 * 8 + t * 2;
-            float t0, t1;
-            unpack_f32x2(ffma2(pack_f32x2(__uint_as_float(sv[col >> 5][col & 31]), __uint_as_float(sv[col >> 5][(col & 31) + 1])),
-                               sc2, nm2), t0, t1);
-            const float e0 = fast_exp2(t0), e1 = fast_exp2(t1);
-            sum2[t & 1] = fadd2(sum2[t & 1], pack_f32x2(e0, e1));
-            w[t] = pack_bf16x2(e0, e1);
-          }
-          const int chunk = g8 >> 3, u = g8 & 7;
-          *reinterpret_cast<uint4*>(p_row + chunk * 16384 + ((u ^ sw) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
-        }
-      }
-      float sa0, sa1, sb0, sb1;
-      unpack_f32x2(sum2[0], sa0, sa1);
-      unpack_f32x2(sum2[1], sb0, sb1);
-      const float sum = (sa0 + sa1) + (sb0 + sb1);
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(p_full);
-
-      // ---- O / l -> (staging in the P buffer) -> global, 4 rows x 128 B per store instruction ----
-      mbar_wait(pv_done, i & 1);
-      tc_fence_after();
-      const float inv_l = (sum > 0.0f) ? 1.0f / sum : 0.0f;
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t o[32];
-        tmem_ld_32x32b_x32(lane_base + TM_O + c * 32, o);
-        tmem_wait_ld();
-        if (!(sum > 0.0f)) {  // no visible key (kv_len == 0, or everything masked to -inf): O was never written
-#pragma unroll
-          for (int i = 0; i < 32; ++i) o[i] = 0u;
-        }
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          uint4 w;
-          w.x = pack_bf16x2(__uint_as_float(o[8 * u + 0]) * inv_l, __uint_as_float(o[8 * u + 1]) * inv_l);
-          w.y = pack_bf16x2(__uint_as_float(o[8 * u + 2]) * inv_l, __uint_as_float(o[8 * u + 3]) * inv_l);
-          w.z = pack_bf16x2(__uint_as_float(o[8 * u + 4]) * inv_l, __uint_as_float(o[8 * u + 5]) * inv_l);
-          w.w = pack_bf16x2(__uint_as_float(o[8 * u + 6]) * inv_l, __uint_as_float(o[8 * u + 7]) * inv_l);
-          *reinterpret_cast<uint4*>(o_stage + lane * 128 + (((c * 4 + u) ^ (lane & 7)) << 4)) = w;
-        }
-      }
-      __syncwarp();
-      __nv_bfloat16* dst0 = p.o + static_cast<long long>(b) * p.o_sb + static_cast<long long>(h) * p.o_sh;
-#pragma unroll
-      for (int it = 0; it < 8; ++it) {
-        const int r = it * 4 + (lane >> 3), u = lane & 7;  // 8 lanes cover one row's 128 bytes
-        const uint4 w = *reinterpret_cast<const uint4*>(o_stage + r * 128 + ((u ^ (r & 7)) << 4));
-        const int q_abs = qt * 128 + qd * 32 + r;
-        if (q_abs < p.Sq) *(reinterpret_cast<uint4*>(dst0 + static_cast<long long>(q_abs) * p.o_ss) + u) = w;
-      }
-      __syncwarp();  // the staging rows are rewritten by next tile's P stores of other rows only after p_full ordering
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc<256>(tmem_base);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------------------
-// Persistent ping-pong attention, D = 64, non-causal, fixed-length batches: the self-attention of SD / SDXL / SD3
-// (Sq, Sk in the thousands, 8..32 key blocks per query tile). One CTA per SM, 384 threads, looping over a contiguous range
-// of work items; a work item = TWO consecutive 128-row query tiles of one (batch, head):
-//   warp 9      TMA producer: Q of the next item (2-slot ring), K / V blocks through KS-deep rings. Each K / V block is
-//               loaded ONCE for both query tiles.   (warps 8-11 form the producer warpgroup; warps 10, 11 idle)
-//   warp 8      MMA issuer. The two single-thread roles sit at the HIGHEST warp indices on purpose: the warp scheduler
-//               of an SM sub-partition prefers the highest warp id among eligible warps (B300_MICROARCH.md, "multi-warp
-//               arbiter"), and with the issuer at warp 1 the always-eligible softmax warps above it starved it - measured
-//               with the ATTN_PROF build: the issuer spent 82 % of a key block getting 24 MMAs + 6 commits issued, and
-//               the softmax warps waited 500 cycles per block for S. Per key block s, in this fixed order:  S0(s+1) = Q0 K^T,  O0 += P0(s) V,
-//               S1(s+1) = Q1 K^T,  O1 += P1(s) V.  The block sequence runs across item boundaries (the first QK^T of
-//               the next item is issued while the current item's last blocks are still in softmax), so there is no
-//               per-tile prologue / epilogue bubble: a CTA pays barrier init, TMEM allocation and pipeline fill once.
-//   warps 0-3   softmax warpgroup of query tile 0, warps 4-7 of query tile 1: one query row per thread. While one
-//               warpgroup exponentiates (MUFU), the other drains S / takes its row max / writes its output, and the
-//               tensor cores run the other tile's MMAs.
-// P never touches shared memory: the bf16 probabilities are stored to TMEM (two keys per 32-bit column) and feed the
-// PV MMA as its A operand (tcgen05.mma with A in TMEM), which removes 64 KB of shared-memory writes + 64 KB of reads
-// per key block: with P in shared memory the two MMAs plus the P round trip need ~2000 clk of the 128 B/clk shared-memory
-// port per block pair, the same as the 2048 clk MUFU bound of the exponentials.
-// TMEM (512 columns): tile t owns [256 t, 256 t + 256): S fp32 (128) | P bf16x2 (64) | O fp32 (64).
-// Softmax inner loop uses the Blackwell packed-fp32 instructions (FFMA2 / FADD2) and the 3-input max (FMNMX3).
-// Rows past the end of the sequence (odd number of query tiles) are computed on zero-filled Q rows and not stored.
-// ------------------------------------------------------------------------------------------------------------
-// bf16 pair of two probabilities for the PV operand. cvt.rn.bf16x2.f32 (F2FP) issues on the same quarter-rate XU pipe
-// as the exponentials (tools/mufu_bench.py), so with ATTN_INT_PACK the pack runs on the integer pipe instead:
-// round-half-up (+0x8000 on the fp32 bits; the values are finite and non-negative) and one PRMT of the two high halves.
-#ifndef ATTN_INT_PACK
-#define ATTN_INT_PACK 0
-#endif
-__device__ __forceinline__ uint32_t pack_p_bf16x2(float lo, float hi) {
-#if ATTN_INT_PACK
-  uint32_t r;
-  asm("prmt.b32 %0, %1, %2, 0x7632;" : "=r"(r) : "r"(__float_as_uint(lo) + 0x8000u), "r"(__float_as_uint(hi) + 0x8000u));
-  return r;
-#else
-  return pack_bf16x2(lo, hi);
-#endif
-}
-
-// ATTN_PROF build (tools/attn_prof.py): cycles every role spends in each of its waits / phases, accumulated per CTA into
-// g_attn_prof[blockIdx.x][slot] (slots: see tools/attn_prof.py). Not compiled into the product library.
-#ifndef ATTN_PROF
-#define ATTN_PROF 0
-#endif
-#if ATTN_PROF
-__device__ unsigned long long g_attn_prof[148 * 32];
-#define PROF_DECL unsigned long long prof_t0 = 0, prof_acc[8] = {0, 0, 0, 0, 0, 0, 0, 0}
-#define PROF_BEGIN() prof_t0 = clock64()
-#define PROF_END(slot) prof_acc[slot] += clock64() - prof_t0
-#define PROF_FLUSH(base, n)                                                     \
-  for (int i_ = 0; i_ < (n); ++i_) g_attn_prof[blockIdx.x * 32 + (base) + i_] = prof_acc[i_]
-#else
-#define PROF_DECL
-#define PROF_BEGIN()
-#define PROF_END(slot)
-#define PROF_FLUSH(base, n)
-#endif
-
-// exp2 of two values on the FMA / ALU pipes (no MUFU): Cody-Waite split t = n + f with n = round(t), f in [-0.5, 0.5]
-// (magic-number add), 2^f by a degree-3 minimax polynomial (max relative error 7.5e-5, 50x below the bf16 rounding of P),
-// 2^n added into the exponent field. With ATTN_POLY_EVERY = N every N-th pair of a row takes this path, which moves
-// 1/N of the exponentials off the quarter-rate MUFU pipe that bounds the D = 64 kernel (packed FADD2 / FFMA2 keep the
-// extra issue slots at 4 per element). Inputs are clamped to >= -125 (masked scores are -inf).
-#ifndef ATTN_POLY_EVERY
-#define ATTN_POLY_EVERY 8  // measured (tools/attn_probe.py, S = 4096): 0 -> 808, 8 -> 830, 4 -> 804, 3 -> 770 TFLOP/s
-#endif
-#ifndef ATTN_EXP_TURNS
-#define ATTN_EXP_TURNS 0
-#endif
-#ifndef ATTN_QK_FIRST
-#define ATTN_QK_FIRST 0
-#endif
-__device__ __forceinline__ void poly_exp2_x2(uint64_t t2, float& e0, float& e1) {
-  float t0, t1;
-  unpack_f32x2(t2, t0, t1);
-  t2 = pack_f32x2(fmaxf(t0, -125.0f), fmaxf(t1, -125.0f));
-  const uint64_t magic = pack_f32x2(12582912.0f, 12582912.0f), nmagic = pack_f32x2(-12582912.0f, -12582912.0f);
-  const uint64_t r2 = fadd2(t2, magic);                                      // low mantissa bits = round(t)
-  const uint64_t f2 = ffma2(fadd2(r2, nmagic), pack_f32x2(-1.0f, -1.0f), t2);  // t - round(t)
-  uint64_t p2 = ffma2(pack_f32x2(0.05517162f, 0.05517162f), f2, pack_f32x2(0.24261113f, 0.24261113f));
-  p2 = ffma2(p2, f2, pack_f32x2(0.69326097f, 0.69326097f));
-  p2 = ffma2(p2, f2, pack_f32x2(0.99992806f, 0.99992806f));
-  float r0, r1, p0, p1;
-  unpack_f32x2(r2, r0, r1);
-  unpack_f32x2(p2, p0, p1);
-  e0 = t0 < -125.0f ? 0.0f : __uint_as_float(__float_as_uint(p0) + (__float_as_uint(r0) << 23));
-  e1 = t1 < -125.0f ? 0.0f : __uint_as_float(__float_as_uint(p1) + (__float_as_uint(r1) << 23));
-}
-
-template <int KS>
-struct AttnPPCfg {
-  static constexpr int TILE = 128 * 64 * 2;  // a 128-row x 64 bf16 tile: Q, K or V
-  static constexpr int SMEM = 4 * TILE /*Q: 2 slots x 2 tiles*/ + 2 * KS * TILE /*K and V rings*/ +
-                              2 * TILE /*O staging*/ + 512 /*barriers*/;
-};
-
-template <int KS>
-__global__ void __launch_bounds__(384, 1)
-    attn_pp_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                   const __grid_constant__ CUtensorMap tmV, const __grid_constant__ AttnParams p, int npairs,
-                   int total_items) {
-  constexpr int D = 64;
-  constexpr int TILE = AttnPPCfg<KS>::TILE;
-  constexpr uint32_t TM_TILE = 256, TM_S = 0, TM_P = 128, TM_O = 192;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* sQ = smem;                  // [slot][tile]
-  uint8_t* sK = sQ + 4 * TILE;         // [KS]
-  uint8_t* sV = sK + KS * TILE;        // [KS]
-  uint8_t* sO = sV + KS * TILE;        // [tile]: output staging for coalesced stores
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sO + 2 * TILE);
-  uint64_t* q_full = bars;             // 2
-  uint64_t* q_empty = bars + 2;        // 2
-  uint64_t* s_full = bars + 4;         // 2 (per tile)
-  uint64_t* s_empty = bars + 6;        // 2, 128 arrivals
-  uint64_t* p_full = bars + 8;         // 2, 128 arrivals
-  uint64_t* pv_done = bars + 10;       // 2
-  uint64_t* k_full = bars + 12;        // KS
-  uint64_t* k_empty = k_full + KS;
-  uint64_t* v_full = k_empty + KS;
-  uint64_t* v_empty = v_full + KS;
-  uint64_t* exp_turn = v_empty + KS;   // 2, 128 arrivals: whose turn it is to use the MUFU pipe (ATTN_EXP_TURNS)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(exp_turn + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&q_full[i], 1), mbar_init(&q_empty[i], 1);
-      mbar_init(&s_full[i], 1), mbar_init(&s_empty[i], 128);
-      mbar_init(&p_full[i], 128), mbar_init(&pv_done[i], 1);
-      mbar_init(&exp_turn[i], 128);
-    }
-    for (int i = 0; i < KS; ++i) {
-      mbar_init(&k_full[i], 1), mbar_init(&k_empty[i], 1);
-      mbar_init(&v_full[i], 1), mbar_init(&v_empty[i], 1);
+      mbar_init(&v_empty[s], 8);
     }
     fence_barrier_init();
     prefetch_tmap(&tmQ);
     prefetch_tmap(&tmK);
     prefetch_tmap(&tmV);
   }
-  if (warp == 8) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();
   pdl_launch_dependents();
 
-  // my contiguous slice of the flattened (batch, head, query-tile pair) space
-  const int f0 = static_cast<int>(static_cast<long long>(blockIdx.x) * total_items / gridDim.x);
-  const int f1 = static_cast<int>(static_cast<long long>(blockIdx.x + 1) * total_items / gridDim.x);
-  const int rep = p.Hq / p.Hkv;
-  // key blocks of batch element b (at least one: a batch element without visible keys runs one fully masked block)
-  auto blocks_of = [&](int b) -> int {
-    const int kv_len = p.kv_lens ? min(p.Sk, __ldg(p.kv_lens + b)) : p.Sk;
-    return max(1, (kv_len + 127) >> 7);
-  };
-
-  // register re-allocation between the warpgroups: the producer warpgroup keeps 72 registers per thread, each softmax
-  // thread gets 216 (its 128 scores + 32 packed probabilities + addresses stay in registers, no spills)
-  if (warp >= 8) {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 72;");
-  // Both single-thread roles run their loops with the whole converged warp (every lane polls the barriers and keeps
-  // the same ring state); only the issuing instructions sit under elect_one_sync() - see ptx.cuh.
-  if (warp == 9) {
-    {
-      // ===== TMA producer =====
-      int kst = 0, vst = 0;
-      uint32_t kph = 0, vph = 0;
-      for (int f = f0, n = 0; f < f1; ++f, ++n) {
-        const int grp = f / npairs, pr = f - grp * npairs;
-        const int b = grp / p.Hq, h = grp - b * p.Hq;
-        const int slot = n & 1;
-        mbar_wait(&q_empty[slot], ((n >> 1) & 1) ^ 1);
-        if (elect_one_sync()) {
-          mbar_expect_tx(&q_full[slot], 2 * TILE);
-          tma_load_rows(sQ + (slot * 2 + 0) * TILE, &tmQ, &q_full[slot], p.q_pos, 0, pr * 256, h, b);
-          tma_load_rows(sQ + (slot * 2 + 1) * TILE, &tmQ, &q_full[slot], p.q_pos, 0, pr * 256 + 128, h, b);
-        }
-        __syncwarp();
-        const int nb = blocks_of(b), hk = h / rep;
-        for (int j = 0; j < nb; ++j) {
-          mbar_wait(&k_empty[kst], kph ^ 1);
-          if (elect_one_sync()) {
-            mbar_expect_tx(&k_full[kst], TILE);
-            tma_load_rows(sK + kst * TILE, &tmK, &k_full[kst], p.k_pos, 0, j * 128, hk, b);
-          }
-          __syncwarp();
-          if (++kst == KS) kst = 0, kph ^= 1;
-          mbar_wait(&v_empty[vst], vph ^ 1);
-          if (elect_one_sync()) {
-            mbar_expect_tx(&v_full[vst], TILE);
-            tma_load_rows(sV + vst * TILE, &tmV, &v_full[vst], p.v_pos, 0, j * 128, hk, b);
-          }
-          __syncwarp();
-          if (++vst == KS) vst = 0, vph ^= 1;
-        }
-      }
-    }
-  } else if (warp == 8) {
-    if (f0 < f1) {
-      // ===== MMA issuer =====
-      constexpr uint32_t idesc_qk = make_idesc_bf16(128, 128, 0, 0);
-      constexpr uint32_t idesc_pv = make_idesc_bf16(128, D, 0, 1);  // B (= V) is MN-major
-      auto issue_qk = [&](int t, int slot, int st) {
-        const uint32_t q_addr = smem_u32(sQ + (slot * 2 + t) * TILE), k_addr = smem_u32(sK + st * TILE);
-#pragma unroll
-        for (int k = 0; k < D / 16; ++k)
-          umma_bf16_ss(tmem_base + t * TM_TILE + TM_S, make_smem_desc_sw128(q_addr + k * 32, 16, 1024),
-                       make_smem_desc_sw128(k_addr + k * 32, 16, 1024), idesc_qk, k != 0 ? 1u : 0u);
-      };
-      auto issue_pv = [&](int t, int st, bool acc) {
-        const uint32_t v_addr = smem_u32(sV + st * TILE);
-#pragma unroll
-        for (int k = 0; k < 8; ++k)
-          umma_bf16_ts(tmem_base + t * TM_TILE + TM_O, tmem_base + t * TM_TILE + TM_P + k * 8,
-                       make_smem_desc_sw128(v_addr + k * 2048, 16384, 1024), idesc_pv, (acc || k != 0) ? 1u : 0u);
-      };
-      int kst = 0, vst = 0;
-      uint32_t kph = 0, vph = 0;
-      uint32_t sidx = 0;  // key blocks issued so far (per tile): parity source of s_empty / p_full
-      const int nitems = f1 - f0;
-      PROF_DECL;
-      int nb = blocks_of((f0 / npairs) / p.Hq);
-      // pipeline fill: both QK^T of the very first block
-      mbar_wait(&q_full[0], 0);
-      mbar_wait(&k_full[0], 0);
-      tc_fence_after();
-      if (elect_one_sync()) {
-        issue_qk(0, 0, 0);
-        umma_commit(&s_full[0]);
-        issue_qk(1, 0, 0);
-        umma_commit(&s_full[1]);
-        umma_commit(&k_empty[0]);
-        if (nb == 1) umma_commit(&q_empty[0]);
-      }
-      __syncwarp();
-      if (++kst == KS) kst = 0, kph ^= 1;
-      for (int n = 0; n < nitems; ++n) {
-        const int nb_next = (n + 1 < nitems) ? blocks_of(((f0 + n + 1) / npairs) / p.Hq) : 0;
-        for (int j = 0; j < nb; ++j, ++sidx) {
-          const bool same = j + 1 < nb;
-          const bool has_next = same || (n + 1 < nitems);
-          const int n2 = same ? n : n + 1;
-          const bool last_qk_of_item = same ? (j + 2 == nb) : (nb_next == 1);
-          if (has_next) {
-            PROF_BEGIN();
-            if (!same) mbar_wait(&q_full[n2 & 1], (n2 >> 1) & 1);
-            mbar_wait(&k_full[kst], kph);
-            PROF_END(0);
-          }
-#if ATTN_QK_FIRST
-          // variant: both QK^T of the next block first, then both PV of this block
-          if (has_next) {
-#pragma unroll
-            for (int t = 0; t < 2; ++t) {
-              PROF_BEGIN();
-              mbar_wait(&s_empty[t], sidx & 1);  // softmax warpgroup t has S_t(s) in registers
-              PROF_END(1 + t);
-              tc_fence_after();
-              if (elect_one_sync()) {
-                issue_qk(t, n2 & 1, kst);
-                umma_commit(&s_full[t]);
-                if (t == 1) {
-                  umma_commit(&k_empty[kst]);
-                  if (last_qk_of_item) umma_commit(&q_empty[n2 & 1]);
-                }
-              }
-              __syncwarp();
-            }
-            if (++kst == KS) kst = 0, kph ^= 1;
-          }
-#pragma unroll
-          for (int t = 0; t < 2; ++t) {
-            PROF_BEGIN();
-            mbar_wait(&p_full[t], sidx & 1);  // P_t(s) is in TMEM (and the warpgroup is done with O_t)
-            PROF_END(3 + t);
-            PROF_BEGIN();
-            if (t == 0) mbar_wait(&v_full[vst], vph);
-            PROF_END(5);
-            tc_fence_after();
-            if (elect_one_sync()) {
-              issue_pv(t, vst, j != 0);
-              umma_commit(&pv_done[t]);
-              if (t == 1) umma_commit(&v_empty[vst]);
-            }
-            __syncwarp();
-          }
-          if (++vst == KS) vst = 0, vph ^= 1;
-#else
-          // Order per block: QK0(s+1) PV0(s) QK1(s+1) PV1(s). The in-order issuer thereby releases S1(s+1) only after
-          // warpgroup 0 has finished the exponentials of block s (and S0(s+2) after warpgroup 1's), which keeps the two
-          // warpgroups STAGGERED: one drains S / takes its row max while the other feeds the MUFU pipe. Issuing both
-          // QK^T first (ATTN_QK_FIRST) lets the warpgroups drift into phase - both exponentiate, then both leave the
-          // MUFU pipe idle - and costs 15 % (808 -> 684 TFLOP/s at S = 4096), as does a strict alternation of the
-          // exponential phases (ATTN_EXP_TURNS: one warp per sub-partition cannot saturate the MUFU pipe alone).
-#pragma unroll
-          for (int t = 0; t < 2; ++t) {
-            if (has_next) {
-              PROF_BEGIN();
-              mbar_wait(&s_empty[t], sidx & 1);  // softmax warpgroup t has S_t(s) in registers
-              PROF_END(1 + t);
-              tc_fence_after();
-              if (elect_one_sync()) {
-                issue_qk(t, n2 & 1, kst);
-                umma_commit(&s_full[t]);
-                if (t == 1) {
-                  umma_commit(&k_empty[kst]);
-                  if (last_qk_of_item) umma_commit(&q_empty[n2 & 1]);
-                }
-              }
-              __syncwarp();
-              if (t == 1) {
-                if (++kst == KS) kst = 0, kph ^= 1;
-              }
-            }
-            PROF_BEGIN();
-            mbar_wait(&p_full[t], sidx & 1);  // P_t(s) is in TMEM (and the warpgroup is done with O_t)
-            PROF_END(3 + t);
-            PROF_BEGIN();
-            if (t == 0) mbar_wait(&v_full[vst], vph);
-            PROF_END(5);
-            tc_fence_after();
-            if (elect_one_sync()) {
-              issue_pv(t, vst, j != 0);
-              umma_commit(&pv_done[t]);
-              if (t == 1) umma_commit(&v_empty[vst]);
-            }
-            __syncwarp();
-            if (t == 1) {
-              if (++vst == KS) vst = 0, vph ^= 1;
-            }
-          }
-#endif
-        }
-        nb = nb_next;
-      }
-#if ATTN_PROF
-      if (lane == 0) PROF_FLUSH(0, 6);
-#endif
-    }
-  }
-  } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 216;");
-    // ===== softmax warpgroups: one query row per thread =====
-    const int t = warp >> 2;
-    const int qd = warp & 3;
-    const int row = qd * 32 + lane;
-    const uint32_t lane_base = tmem_base + (static_cast<uint32_t>(qd * 32) << 16) + t * TM_TILE;
-    uint8_t* o_stage = sO + t * TILE + qd * 4096;  // this warp's 32 rows x 128 B
-    const uint64_t sc2 = pack_f32x2(p.scale_log2, p.scale_log2);
-    uint32_t sidx = 0;
-    PROF_DECL;
-#if ATTN_EXP_TURNS
-    if (t == 1) mbar_arrive(&exp_turn[0]);  // the first turn belongs to warpgroup 0
-#endif
-#if ATTN_PROF
-    const unsigned long long prof_start = clock64();
-#endif
-    for (int f = f0; f < f1; ++f) {
-      const int grp = f / npairs, pr = f - grp * npairs;
-      const int b = grp / p.Hq, h = grp - b * p.Hq;
-      const int kv_len = p.kv_lens ? min(p.Sk, __ldg(p.kv_lens + b)) : p.Sk;
-      const int nb = max(1, (kv_len + 127) >> 7);
-      const int q0 = pr * 256 + t * 128;
-      const long long mask_row = static_cast<long long>(b) * p.m_sb + static_cast<long long>(h) * p.m_sh +
-                                 static_cast<long long>(min(q0 + row, p.Sq - 1)) * p.m_sq;
-      float m = -INFINITY, l = 0.0f;
-      for (int j = 0; j < nb; ++j, ++sidx) {
-        PROF_BEGIN();
-        mbar_wait(&s_full[t], sidx & 1);
-        PROF_END(0);
-        tc_fence_after();
-        PROF_BEGIN();
-        uint32_t sv[4][32];
-#pragma unroll
-        for (int c = 0; c < 4; ++c) tmem_ld_32x32b_x32(lane_base + TM_S + c * 32, sv[c]);
-        tmem_wait_ld();
-        tc_fence_before();
-        mbar_arrive(&s_empty[t]);  // QK^T of the next block may overwrite S_t
-        PROF_END(1);
-        PROF_BEGIN();
-        if (p.mask) {
-#pragma unroll
-          for (int c = 0; c < 4; ++c) add_mask_chunk(sv[c], p, mask_row, j * 128 + c * 32);
-        }
-        const int limit = kv_len - j * 128;  // columns [0, limit) of this block are visible
-        if (limit < 128) {
-#pragma unroll
-          for (int c = 0; c < 4; ++c)
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (c * 32 + i >= limit) sv[c][i] = 0xff800000u;  // -inf
-        }
-        float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};  // four independent FMNMX3 chains
-#pragma unroll
-        for (int c = 0; c < 4; ++c)
-#pragma unroll
-          for (int i = 0; i < 16; ++i)
-            mx4[i & 3] = fmax3(mx4[i & 3], __uint_as_float(sv[c][2 * i]), __uint_as_float(sv[c][2 * i + 1]));
-        const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-        const float m_cand = fmaxf(m, mx);
-        const bool grow = (m_cand - m) * p.scale_log2 > 8.0f;  // also true for the first finite block (m = -inf)
-        float alpha = 1.0f;
-        if (grow) {
-          alpha = fast_exp2((m - m_cand) * p.scale_log2);
-          m = m_cand;
-          l *= alpha;
-        }
-        const float m_scaled = (m == -INFINITY) ? 0.0f : m * p.scale_log2;
-        PROF_END(2);
-        if (j > 0) {
-          // P_t and O_t are free once PV_t of the previous block has completed
-          PROF_BEGIN();
-          mbar_wait(&pv_done[t], (sidx - 1) & 1);
-          PROF_END(3);
-          tc_fence_after();
-          if (__any_sync(0xffffffffu, grow)) {  // lazy rescale: only when the running max grew by more than 2^8
-#pragma unroll 1
-            for (int c = 0; c < D / 32; ++c) {
-              uint32_t o[32];
-              tmem_ld_32x32b_x32(lane_base + TM_O + c * 32, o);
-              tmem_wait_ld();
-#pragma unroll
-              for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-              tmem_st_32x32b_x32(lane_base + TM_O + c * 32, o);
-            }
-          }
-        }
-        // exponentials: (s * scale_log2 - m_scaled) two at a time (FFMA2), ex2 on the MUFU pipe, packed row sum
-        // (FADD2), bf16 pairs straight back to TMEM as the A operand of the PV MMA
-#if ATTN_EXP_TURNS
-        // The two warpgroups take strict turns on the exponentials: one warp per sub-partition then has the MUFU pipe
-        // to itself (1024 cycles per block) while the other warpgroup drains S / takes its row max / waits for its MMAs.
-        // Left to themselves the warpgroups drift into phase (both exponentiate, then both idle the MUFU pipe).
-        mbar_wait(&exp_turn[t], sidx & 1);
-#endif
-        PROF_BEGIN();
-        const uint64_t nm2 = pack_f32x2(-m_scaled, -m_scaled);
-        uint64_t sum2[2] = {0ull, 0ull};
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          uint32_t* pk = sv[c & 2];  // chunks 0 / 2 are dead by the time their packed words overwrite them
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const uint64_t s2 = pack_f32x2(__uint_as_float(sv[c][2 * i]), __uint_as_float(sv[c][2 * i + 1]));
-            float e0, e1;
-            if (ATTN_POLY_EVERY > 0 && (i % (ATTN_POLY_EVERY > 0 ? ATTN_POLY_EVERY : 1)) == 0) {
-              poly_exp2_x2(ffma2(s2, sc2, nm2), e0, e1);
-            } else {
-              float t0, t1;
-              unpack_f32x2(ffma2(s2, sc2, nm2), t0, t1);
-              e0 = fast_exp2(t0), e1 = fast_exp2(t1);
-            }
-            sum2[i & 1] = fadd2(sum2[i & 1], pack_f32x2(e0, e1));
-            pk[(c & 1) * 16 + i] = pack_p_bf16x2(e0, e1);
-          }
-          if (c & 1) tmem_st_32x32b_x32(lane_base + TM_P + (c >> 1) * 32, sv[c & 2]);
-        }
-        float a0, a1, b0, b1;
-        unpack_f32x2(sum2[0], a0, a1);
-        unpack_f32x2(sum2[1], b0, b1);
-        l += (a0 + a1) + (b0 + b1);
-#if ATTN_EXP_TURNS
-        mbar_arrive(&exp_turn[t ^ 1]);
-#endif
-        tmem_wait_st();
-        tc_fence_before();
-        mbar_arrive(&p_full[t]);
-        PROF_END(4);
-      }
-
-      // ---- item epilogue: O / l -> staging (swizzled) -> global, 4 rows x 128 B per store instruction ----
-      PROF_BEGIN();
-      mbar_wait(&pv_done[t], (sidx - 1) & 1);
-      PROF_END(5);
-      PROF_BEGIN();
-      tc_fence_after();
-      const float inv_l = (l > 0.0f) ? 1.0f / l : 0.0f;
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t o[32];
-        tmem_ld_32x32b_x32(lane_base + TM_O + c * 32, o);
-        tmem_wait_ld();
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          uint4 w;
-          w.x = pack_bf16x2(__uint_as_float(o[8 * u + 0]) * inv_l, __uint_as_float(o[8 * u + 1]) * inv_l);
-          w.y = pack_bf16x2(__uint_as_float(o[8 * u + 2]) * inv_l, __uint_as_float(o[8 * u + 3]) * inv_l);
-          w.z = pack_bf16x2(__uint_as_float(o[8 * u + 4]) * inv_l, __uint_as_float(o[8 * u + 5]) * inv_l);
-          w.w = pack_bf16x2(__uint_as_float(o[8 * u + 6]) * inv_l, __uint_as_float(o[8 * u + 7]) * inv_l);
-          *reinterpret_cast<uint4*>(o_stage + lane * 128 + (((c * 4 + u) ^ (lane & 7)) << 4)) = w;
-        }
-      }
-      __syncwarp();
-      __nv_bfloat16* dst0 = p.o + static_cast<long long>(b) * p.o_sb + static_cast<long long>(h) * p.o_sh;
-#pragma unroll
-      for (int it = 0; it < 8; ++it) {
-        const int r = it * 4 + (lane >> 3), u = lane & 7;  // 8 lanes cover one row's 128 bytes
-        const uint4 w = *reinterpret_cast<const uint4*>(o_stage + r * 128 + ((u ^ (r & 7)) << 4));
-        const int q_abs = q0 + qd * 32 + r;
-        if (q_abs < p.Sq) *(reinterpret_cast<uint4*>(dst0 + static_cast<long long>(q_abs) * p.o_ss) + u) = w;
-      }
-      __syncwarp();
-      PROF_END(6);
-    }
-#if ATTN_PROF
-    prof_acc[7] = clock64() - prof_start;
-    if ((warp & 3) == 0 && lane == 0) PROF_FLUSH(8 + t * 8, 8);
-#endif
-  }
-
-  tc_fence_before();
-  __syncthreads();
   if (warp == 8) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
+    // ===== TMA producer (converged warp, one elected lane issues: see ptx.cuh) =====
+    if (elect_one_sync()) {
+      mbar_expect_tx(q_full, TILE_BYTES);
+#pragma unroll
+      for (int dc = 0; dc < DC; ++dc) tma_load_rows(sQ + dc * 16384, &tmQ, q_full, p.q_pos, dc * 64, q_begin, h, b);
+    }
+    __syncwarp();
+    int st = 0;
+    uint32_t ph = 0;
+    for (int j = 0; j < n_tiles; ++j) {
+      const int row0 = kv_begin + j * BN;
+      mbar_wait(&k_empty[st], ph ^ 1);
+      if (elect_one_sync()) {
+        mbar_expect_tx(&k_full[st], KV_BYTES);
+#pragma unroll
+        for (int dc = 0; dc < DC; ++dc)
+          tma_load_rows(sK + st * KV_BYTES + dc * KV_PANEL, &tmK, &k_full[st], p.k_pos, dc * 64, row0, hk, b);
+      }
+      __syncwarp();
+      mbar_wait(&v_empty[st], ph ^ 1);
+      if (elect_one_sync()) {
+        mbar_expect_tx(&v_full[st], KV_BYTES);
+#pragma unroll
+        for (int dc = 0; dc < DC; ++dc)
+          tma_load_rows(sV + st * KV_BYTES + dc * KV_PANEL, &tmV, &v_full[st], p.v_pos, dc * 64, row0, hk, b);
+      }
+      __syncwarp();
+      if (++st == KS) st = 0, ph ^= 1;
+    }
+    return;
+  }
+
+  // ===== consumers: accumulator fragment rows r0 = 16 w + lane / 4 and r0 + 8 of the warpgroup's 64 rows, columns
+  // 8 n + 2 (lane % 4) + {0, 1} of every 8-column block n =====
+  const int grp = warp >> 2, w = warp & 3;
+  const int lm = lane & 3;
+  const int rloc = 64 * grp + 16 * w + (lane >> 2);  // query row (in the tile) of fragment elements 0, 1; +8 for 2, 3
+  int row_limit[2];
+  long long mask_row[2];
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    const int row = rloc + 8 * e;
+    row_limit[e] = p.causal ? min(kv_len, q_rel0 + row + causal_off + 1) : kv_len;
+    // additive mask row of this query (rows past the end of the sequence read row Sq - 1: in bounds, never stored)
+    mask_row[e] = static_cast<long long>(b) * p.m_sb + static_cast<long long>(h) * p.m_sh +
+                  static_cast<long long>(min(q_begin + row, p.Sq - 1)) * p.m_sq;
+  }
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.0f, 0.0f};
+  float o[D / 2];
+#pragma unroll
+  for (int i = 0; i < D / 2; ++i) o[i] = 0.0f;
+  const uint32_t q_addr = smem_u32(sQ) + grp * 64 * 128;
+  mbar_wait(q_full, 0);
+  int st = 0;
+  uint32_t ph = 0;
+  for (int j = 0; j < n_tiles; ++j) {
+    float s[BN / 2];
+    mbar_wait(&k_full[st], ph);
+    const uint32_t k_addr = smem_u32(sK + st * KV_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < D / 16; ++k)
+      wgmma_ss(s, make_wgmma_desc_sw128(q_addr + (k >> 2) * 16384 + (k & 3) * 32, 16, 1024),
+               make_wgmma_desc_sw128(k_addr + (k >> 2) * KV_PANEL + (k & 3) * 32, 16, 1024), k != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operands(s);
+    if (lane == 0) mbar_arrive(&k_empty[st]);
+
+    const int k0 = j * BN;
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int n = 0; n < BN / 8; ++n)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int col = 8 * n + 2 * lm + (e & 1);
+        float v = s[4 * n + e];
+        if (p.mask && k0 + col < kv_len) v = fmaf(mask_value(p, mask_row[e >> 1], kv_begin + k0 + col), p.inv_scale, v);
+        v = (k0 + col < row_limit[e >> 1]) ? v : -INFINITY;  // columns [0, limit) of this tile are visible
+        s[4 * n + e] = v;
+        mx[e >> 1] = fmaxf(mx[e >> 1], v);
+      }
+    float alpha[2], m_scaled[2];
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      mx[e] = fmaxf(mx[e], __shfl_xor_sync(0xffffffffu, mx[e], 1));
+      mx[e] = fmaxf(mx[e], __shfl_xor_sync(0xffffffffu, mx[e], 2));
+      const float m_cand = fmaxf(m_run[e], mx[e]);
+      const bool grow = (m_cand - m_run[e]) * p.scale_log2 > 8.0f;  // also true for the first finite tile (m = -inf)
+      alpha[e] = 1.0f;
+      if (grow) {
+        alpha[e] = fast_exp2((m_run[e] - m_cand) * p.scale_log2);
+        m_run[e] = m_cand;
+        l_run[e] *= alpha[e];
+      }
+      m_scaled[e] = (m_run[e] == -INFINITY) ? 0.0f : m_run[e] * p.scale_log2;
+    }
+#pragma unroll
+    for (int n = 0; n < D / 8; ++n)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) o[4 * n + e] *= alpha[e >> 1];
+    // P = exp2(s * scale_log2 - m) as bf16 A fragments of the PV MMA: 16-key slice kk is n8 blocks 2 kk and 2 kk + 1
+    uint32_t pa[BN / 16][4];
+#pragma unroll
+    for (int kk = 0; kk < BN / 16; ++kk)
+#pragma unroll
+      for (int half = 0; half < 2; ++half) {
+        const int n = 2 * kk + half;
+        const float e0 = fast_exp2(fmaf(s[4 * n + 0], p.scale_log2, -m_scaled[0]));
+        const float e1 = fast_exp2(fmaf(s[4 * n + 1], p.scale_log2, -m_scaled[0]));
+        const float e2 = fast_exp2(fmaf(s[4 * n + 2], p.scale_log2, -m_scaled[1]));
+        const float e3 = fast_exp2(fmaf(s[4 * n + 3], p.scale_log2, -m_scaled[1]));
+        l_run[0] += e0 + e1;
+        l_run[1] += e2 + e3;
+        pa[kk][2 * half + 0] = pack_bf16x2(e0, e1);
+        pa[kk][2 * half + 1] = pack_bf16x2(e2, e3);
+      }
+    mbar_wait(&v_full[st], ph);
+    const uint32_t v_addr = smem_u32(sV + st * KV_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BN / 16; ++kk)
+      wgmma_rs_mn(o, pa[kk], make_wgmma_desc_sw128(v_addr + kk * 2048, KV_PANEL, 1024), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operands(o);
+    if (lane == 0) mbar_arrive(&v_empty[st]);
+    if (++st == KS) st = 0, ph ^= 1;
+  }
+
+  // ---- epilogue: O / l -> global (a row without any visible key gets zeros: O was never written) ----
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    l_run[e] += __shfl_xor_sync(0xffffffffu, l_run[e], 1);
+    l_run[e] += __shfl_xor_sync(0xffffffffu, l_run[e], 2);
+  }
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    const float inv_l = (l_run[e] > 0.0f) ? 1.0f / l_run[e] : 0.0f;
+    const int q_abs = q_begin + rloc + 8 * e;
+    if (q_abs >= q_end) continue;
+    __nv_bfloat16* dst = p.o + static_cast<long long>(b) * p.o_sb + static_cast<long long>(q_abs) * p.o_ss +
+                         static_cast<long long>(h) * p.o_sh + 2 * lm;
+#pragma unroll
+    for (int n = 0; n < D / 8; ++n)
+      *reinterpret_cast<uint32_t*>(dst + 8 * n) = pack_bf16x2(o[4 * n + 2 * e] * inv_l, o[4 * n + 2 * e + 1] * inv_l);
   }
 }
 
@@ -1316,79 +322,28 @@ static int make_attn_tmap(CUtensorMap* tm, const void* ptr, int64_t D, int64_t S
   return encode_tmap_bf16_sw128(tm, ptr, 4, dims, strides, box);
 }
 
-template <int D, int BN, bool PTM = false>
+template <int D, int BN>
 static int launch_attn(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttnParams& p,
                        dim3 grid, cudaStream_t stream) {
-  constexpr int smem_bytes = AttnCfg<D, BN, PTM>::SMEM;
+  constexpr int smem_bytes = AttnCfg<D, BN>::SMEM;
+  static_assert(smem_bytes <= 227 * 1024, "K/V ring does not fit shared memory");
   static bool configured = false;
   if (!configured) {
-    B200_CUDA(cudaFuncSetAttribute(attn_kernel<D, BN, PTM>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    B200_CUDA(cudaFuncSetAttribute(attn_kernel<D, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
     configured = true;
   }
-  B200_CUDA(launch_pdl(attn_kernel<D, BN, PTM>, grid, dim3(192), smem_bytes, stream, 1, tq, tk, tv, p));
+  B200_CUDA(launch_pdl(attn_kernel<D, BN>, grid, dim3(ATTN_THREADS), smem_bytes, stream, 1, tq, tk, tv, p));
   return 0;
 }
 
-static int g_no_shortkv = 0;  // test hook: 1 = always use the general kernel
-#ifndef ATTN_BN64_DEFAULT
-#define ATTN_BN64_DEFAULT 0
-#endif
-// D = 64: 1 = 64-key blocks, 3 CTAs per SM; 0 (default) = 128-key blocks, 2 CTAs per SM. Measured (tools/attn_probe.py):
-// the third CTA does not pay for the halved block (twice the barrier round trips per key, 96 registers per thread):
-// 629 vs 680 TFLOP/s at S = 4096, 512 vs 517 at S = 1024. Kept selectable for A/B runs and tested.
-static int g_attn_bn64 = ATTN_BN64_DEFAULT;
-static int g_attn_ptmem = 0;  // D = 64: 1 = keep P in TMEM (A operand of the PV MMA); measured slower on long sequences
-
-static int launch_attn_shortkv(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttnParams& p,
-                               int B, cudaStream_t stream) {
-  static bool configured = false;
-  if (!configured) {
-    B200_CUDA(cudaFuncSetAttribute(attn_shortkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SKV_SMEM));
-    configured = true;
-  }
-  const int nq = (p.Sq + 127) / 128;
-  const long long total = static_cast<long long>(B) * p.Hq * nq;
-  const int grid = static_cast<int>(std::min<long long>(total, 2ll * num_sms()));
-  B200_CUDA(launch_pdl(attn_shortkv_kernel, dim3(grid), dim3(192), SKV_SMEM, stream, 1, tq, tk, tv, p, nq, (int)total));
-  return 0;
-}
-
-#ifndef ATTN_PP_STAGES
-#define ATTN_PP_STAGES 3
-#endif
-static int g_attn_pp = 1;  // test / measurement hook: 0 = D = 64 self-attention goes through attn_kernel<64> again
-
-static int launch_attn_pp(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttnParams& p, int B,
-                          cudaStream_t stream) {
-  constexpr int smem_bytes = AttnPPCfg<ATTN_PP_STAGES>::SMEM;
-  static_assert(smem_bytes <= 227 * 1024, "ring depth does not fit shared memory");
-  static bool configured = false;
-  if (!configured) {
-    B200_CUDA(cudaFuncSetAttribute(attn_pp_kernel<ATTN_PP_STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   smem_bytes));
-    configured = true;
-  }
-  const int npairs = (p.Sq + 255) / 256;
-  const long long total = static_cast<long long>(B) * p.Hq * npairs;
-  const int grid = static_cast<int>(std::min<long long>(total, num_sms()));
-  B200_CUDA(launch_pdl(attn_pp_kernel<ATTN_PP_STAGES>, dim3(grid), dim3(384), smem_bytes, stream, 1, tq, tk, tv, p,
-                       npairs, (int)total));
-  return 0;
-}
+// D = 64: 1 = 64-key blocks, 0 (default) = 128-key blocks. Kept selectable for A/B runs and tested.
+static int g_attn_bn64 = 0;
 
 }  // namespace b200
 
 using namespace b200;
 
-extern "C" void b200mix_debug_no_shortkv(int on) { b200::g_no_shortkv = on; }
 extern "C" void b200mix_debug_attn_bn64(int on) { b200::g_attn_bn64 = on; }
-extern "C" void b200mix_debug_attn_ptmem(int on) { b200::g_attn_ptmem = on; }
-extern "C" void b200mix_debug_attn_pingpong(int on) { b200::g_attn_pp = on; }
-#if ATTN_PROF
-extern "C" int b200mix_debug_attn_prof_read(unsigned long long* host_out) {
-  return cudaMemcpyFromSymbol(host_out, b200::g_attn_prof, sizeof(unsigned long long) * 148 * 32) == cudaSuccess ? 0 : -1;
-}
-#endif
 
 extern "C" int b200mix_sdpa(const void* q, const void* k, const void* v, void* o, int64_t B, int64_t Hq, int64_t Hkv,
                             int64_t Sq, int64_t Sk, int64_t D, int64_t q_sb, int64_t q_ss, int64_t q_sh, int64_t k_sb,
@@ -1431,25 +386,13 @@ extern "C" int b200mix_sdpa(const void* q, const void* k, const void* v, void* o
   p.inv_scale = attn_mask ? 1.0f / scale : 0.0f;
   CUtensorMap tq, tk, tv;
   if (int rc = make_attn_tmap(&tq, q, D, Sq, Hq, B, q_ss, q_sh, q_sb, p.q_pos)) return rc;
-  // short-KV kernel: 128-key boxes; general kernel at D = 64: 128-key blocks unless the 64-key variant is switched on
-  const bool shortkv = D == 64 && !causal && !cu_seqlens && Sk <= 128 && !g_no_shortkv &&
-                       B * Hq * ((Sq + 127) / 128) < (1ll << 31);
-  const bool pingpong = D == 64 && !causal && !cu_seqlens && !shortkv && g_attn_pp && !g_attn_bn64 && !g_attn_ptmem &&
-                        Sk > 128 && B * Hq * ((Sq + 255) / 256) < (1ll << 31);
-  const uint32_t kv_box = (D == 64 && !shortkv && !pingpong && g_attn_bn64) ? 64u : 128u;
+  const uint32_t kv_box = (D == 64 && !g_attn_bn64) ? 128u : 64u;
   if (int rc = make_attn_tmap(&tk, k, D, Sk, Hkv, B, k_ss, k_sh, k_sb, p.k_pos, kv_box)) return rc;
   if (int rc = make_attn_tmap(&tv, v, D, Sk, Hkv, B, v_ss, v_sh, v_sb, p.v_pos, kv_box)) return rc;
-  cudaStream_t st0 = reinterpret_cast<cudaStream_t>(stream);
-  if (shortkv) return launch_attn_shortkv(tq, tk, tv, p, (int)B, st0);
-  if (pingpong) return launch_attn_pp(tq, tk, tv, p, (int)B, st0);
   int64_t q_tiles = (Sq + 127) / 128 + (cu_seqlens ? nseq : 0);
   dim3 grid((unsigned)q_tiles, (unsigned)Hq, (unsigned)B);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (D == 64) {
-    if (kv_box == 64) return launch_attn<64, 64>(tq, tk, tv, p, grid, st);
-    return (g_attn_ptmem && !attn_mask) ? launch_attn<64, 128, true>(tq, tk, tv, p, grid, st)
-                                        : launch_attn<64, 128>(tq, tk, tv, p, grid, st);
-  }
-  if (D == 128) return launch_attn<128, 128>(tq, tk, tv, p, grid, st);
-  return launch_attn<192, 128>(tq, tk, tv, p, grid, st);
+  if (D == 64) return kv_box == 64 ? launch_attn<64, 64>(tq, tk, tv, p, grid, st) : launch_attn<64, 128>(tq, tk, tv, p, grid, st);
+  if (D == 128) return launch_attn<128, 64>(tq, tk, tv, p, grid, st);
+  return launch_attn<192, 64>(tq, tk, tv, p, grid, st);
 }

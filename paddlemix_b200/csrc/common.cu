@@ -32,8 +32,8 @@ int ensure_device() {
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
   cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (major != 10) {
-    set_error("device %d is sm_%d%d; b200mix kernels are sm_100a only", dev, major, minor);
+  if (major != 9 || minor != 0) {
+    set_error("device %d is sm_%d%d; b200mix kernels are sm_90a only", dev, major, minor);
     return B200MIX_ERR_NO_DEVICE;
   }
   g_sms = sms;
@@ -41,7 +41,7 @@ int ensure_device() {
   return 0;
 }
 
-int num_sms() { return g_sms > 0 ? g_sms : 148; }
+int num_sms() { return g_sms > 0 ? g_sms : 132; }
 
 bool pdl_enabled() {
   static const bool on = (getenv("B200MIX_NO_PDL") == nullptr);
@@ -111,7 +111,7 @@ int encode_tmap_bf16_sw128(CUtensorMap* out, const void* gptr, int rank, const u
 extern "C" {
 
 const char* b200mix_last_error(void) { return b200::g_err; }
-const char* b200mix_version(void) { return "b200mix 0.1 (sm_100a)"; }
+const char* b200mix_version(void) { return "b200mix 0.1 (sm_90a)"; }
 
 int b200mix_init(int device) {
   cudaError_t e = cudaSetDevice(device);

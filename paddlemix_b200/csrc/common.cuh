@@ -11,7 +11,7 @@
 namespace b200 {
 
 void set_error(const char* fmt, ...);
-int ensure_device();  // 0 if an sm_100 device is current, else negative status (with message)
+int ensure_device();  // 0 if an sm_90 device is current, else negative status (with message)
 int num_sms();
 
 #define B200_CHECK_ARG(cond, ...)                 \

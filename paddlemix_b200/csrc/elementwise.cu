@@ -510,7 +510,7 @@ __global__ void scatter_rows_kernel(const uint4* __restrict__ src, const long lo
 
 static inline unsigned ew_grid(long long n, int threads) {
   long long g = (n + threads - 1) / threads;
-  const long long cap = 148LL * 16;
+  const long long cap = (long long)num_sms() * 16;
   return (unsigned)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
@@ -1059,88 +1059,3 @@ extern "C" int b200mix_unpatchify3d(const void* x, float* y, int64_t B, int64_t 
   return 0;
 }
 
-// Microbenchmark (debug, not in the public header): MUFU throughput of ex2.approx.f32 vs ex2.approx.f16x2, used to
-// decide how the attention kernel exponentiates (see DESIGN.md). mode 0: f32, mode 1: f16x2.
-namespace b200 {
-__global__ void mufu_bench_kernel(float* out, int iters, int mode) {
-  float a = threadIdx.x * 1e-3f, b = a + 0.5f, c = a - 0.25f, d = a + 0.125f;
-  uint32_t ha, hb, hc, hd;
-  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(ha) : "f"(a), "f"(b));
-  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(hb) : "f"(c), "f"(d));
-  hc = ha ^ 0x00010001u, hd = hb ^ 0x00010001u;
-  uint32_t acc = 0;
-  uint64_t p0 = pack_f32x2(a, b), p1 = pack_f32x2(c, d);
-  const uint64_t k2 = pack_f32x2(0.999f, 1.001f), m2 = pack_f32x2(-0.01f, 0.01f);
-  for (int i = 0; i < iters; ++i) {
-    if (mode == 0 || mode >= 3) {  // 4 x ex2.f32 per iteration (the reference unit of every mixed mode)
-      if (mode != 7 && mode != 8 && mode != 9) {
-        asm volatile("ex2.approx.ftz.f32 %0, %0;" : "+f"(a));
-        asm volatile("ex2.approx.ftz.f32 %0, %0;" : "+f"(b));
-        asm volatile("ex2.approx.ftz.f32 %0, %0;" : "+f"(c));
-        asm volatile("ex2.approx.ftz.f32 %0, %0;" : "+f"(d));
-      }
-    } else if (mode == 1) {
-      asm volatile("ex2.approx.f16x2 %0, %0;" : "+r"(ha));
-      asm volatile("ex2.approx.f16x2 %0, %0;" : "+r"(hb));
-      asm volatile("ex2.approx.f16x2 %0, %0;" : "+r"(hc));
-      asm volatile("ex2.approx.f16x2 %0, %0;" : "+r"(hd));
-    }
-    if (mode == 2 || mode == 3 || mode == 4) {  // 2 x cvt.rn.bf16x2.f32 (F2FP): with mode 2, 4 of them and no ex2
-      uint32_t w0, w1;
-      asm volatile("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(w0) : "f"(a), "f"(b));
-      asm volatile("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(w1) : "f"(c), "f"(d));
-      acc ^= w0 ^ w1;
-      if (mode == 2) {
-        asm volatile("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(w0) : "f"(b), "f"(c));
-        asm volatile("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(w1) : "f"(d), "f"(a));
-        acc ^= w0 ^ w1;
-        a += 1e-7f, b += 1e-7f, c += 1e-7f, d += 1e-7f;
-      }
-    }
-    if (mode == 4 || mode == 6) {  // + the packed scale-subtract and row-sum of the softmax loop: 2 FFMA2 + 2 FADD2
-      p0 = ffma2(pack_f32x2(a, b), k2, m2);
-      p1 = ffma2(pack_f32x2(c, d), k2, m2);
-      unpack_f32x2(p0, a, b);
-      unpack_f32x2(p1, c, d);
-      asm volatile("add.rn.f32x2 %0, %0, %1;" : "+l"(p0) : "l"(m2));
-      asm volatile("add.rn.f32x2 %0, %0, %1;" : "+l"(p1) : "l"(m2));
-    }
-    if (mode == 5 || mode == 6) {  // bf16 pack on the integer pipe: round-half-up (+0x8000) and PRMT of the high halves
-      uint32_t w0, w1;
-      const uint32_t ia = __float_as_uint(a) + 0x8000u, ib = __float_as_uint(b) + 0x8000u;
-      const uint32_t ic = __float_as_uint(c) + 0x8000u, id = __float_as_uint(d) + 0x8000u;
-      asm volatile("prmt.b32 %0, %1, %2, 0x7632;" : "=r"(w0) : "r"(ia), "r"(ib));
-      asm volatile("prmt.b32 %0, %1, %2, 0x7632;" : "=r"(w1) : "r"(ic), "r"(id));
-      acc ^= w0 ^ w1;
-    }
-    if (mode == 7) {  // FFMA2 alone (4 per iteration)
-      asm volatile("fma.rn.f32x2 %0, %0, %1, %2;" : "+l"(p0) : "l"(k2), "l"(m2));
-      asm volatile("fma.rn.f32x2 %0, %0, %1, %2;" : "+l"(p1) : "l"(k2), "l"(m2));
-      asm volatile("fma.rn.f32x2 %0, %0, %1, %2;" : "+l"(p0) : "l"(k2), "l"(m2));
-      asm volatile("fma.rn.f32x2 %0, %0, %1, %2;" : "+l"(p1) : "l"(k2), "l"(m2));
-    }
-    if (mode == 8) {  // FMNMX3 alone (4 per iteration)
-      asm volatile("max.f32 %0, %0, %1, %2;" : "+f"(a) : "f"(b), "f"(c));
-      asm volatile("max.f32 %0, %0, %1, %2;" : "+f"(b) : "f"(c), "f"(d));
-      asm volatile("max.f32 %0, %0, %1, %2;" : "+f"(c) : "f"(d), "f"(a));
-      asm volatile("max.f32 %0, %0, %1, %2;" : "+f"(d) : "f"(a), "f"(b));
-    }
-    if (mode == 9) {  // plain FFMA (3 register operands), 4 per iteration
-      asm volatile("fma.rn.f32 %0, %0, %1, %2;" : "+f"(a) : "f"(b), "f"(c));
-      asm volatile("fma.rn.f32 %0, %0, %1, %2;" : "+f"(b) : "f"(c), "f"(d));
-      asm volatile("fma.rn.f32 %0, %0, %1, %2;" : "+f"(c) : "f"(d), "f"(a));
-      asm volatile("fma.rn.f32 %0, %0, %1, %2;" : "+f"(d) : "f"(a), "f"(b));
-    }
-  }
-  float q0, q1, q2, q3;
-  unpack_f32x2(p0, q0, q1);
-  unpack_f32x2(p1, q2, q3);
-  out[blockIdx.x * blockDim.x + threadIdx.x] = a + b + c + d + q0 + q1 + q2 + q3 + __uint_as_float(ha ^ hb ^ hc ^ hd ^ acc);
-}
-}  // namespace b200
-extern "C" int b200mix_debug_mufu_bench(float* out, int blocks, int threads, int iters, int mode, void* stream) {
-  if (int rc = ensure_device()) return rc;
-  mufu_bench_kernel<<<blocks, threads, 0, ST(stream)>>>(out, iters, mode);
-  B200_LAUNCH_CHECK();
-  return 0;
-}

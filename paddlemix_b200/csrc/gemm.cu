@@ -1,20 +1,14 @@
-// Implicit-GEMM on 5th-gen tensor cores: one persistent, warp-specialised kernel that serves
+// Implicit-GEMM on Hopper tensor cores: one persistent, warp-specialised kernel that serves
 //   * Linear / 1x1 conv        C[M,N] = A[M,K] W[N,K]^T                       (1 tap)
 //   * conv3x3 NHWC, stride 1|2 y = sum_taps shift(x) W_tap^T                  (9 taps, im2col-free)
 // Data path: TMA (cp.async.bulk.tensor, 128B swizzle, hardware zero fill for halos / ragged edges) -> shared memory
-// ring -> tcgen05.mma (bf16 x bf16 -> fp32, 128 x BN x 16 per instruction) -> double-buffered TMEM accumulators ->
-// tcgen05.ld -> fused epilogue (bias / temb row-add / activation / GEGLU|SwiGLU / AdaLN gate / residual) -> HBM.
+// ring -> wgmma (bf16 x bf16 -> fp32 register accumulators, 64 x BN x 16 per instruction and consumer warpgroup) ->
+// fused epilogue (bias / temb row-add / activation / GEGLU|SwiGLU / AdaLN gate / residual) -> HBM.
 //
 // CTAs run as clusters of 2 along M: both CTAs of a cluster work on the same n-tile, and each loads one half of the
 // weight tile with TMA multicast into both CTAs' shared memory, so the L2 -> SM traffic per MAC drops from
-// (128+BN)/(128*BN) to (128+BN/2)/(128*BN) (a 128x256 tile at full tensor rate would otherwise need ~14 KB/clk from
-// L2 chip-wide, more than L2 delivers). Stage hand-back is one multicast tcgen05.commit to both CTAs' empty barriers.
-//
-// Roles (320 threads): warps 0..7 = epilogue (two warpgroups; warp%4 selects the TMEM lane quarter, the warpgroup the
-// column chunks), warp 8 = TMEM owner + MMA issuer (1 elected lane), warp 9 = TMA producer (1 elected lane). The
-// single-thread roles have the HIGHEST warp ids: the sub-partition scheduler prefers the highest eligible warp id
-// (B300_MICROARCH.md), so the epilogue warps of tile i cannot starve the MMA issue / TMA refill of tile i+1. The
-// epilogue of tile i overlaps the main loop of tile i+1 through the two TMEM accumulator stages.
+// (128+BN)/(128*BN) to (128+BN/2)/(128*BN). A stage goes back to the producers when every consumer warp of both CTAs
+// has arrived on its empty barrier (local arrive + remote arrive through the cluster's shared-memory window).
 //
 // Replaces (reference): F.linear / F.conv2d call sites ppdiffusers/models/lora.py:365-377,453-459,
 // resnet.py:728-808, attention.py:623-677 (FeedForward/GEGLU), and their cuBLASLt / cuDNN kernels inside Paddle.
@@ -38,7 +32,7 @@ struct IGemmParams {
   int tap_dc[16], tap_dx[16], tap_p[16], tap_dy[16];
   // fused nearest-2x upsample (b200mix_conv3x3_up2x): m-tiles enumerate (output parity, low-resolution tile); tile
   // `mt` has parity mt / par_tiles and uses taps [4 * parity, 4 * parity + 4); its rows land on output pixels
-  // (2y + parity / 2, 2x + parity % 2). par_tiles = tiles per parity rounded up to even (a CTA pair shares one B tile).
+  // (2y + parity / 2, 2x + parity % 2). par_tiles = tiles per parity rounded up to even (the two CTAs of a cluster share one n-tile).
   int up, par_tiles;
   // epilogue
   const float* bias;
@@ -79,9 +73,6 @@ struct IGemmParams {
 // the head piece's epilogue - which runs (1 + T mod C / C) tiles later - adds them to its own accumulators and finishes
 // the tile (fixed split and fixed order: results are reproducible run to run). The remaining T - sk_tiles tiles (a
 // multiple of C) follow round-robin as before. Every cluster thus gets T / C tiles' worth of k-blocks.
-#ifndef LN_PROBE  // measurement builds (tools/ln_fold_probe.py): 1 = no statistics load / math, 2 = no transform of r[]
-#define LN_PROBE 0
-#endif
 constexpr int SK_WS_FLOAT4_PER_CTA = 8 * 8 * 128;  // 8 chunks x 8 float4 x 128 rows = 128 KB
 enum { SEG_FULL = 0, SEG_TAIL = 1, SEG_HEAD = 2 };
 struct SegIter {
@@ -188,7 +179,7 @@ __device__ __forceinline__ float act_eval(float x, const ActCoef& a) {
   return x_sigmoid_neg_log2(x, x * fmaf(fmaf(a.c2, x2, a.c1), x2, a.c0));
 }
 
-// Global-memory operands of one 32-column chunk of one accumulator row, fetched ahead of the TMEM load completing.
+// Global-memory operands of one 32-column chunk of one accumulator row.
 struct EpiOperands {  // direct (row-per-thread) path: GLU / fp32 output / unaligned or partial chunks
   float4 bias[8];
   bool vec;
@@ -318,7 +309,7 @@ __device__ __forceinline__ void epilogue_chunk(const IGemmParams& p, const ActCo
 }
 
 // ---- coalesced epilogue (bf16 output, no GLU, aligned full chunk) -------------------------------------------------
-// tcgen05.ld hands every thread one accumulator ROW (32 consecutive columns = 64 bytes of bf16). Writing / reading
+// The epilogue hands every thread one accumulator ROW (32 consecutive columns = 64 bytes of bf16). Writing / reading
 // global memory in that shape makes each lane of a 16-byte access hit a different 128-byte line (32 L1 wavefronts per
 // instruction). The chunk is therefore transposed through a 2 KB per-warp shared-memory buffer so that a warp's
 // global access covers 8 rows x 64 contiguous bytes (8 wavefronts): 4 lanes per row, lane L -> row s*8 + L/4,
@@ -425,40 +416,42 @@ __device__ __forceinline__ void epilogue_chunk_staged(const IGemmParams& p, cons
   __syncwarp();
 }
 
-// PAIR = the two CTAs of a cluster run ONE 256 x BN MMA (tcgen05 cta_group::2): each CTA stages its own 128 rows of A and
-// only BN/2 rows of B, so a pipeline stage is 1/3 smaller and the B operand is read from shared memory once per pair.
-// !PAIR = each CTA runs its own 128 x BN MMA and the two halves of the B tile are multicast to both.
-template <int BN, bool PAIR>
+// MCAST = the two CTAs of a cluster work on the same n-tile and each loads one half of the B tile with TMA multicast into
+// both CTAs' shared memory, so the L2 -> SM traffic per MAC drops from (128+BN)/(128*BN) to (128+BN/2)/(128*BN).
+// !MCAST = every CTA loads its whole B tile itself (no cluster); the tile schedule is the same.
+template <int BN>
 struct IGemmCfg {
   static constexpr int A_BYTES = 128 * 128;  // 128 rows x 64 bf16 (128 B per row, SW128)
-  static constexpr int B_BYTES = (PAIR ? BN / 2 : BN) * 128;
+  static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int ACC_STRIDE = BN <= 32 ? 32 : (BN <= 64 ? 64 : (BN <= 128 ? 128 : 256));
-  static constexpr int TMEM_COLS = 2 * ACC_STRIDE;
+  // fp32 staging of 64 accumulator columns of one warpgroup's 64 rows; the row stride of 68 floats makes the row-wise
+  // float4 reads of the epilogue conflict-free
+  static constexpr int ACC_LD = 68;
+  static constexpr int ACC_BYTES = 2 * 64 * ACC_LD * 4;
+  // barriers | accumulator staging | 8 epilogue warps x 2 KB transpose buffers | 8 x 128 bias + 8 x 128 column sums
+  static constexpr int EXTRA_BYTES = 1024 + 256 + ACC_BYTES + 8 * 2048 + 2 * 8 * 512;
 };
 
-// warp roles (IGEMM_ROLES_LOW=1 restores the round-1 order, TMA = warp 0 / MMA = warp 1 / epilogue = warps 2-9, for A/B runs)
-#ifndef IGEMM_ROLES_LOW
-#define IGEMM_ROLES_LOW 0
-#endif
-constexpr int IG_WARP_MMA = IGEMM_ROLES_LOW ? 1 : 8, IG_WARP_TMA = IGEMM_ROLES_LOW ? 0 : 9, IG_EPI_BASE = IGEMM_ROLES_LOW ? 2 : 0;
+// Roles (288 threads): warps 0-7 = two consumer warpgroups, warp 8 = TMA producer (one elected lane). Consumer
+// warpgroup g multiplies rows [64 g, 64 g + 64) of the 128-row tile (wgmma m64 x BN x k16, accumulators in registers)
+// and then runs the epilogue of those rows: 64 accumulator columns at a time go through shared memory so that every
+// thread owns 32 consecutive columns of one row (warp w of the group: rows 32 (w & 1) + lane, chunk parity w >> 1).
+constexpr int IG_THREADS = 288;
+constexpr int IG_WARP_TMA = 8;
 
-// LNM: the folded-LayerNorm epilogues are separate instantiations - the plain kernel carries none of their code (with
-// runtime flags only, their live ranges and branches cost every GEMM of the step ~2 %: 58.2 vs 57.0 ms on one clock).
+// LNM: the folded-LayerNorm epilogues are separate instantiations - the plain kernel carries none of their code.
 enum { LNM_NONE = 0, LNM_CONSUMER = 1, LNM_PRODUCER = 2 };
-template <int BN, int STAGES, bool PAIR, int LNM>
-__global__ void __launch_bounds__(320, 1)
+template <int BN, int STAGES, bool MCAST, int LNM>
+__global__ void __launch_bounds__(IG_THREADS, 1)
     igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ IGemmParams p) {
-  using Cfg = IGemmCfg<BN, PAIR>;
+  using Cfg = IGemmCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull = empty_bar + STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-  uint8_t* stage_all = smem + STAGES * Cfg::STAGE_BYTES + 256;  // 8 epilogue warps x 2 KB transpose buffers
+  float* acc_all = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES + 256);
+  uint8_t* stage_all = reinterpret_cast<uint8_t*>(acc_all) + Cfg::ACC_BYTES;
   float* bias_all = reinterpret_cast<float*>(stage_all + 8 * 2048);  // 8 epilogue warps x 128 floats (their 4 chunks)
   float* colsum_all = bias_all + 8 * 128;                            // same layout: folded-LayerNorm column sums
 
@@ -468,30 +461,19 @@ __global__ void __launch_bounds__(320, 1)
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], PAIR ? 1 : 2);  // one multicast commit from each MMA-issuing CTA of the cluster
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull[s], 1);
-      mbar_init(&tempty[s], PAIR ? 512 : 256);  // PAIR: the leader's barrier collects both CTAs' epilogue threads
+      mbar_init(&empty_bar[s], MCAST ? 16 : 8);  // every consumer warp of every CTA that reads the stage
     }
     fence_barrier_init();
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
   }
-  if (warp == IG_WARP_MMA) {
-    if (PAIR) tmem_alloc_pair<Cfg::TMEM_COLS>(tmem_slot);
-    else tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  }
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();  // barrier inits of both CTAs visible before any multicast TMA / remote commit
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (MCAST) cluster_sync_all();  // barrier inits of both CTAs visible before any multicast TMA / remote arrival
   // everything above overlapped the tail of the previous kernel; from here on we touch its outputs
   pdl_wait();
   pdl_launch_dependents();
 
-  const uint32_t cta_rank = cluster_ctarank();
+  const uint32_t cta_rank = MCAST ? cluster_ctarank() : (blockIdx.x & 1u);
   const int cluster_id = blockIdx.x >> 1;
   const int num_clusters = gridDim.x >> 1;
   const int tiles_m = p.up ? 4 * p.par_tiles : p.tiles_x * p.tiles_y * p.tiles_b;
@@ -500,112 +482,98 @@ __global__ void __launch_bounds__(320, 1)
   const int kblocks = p.ntaps * p.kchunks;
 
   if (warp == IG_WARP_TMA) {
-    {
-      // ===== TMA producer (whole warp runs the loop, one elected lane issues: see elect_one_sync) =====
-      int stage = 0;
-      uint32_t phase = 0;
-      for (SegIter seg(p.sk_tiles, total_super, kblocks, cluster_id, num_clusters); seg.next();) {
-        const int st = seg.st;
-        const int mp = st / p.tiles_n, nt = st - mp * p.tiles_n;
-        int mt = mp * 2 + (int)cta_rank;  // may be == tiles_m (phantom): its A box is out of bounds -> zeros
-        int tap_base = 0;
-        if (p.up) {  // phantom tiles of a parity (index >= tiles of the grid) get b0 >= Bn: zeros as well
-          const int par = mt / p.par_tiles;
-          mt -= par * p.par_tiles, tap_base = par * 4;
-        }
-        const int tx = mt % p.tiles_x;
-        const int ty = (mt / p.tiles_x) % p.tiles_y;
-        const int tb = mt / (p.tiles_x * p.tiles_y);
-        const int x0 = tx * p.TW, y0 = ty * p.TH, b0 = tb * p.TB, n0 = nt * BN;
-        int tap = seg.kb0 / p.kchunks, kc = seg.kb0 - tap * p.kchunks;
-        for (int kb = seg.kb0; kb < seg.kb1; ++kb) {
-          const int tg = tap_base + tap;
-          const int dc = p.tap_dc[tg], dx = p.tap_dx[tg], pp = p.tap_p[tg], dy = p.tap_dy[tg];
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
-          uint8_t* sB = sA + Cfg::A_BYTES;
-          if (elect_one_sync()) {
-            if (PAIR) {
-              // both CTAs' boxes complete on the LEADER's barrier (it alone issues the MMA): my A rows, my half of B
-              if (cta_rank == 0) mbar_expect_tx(&full_bar[stage], 2 * Cfg::STAGE_BYTES);
-              const uint32_t lbar = mapa_smem(&full_bar[stage], 0);
-              tma_load_5d_pair(sA, &tmA, lbar, kc * 64 + dc, x0 + dx, pp, y0 + dy, b0);
-              tma_load_2d_pair(sB, &tmB, lbar, tg * p.Kc + kc * 64, n0 + (int)cta_rank * (BN / 2));
-            } else {
-              mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-              tma_load_5d(sA, &tmA, &full_bar[stage], kc * 64 + dc, x0 + dx, pp, y0 + dy, b0);
-              // my half of the weight tile, delivered to both CTAs of the cluster
-              tma_load_2d_mcast(sB + cta_rank * (Cfg::B_BYTES / 2), &tmB, &full_bar[stage], tg * p.Kc + kc * 64,
-                                n0 + (int)cta_rank * (BN / 2), (uint16_t)0x3);
-            }
-          }
-          __syncwarp();
-          if (++stage == STAGES) stage = 0, phase ^= 1;
-          if (++kc == p.kchunks) kc = 0, ++tap;
-        }
+    // ===== TMA producer (whole warp runs the loop, one elected lane issues: see elect_one_sync) =====
+    int stage = 0;
+    uint32_t phase = 0;
+    for (SegIter seg(p.sk_tiles, total_super, kblocks, cluster_id, num_clusters); seg.next();) {
+      const int st = seg.st;
+      const int mp = st / p.tiles_n, nt = st - mp * p.tiles_n;
+      int mt = mp * 2 + (int)cta_rank;  // may be == tiles_m (phantom): its A box is out of bounds -> zeros
+      int tap_base = 0;
+      if (p.up) {  // phantom tiles of a parity (index >= tiles of the grid) get b0 >= Bn: zeros as well
+        const int par = mt / p.par_tiles;
+        mt -= par * p.par_tiles, tap_base = par * 4;
       }
-    }
-  } else if (warp == IG_WARP_MMA) {
-    if (!PAIR || cta_rank == 0) {
-      // ===== MMA issuer (PAIR: the leader CTA drives the tensor cores of both SMs); converged warp, elected lane =====
-      constexpr uint32_t idesc = make_idesc_bf16(PAIR ? 256 : 128, BN, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      for (SegIter seg(p.sk_tiles, total_super, kblocks, cluster_id, num_clusters); seg.next();) {
-        if (PAIR) mbar_wait_cluster(&tempty[as], aphase ^ 1);
-        else mbar_wait(&tempty[as], aphase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * Cfg::ACC_STRIDE;
-        const int kb_first = seg.kb0, kb_last = seg.kb1 - 1;
-        for (int kb = kb_first; kb <= kb_last; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-          const uint32_t b_addr = a_addr + Cfg::A_BYTES;
-          if (elect_one_sync()) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint64_t ad = make_smem_desc_sw128(a_addr + k * 32, 16, 1024);
-              const uint64_t bd = make_smem_desc_sw128(b_addr + k * 32, 16, 1024);
-              const uint32_t accumulate = (kb != kb_first || k != 0) ? 1u : 0u;  // a piece starts from zero
-              if (PAIR) umma_bf16_ss_pair(d_tmem, ad, bd, idesc, accumulate);
-              else umma_bf16_ss(d_tmem, ad, bd, idesc, accumulate);
-            }
-            // frees this stage in both CTAs
-            if (PAIR) umma_commit_pair_mcast(&empty_bar[stage], (uint16_t)0x3);
-            else umma_commit_mcast(&empty_bar[stage], (uint16_t)0x3);
-            if (kb == kb_last) {
-              if (PAIR) umma_commit_pair_mcast(&tfull[as], (uint16_t)0x3);  // accumulators of both CTAs are ready
-              else umma_commit(&tfull[as]);
-            }
+      const int tx = mt % p.tiles_x;
+      const int ty = (mt / p.tiles_x) % p.tiles_y;
+      const int tb = mt / (p.tiles_x * p.tiles_y);
+      const int x0 = tx * p.TW, y0 = ty * p.TH, b0 = tb * p.TB, n0 = nt * BN;
+      int tap = seg.kb0 / p.kchunks, kc = seg.kb0 - tap * p.kchunks;
+      for (int kb = seg.kb0; kb < seg.kb1; ++kb) {
+        const int tg = tap_base + tap;
+        const int dc = p.tap_dc[tg], dx = p.tap_dx[tg], pp = p.tap_p[tg], dy = p.tap_dy[tg];
+        // MCAST: the peer CTA's consumers release this stage too (remote arrivals)
+        if (MCAST) mbar_wait_cluster(&empty_bar[stage], phase ^ 1);
+        else mbar_wait(&empty_bar[stage], phase ^ 1);
+        uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
+        uint8_t* sB = sA + Cfg::A_BYTES;
+        if (elect_one_sync()) {
+          mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+          tma_load_5d(sA, &tmA, &full_bar[stage], kc * 64 + dc, x0 + dx, pp, y0 + dy, b0);
+          if (MCAST) {
+            // my half of the weight tile, delivered to both CTAs of the cluster
+            tma_load_2d_mcast(sB + cta_rank * (Cfg::B_BYTES / 2), &tmB, &full_bar[stage], tg * p.Kc + kc * 64,
+                              n0 + (int)cta_rank * (BN / 2), (uint16_t)0x3);
+          } else {
+            tma_load_2d(sB, &tmB, &full_bar[stage], tg * p.Kc + kc * 64, n0);
+            tma_load_2d(sB + Cfg::B_BYTES / 2, &tmB, &full_bar[stage], tg * p.Kc + kc * 64, n0 + BN / 2);
           }
-          __syncwarp();
-          if (++stage == STAGES) stage = 0, phase ^= 1;
         }
-        as ^= 1;
-        if (as == 0) aphase ^= 1;
+        __syncwarp();
+        if (++stage == STAGES) stage = 0, phase ^= 1;
+        if (++kc == p.kchunks) kc = 0, ++tap;
       }
     }
   } else {
-    // ===== epilogue: two warpgroups (warps 0-3 and 4-7), each covering all four TMEM lane quarters; warpgroup g
-    // handles the 32-column chunks c == g (mod 2), so every SM sub-partition has two epilogue warps in flight =====
-    const int q = warp & 3;
-    const int wg = (warp - IG_EPI_BASE) >> 2;
-    uint8_t* stage = stage_all + (warp - IG_EPI_BASE) * 2048;
-    float* bias_s = bias_all + (warp - IG_EPI_BASE) * 128;
-    float* colsum_s = colsum_all + (warp - IG_EPI_BASE) * 128;
+    // ===== consumers: MMA of 64 rows, then their epilogue =====
+    const int grp = warp >> 2, w = warp & 3;
+    const int q = 2 * grp + (w & 1);  // 32-row quarter of the tile this warp's epilogue owns
+    const int wg = w >> 1;            // its 32-column chunks are c == wg (mod 2)
+    uint8_t* stage = stage_all + warp * 2048;
+    float* bias_s = bias_all + warp * 128;
+    float* colsum_s = colsum_all + warp * 128;
+    float* sacc = acc_all + grp * 64 * Cfg::ACC_LD;
     const ActCoef ac = act_coef(p.act, p.glu);
     const bool staged_ok = p.vec_ok && !p.glu && !p.out_fp32 && ((p.c_bstride | p.r_bstride) & 7) == 0;
     const int row = q * 32 + lane;
     const int tw = row % p.TW;
     const int th = (row / p.TW) % p.TH;
     const int tbb = row / (p.TW * p.TH);
-    int as = 0;
-    uint32_t aphase = 0;
-    const int epi_tid = (warp - IG_EPI_BASE) * 32 + lane;
+    const uint32_t peer_empty = MCAST ? mapa_smem(&empty_bar[0], cta_rank ^ 1u) : 0u;
+    int kstage = 0;
+    uint32_t kphase = 0;
+    const int epi_tid = warp * 32 + lane;
+    auto release = [&](int s) {  // this warp's wgmma reads of stage s are complete
+      if (lane == 0) {
+        mbar_arrive(&empty_bar[s]);
+        if (MCAST) mbar_arrive_cluster(peer_empty + 8u * s);
+      }
+    };
     for (SegIter seg(p.sk_tiles, total_super, kblocks, cluster_id, num_clusters); seg.next();) {
+      float acc[BN / 2];
+      {
+        int prev = -1;
+        for (int kb = seg.kb0; kb < seg.kb1; ++kb) {
+          mbar_wait(&full_bar[kstage], kphase);
+          const uint32_t a_addr = smem_u32(smem + kstage * Cfg::STAGE_BYTES) + grp * 64 * 128;
+          const uint32_t b_addr = smem_u32(smem + kstage * Cfg::STAGE_BYTES + Cfg::A_BYTES);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < 4; ++k)  // a piece starts from zero
+            wgmma_ss(acc, make_wgmma_desc_sw128(a_addr + k * 32, 16, 1024), make_wgmma_desc_sw128(b_addr + k * 32, 16, 1024),
+                     (kb != seg.kb0 || k != 0) ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<1>();  // the previous k-block's MMAs are done: its stage goes back to the producer(s)
+          wgmma_fence_operands(acc);
+          if (prev >= 0) release(prev);
+          prev = kstage;
+          if (++kstage == STAGES) kstage = 0, kphase ^= 1;
+        }
+        wgmma_wait<0>();
+        wgmma_fence_operands(acc);
+        release(prev);
+      }
+
       const int st = seg.st;
       const int seg_mode = seg.mode();
       // stream-K pieces: the tail piece (my first) goes to MY workspace slot; the head piece (my last) is completed with
@@ -647,8 +615,7 @@ __global__ void __launch_bounds__(320, 1)
         rm.r16[s4] = __shfl_sync(0xffffffffu, static_cast<uint32_t>(r_off >> 3), src);
         rm.valid |= (__shfl_sync(0xffffffffu, valid ? 1u : 0u, src) & 1u) << s4;
       }
-      // this warp's bias values (its <= 4 chunks of the tile) go to shared memory while the mainloop still runs: read
-      // back as broadcast float4s they cost ~30 cycles per chunk instead of an L2 round trip (L1 does not keep them).
+      // this warp's bias values (its <= 4 chunks of the tile) go to shared memory, read back as broadcast float4s.
       // Folded LayerNorm (consumer side): y = rstd * (acc - mean * colsum[n]) + bias'[n] needs the column sums the same
       // way plus this row's fixed-point totals. ALL of these loads are issued before any of them is consumed, so a tile's
       // preparation costs one L2 round trip, not three.
@@ -668,7 +635,7 @@ __global__ void __launch_bounds__(320, 1)
           const int col = n0 + (wg + 2 * i) * 32 + lane;
           cs_r[i] = (wg + 2 * i < BN / 32 && col < p.N) ? __ldg(p.ln_colsum + col) : 0.0f;
         }
-        if (LN_PROBE != 1) t_stats = __ldg(reinterpret_cast<const longlong2*>(p.ln_stats) + (valid ? gm : 0ll));
+        t_stats = __ldg(reinterpret_cast<const longlong2*>(p.ln_stats) + (valid ? gm : 0ll));
       }
       if (p.bias) {
 #pragma unroll
@@ -680,27 +647,18 @@ __global__ void __launch_bounds__(320, 1)
       }
       __syncwarp();
       float ln_rstd = 1.0f, ln_shift = 0.0f;
-      if (LNM == LNM_CONSUMER && LN_PROBE != 1) {  // mean / rstd of my row from the totals the producing GEMM's epilogues accumulated
-        // fp32 on purpose: ~10 FP64 instructions per thread and tile cost the 1280-deep GEMMs 12 % (tools/ln_fold_probe.py,
-        // profiles/r02_ln_fold_probe.txt). E[x^2] - mean^2 in fp32 is good to ~1e-7 * mean^2 / var relative: below the bf16
-        // resolution of the inputs themselves for any row bf16 can represent (|mean| / std < 2^8).
+      if (LNM == LNM_CONSUMER) {  // mean / rstd of my row from the totals the producing GEMM's epilogues accumulated
+        // fp32 on purpose (FP64 is slow on the epilogue's critical path). E[x^2] - mean^2 in fp32 is good to
+        // ~1e-7 * mean^2 / var relative: below the bf16 resolution of the inputs themselves for any row bf16 can
+        // represent (|mean| / std < 2^8).
         const float mean = p.ln_rms ? 0.0f : __ll2float_rn(t_stats.x) * p.ln_inv_k;
         const float var = fmaxf(fmaf(-mean, mean, __ll2float_rn(t_stats.y) * p.ln_inv_k), 0.0f);
         ln_rstd = rsqrtf(var + p.ln_eps);
         ln_shift = -ln_rstd * mean;
       }
       uint64_t st_acc[2] = {0ull, 0ull};  // producer side: packed (even, odd column) sum / sum of squares of my row over my chunks
-      // residual pieces are fetched one chunk ahead (the first chunk's even before the accumulators are ready), so
-      // their L2 latency overlaps the previous chunk's work instead of sitting on the critical path of each chunk
-#ifndef EPI_PIPE
-#define EPI_PIPE 0  // measured: prefetching the residual a chunk ahead costs ~2% (register pressure), keep it off
-#endif
       uint4 res_cur[4];
       bool st_cur = staged_ok && n0 + wg * 32 + 32 <= p.N;
-      if (EPI_PIPE && st_cur) epilogue_prefetch_staged(p, res_cur, rm, lane, n0 + wg * 32);
-      mbar_wait(&tfull[as], aphase);
-      tc_fence_after();
-      const uint32_t t_addr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * Cfg::ACC_STRIDE;
       if (seg_mode == SEG_HEAD) {
         // the partner's partial was published ~a tile ago; a bounded spin (2^35 cycles, ~18 s: far beyond any time slice
         // the context can lose) turns a scheduling accident (the partner cluster never resident) into an error instead
@@ -711,78 +669,77 @@ __global__ void __launch_bounds__(320, 1)
           if (clock64() - t_start > (1ll << 35)) __trap();
         }
       }
-#pragma unroll 1
-      for (int c = wg; c < BN / 32; c += 2) {
+      const int l4 = lane >> 2, lm = lane & 3;
+#pragma unroll
+      for (int i = 0; i < (BN + 63) / 64; ++i) {
+        // columns [64 i, 64 i + 64) of the warpgroup's 64 rows: fragments -> shared memory -> one row per thread
+        named_bar_sync(2 + grp, 128);  // the previous pair of chunks has been read
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int j = 8 * i + jj;  // n8 block of the accumulator fragment
+          if (j < BN / 8) {
+            float* d0 = sacc + (w * 16 + l4) * Cfg::ACC_LD + jj * 8 + 2 * lm;
+            *reinterpret_cast<float2*>(d0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+            *reinterpret_cast<float2*>(d0 + 8 * Cfg::ACC_LD) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+          }
+        }
+        named_bar_sync(2 + grp, 128);
+        const int c = 2 * i + wg;
+        if (c >= BN / 32) continue;
         uint32_t r[32];
-        tmem_ld_32x32b_x32(t_addr + c * 32, r);
+        {
+          const float4* src = reinterpret_cast<const float4*>(sacc + (32 * (w & 1) + lane) * Cfg::ACC_LD + wg * 32);
+#pragma unroll
+          for (int t = 0; t < 8; ++t) {
+            const float4 v4 = src[t];
+            r[4 * t] = __float_as_uint(v4.x), r[4 * t + 1] = __float_as_uint(v4.y);
+            r[4 * t + 2] = __float_as_uint(v4.z), r[4 * t + 3] = __float_as_uint(v4.w);
+          }
+        }
         const int n_abs = n0 + c * 32;
         if (seg_mode == SEG_TAIL) {  // partial accumulators -> workspace (512 contiguous bytes per warp and store)
-          tmem_wait_ld();
 #pragma unroll
           for (int j = 0; j < 8; ++j)
             __stcg(sk_ws + (c * 8 + j) * 128, make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]),
                                                           __uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3])));
           continue;
         }
-        float4 part[8];
         if (seg_mode == SEG_HEAD) {
 #pragma unroll
-          for (int j = 0; j < 8; ++j) part[j] = __ldcg(sk_ws + (c * 8 + j) * 128);
-          tmem_wait_ld();
-#pragma unroll
           for (int j = 0; j < 8; ++j) {
-            r[4 * j + 0] = __float_as_uint(__uint_as_float(r[4 * j + 0]) + part[j].x);
-            r[4 * j + 1] = __float_as_uint(__uint_as_float(r[4 * j + 1]) + part[j].y);
-            r[4 * j + 2] = __float_as_uint(__uint_as_float(r[4 * j + 2]) + part[j].z);
-            r[4 * j + 3] = __float_as_uint(__uint_as_float(r[4 * j + 3]) + part[j].w);
+            const float4 part = __ldcg(sk_ws + (c * 8 + j) * 128);
+            r[4 * j + 0] = __float_as_uint(__uint_as_float(r[4 * j + 0]) + part.x);
+            r[4 * j + 1] = __float_as_uint(__uint_as_float(r[4 * j + 1]) + part.y);
+            r[4 * j + 2] = __float_as_uint(__uint_as_float(r[4 * j + 2]) + part.z);
+            r[4 * j + 3] = __float_as_uint(__uint_as_float(r[4 * j + 3]) + part.w);
           }
         }
-        if (LNM == LNM_CONSUMER && LN_PROBE != 2) {
-          tmem_wait_ld();
+        if (LNM == LNM_CONSUMER) {
           const float4* c4 = reinterpret_cast<const float4*>(colsum_s + (c >> 1) * 32);
           const uint64_t rstd2 = pack_f32x2(ln_rstd, ln_rstd), shift2 = pack_f32x2(ln_shift, ln_shift);
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             const float4 cs = c4[j];
-            float a, b;
+            float a, bb;
             unpack_f32x2(ffma2(pack_f32x2(__uint_as_float(r[4 * j + 0]), __uint_as_float(r[4 * j + 1])), rstd2,
-                               fmul2(shift2, pack_f32x2(cs.x, cs.y))), a, b);
-            r[4 * j + 0] = __float_as_uint(a), r[4 * j + 1] = __float_as_uint(b);
+                               fmul2(shift2, pack_f32x2(cs.x, cs.y))), a, bb);
+            r[4 * j + 0] = __float_as_uint(a), r[4 * j + 1] = __float_as_uint(bb);
             unpack_f32x2(ffma2(pack_f32x2(__uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3])), rstd2,
-                               fmul2(shift2, pack_f32x2(cs.z, cs.w))), a, b);
-            r[4 * j + 2] = __float_as_uint(a), r[4 * j + 3] = __float_as_uint(b);
+                               fmul2(shift2, pack_f32x2(cs.z, cs.w))), a, bb);
+            r[4 * j + 2] = __float_as_uint(a), r[4 * j + 3] = __float_as_uint(bb);
           }
         }
         if (st_cur) {  // warp-uniform: coalesced path through the transpose buffer
-#if EPI_PIPE
-          uint4 res_next[4];
-          const bool st_next = (c + 2 < BN / 32) && (n_abs + 96 <= p.N);
-          if (st_next) epilogue_prefetch_staged(p, res_next, rm, lane, n_abs + 64);
-          tmem_wait_ld();
-          epilogue_chunk_staged<LNM == LNM_PRODUCER>(p, ac, r, res_cur, bias_s + (c >> 1) * 32, rm, stage, lane, g, n_abs, st_acc);
-#pragma unroll
-          for (int s4 = 0; s4 < 4; ++s4) res_cur[s4] = res_next[s4];
-          st_cur = st_next;
-#else
           epilogue_prefetch_staged(p, res_cur, rm, lane, n_abs);
-          tmem_wait_ld();
           epilogue_chunk_staged<LNM == LNM_PRODUCER>(p, ac, r, res_cur, bias_s + (c >> 1) * 32, rm, stage, lane, g, n_abs, st_acc);
           st_cur = (c + 2 < BN / 32) && (n_abs + 96 <= p.N);
-#endif
         } else {
-          // global operands of this chunk are requested before the TMEM load is waited for, so their latency overlaps
           const bool active = valid && n_abs < p.N;
           EpiOperands eo;
           if (active) epilogue_prefetch(p, eo, bias_s + (c >> 1) * 32, n_abs);
-          tmem_wait_ld();
           if (active) epilogue_chunk(p, ac, r, eo, c_off, r_off, g, n_abs);
         }
       }
-      tc_fence_before();
-      if (PAIR) mbar_arrive_cluster(mapa_smem(&tempty[as], 0));
-      else mbar_arrive(&tempty[as]);
-      as ^= 1;
-      if (as == 0) aphase ^= 1;
       if (LNM == LNM_PRODUCER && seg_mode != SEG_TAIL && valid) {
         // 2^24 fixed point: integer adds commute, so the row totals are the same bits whatever order the tiles finish in
         float s0, s1, q0, q1;
@@ -793,7 +750,7 @@ __global__ void __launch_bounds__(320, 1)
         atomicAdd(dst + 1, static_cast<unsigned long long>(__float2ll_rn((q0 + q1) * 16777216.0f)));
       }
       if (seg_mode != SEG_FULL) {
-        // tail: all 256 epilogue threads' partials are visible device-wide before the flag goes up;
+        // tail: all 256 consumer threads' partials are visible device-wide before the flag goes up;
         // head: everybody has read the partial before the flag is lowered for the next launch
         if (seg_mode == SEG_TAIL) __threadfence();
         named_bar_sync(1, 256);
@@ -805,14 +762,8 @@ __global__ void __launch_bounds__(320, 1)
     }
   }
 
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();  // the peer may still multicast into my smem / arrive on my barriers until it is done too
-  if (warp == IG_WARP_MMA) {
-    tc_fence_after();
-    if (PAIR) tmem_dealloc_pair<Cfg::TMEM_COLS>(tmem_base);
-    else tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-  }
+  if (MCAST) cluster_sync_all();  // the peer may still multicast into my smem / arrive on my barriers until it is done too
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1040,14 +991,13 @@ static int g_streamk = [] {
   const char* e = getenv("B200MIX_STREAMK");
   return e ? atoi(e) : GEMM_STREAMK_DEFAULT;
 }();
-// A split tile sends its 256 KB of fp32 partials through L2 twice; a tile's own operand traffic is 32 KB per k-block.
-// Measured on the SDXL step (profiles/r02_streamk_ab.txt): 180 k-blocks (conv 8192 x 1280 x 11520) +10.6 %, 360 +11.5 %,
-// 80 (FF2, K = 5120) +2 %, 20 (the 1280-wide projections, already bound by the L2 -> SM operand fill) -20 %.
+// A split tile sends its 256 KB of fp32 partials through L2 twice; a tile's own operand traffic is 32 KB per k-block, so
+// only deep reductions (>= 64 k-blocks: the 3x3 convs and FF2 of the SDXL step) are split.
 constexpr int SK_MIN_KBLOCKS = 64;
 constexpr int SK_MAX_CLUSTERS = 74;
 static int sk_min_kblocks() { return g_streamk >= 2 ? 8 : SK_MIN_KBLOCKS; }  // 2 = tests: split shallow reductions too
 
-// Stream-K workspaces: SK_POOL slots per device (19 MB of partial accumulators + 148 flags each), allocated together on
+// Stream-K workspaces: SK_POOL slots per device (19 MB of partial accumulators + 148 flags each, sized for up to 74 clusters of 2 CTAs), allocated together on
 // the first eager GEMM call (never inside a stream capture). A slot belongs to ONE stream: launches on a stream are
 // ordered (a kernel's first global access follows griddepcontrol.wait = completion of its predecessor), so they can
 // share it; kernels captured into a CUDA graph keep the slot of their capture stream. Streams beyond the pool, and
@@ -1107,14 +1057,14 @@ static bool sk_workspace(cudaStream_t stream, float4** ws, unsigned int** flags)
   return true;
 }
 
-template <int BN, int STAGES, bool PAIR, int LNM>
+template <int BN, int STAGES, bool MCAST, int LNM>
 static int launch_igemm_mode(const CUtensorMap& tmA, const CUtensorMap& tmB, IGemmParams p, cudaStream_t stream) {
-  using Cfg = IGemmCfg<BN, PAIR>;
-  constexpr int smem_bytes = STAGES * Cfg::STAGE_BYTES + 1024 + 256 + 8 * 2048 + 2 * 8 * 512;  // + epilogue transpose / bias / colsum
+  using Cfg = IGemmCfg<BN>;
+  constexpr int smem_bytes = STAGES * Cfg::STAGE_BYTES + Cfg::EXTRA_BYTES;
   static_assert(smem_bytes <= 227 * 1024, "stage count does not fit shared memory");
   static bool configured = false;
   if (!configured) {
-    B200_CUDA(cudaFuncSetAttribute(igemm_kernel<BN, STAGES, PAIR, LNM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    B200_CUDA(cudaFuncSetAttribute(igemm_kernel<BN, STAGES, MCAST, LNM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                    smem_bytes));
     configured = true;
   }
@@ -1129,44 +1079,41 @@ static int launch_igemm_mode(const CUtensorMap& tmA, const CUtensorMap& tmB, IGe
   if (g_streamk && rem != 0 && total_super > clusters && clusters <= SK_MAX_CLUSTERS &&
       p.ntaps * p.kchunks >= sk_min_kblocks() && sk_workspace(stream, &p.sk_ws, &p.sk_flags))
     p.sk_tiles = clusters + rem;
-  B200_CUDA(launch_pdl(igemm_kernel<BN, STAGES, PAIR, LNM>, dim3(2 * clusters), dim3(320), smem_bytes, stream, 2, tmA, tmB,
-                       p));
+  B200_CUDA(launch_pdl(igemm_kernel<BN, STAGES, MCAST, LNM>, dim3(2 * clusters), dim3(IG_THREADS), smem_bytes, stream,
+                       MCAST ? 2 : 1, tmA, tmB, p));
   return 0;
 }
 
-template <int BN, int STAGES, bool PAIR>
+template <int BN, int STAGES, bool MCAST>
 static int launch_igemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const IGemmParams& p, cudaStream_t stream) {
   if (p.ln_stats && p.stats_out) {
     set_error("one GEMM cannot both consume and produce row statistics");
     return B200MIX_ERR_INVALID;
   }
   if (p.ln_stats || p.stats_out) {
-    if constexpr (PAIR) {
+    if constexpr (MCAST) {
       return p.ln_stats ? launch_igemm_mode<BN, STAGES, true, LNM_CONSUMER>(tmA, tmB, p, stream)
                         : launch_igemm_mode<BN, STAGES, true, LNM_PRODUCER>(tmA, tmB, p, stream);
     } else {
-      set_error("the folded-LayerNorm epilogues are built for the CTA-pair kernel only");
+      set_error("the folded-LayerNorm epilogues are built for the multicast kernel only");
       return B200MIX_ERR_INVALID;
     }
   }
-  return launch_igemm_mode<BN, STAGES, PAIR, LNM_NONE>(tmA, tmB, p, stream);
+  return launch_igemm_mode<BN, STAGES, MCAST, LNM_NONE>(tmA, tmB, p, stream);
 }
 
-// Test / measurement hook (see b200mix_debug_gemm_pair): 1 = CTA-pair MMA (default), 0 = per-CTA MMA + multicast B.
-#ifndef GEMM_PAIR_DEFAULT
-#define GEMM_PAIR_DEFAULT 1
-#endif
-static int g_gemm_pair = GEMM_PAIR_DEFAULT;
+// Test / measurement hook (see b200mix_debug_gemm_pair): 1 = CTA pairs sharing the B tile through TMA multicast
+// (default), 0 = independent CTAs, each loading its own B tile.
+static int g_gemm_pair = 1;
 
 static int pick_bn(long long tiles_m, long long N, int kblocks) {
-  // cost = waves x time per tile; time per tile ~ BN / rate(BN). Rates are the measured mainloop rates of each tile
-  // width relative to BN=256 in CTA-pair mode (tools/bn_sweep.py, 16384x8192x2048): the per-SM operand fill (A tile +
-  // B half per k-chunk, ~60 B/clk) does not shrink with BN as fast as the MMA time does, so narrower tiles are only
-  // chosen when they avoid wave / N-padding waste. (Round 1's table, 1541 / 1448 / 1331 / 1202 / 1032 / 530 / 270, was
-  // dominated by the ~80-cycle election loop the compiler put around every MMA issued from an `if (lane == 0)` region.)
+  // cost = waves x time per tile; time per tile ~ BN / rate(BN). The relative rates follow the operand traffic of a
+  // 128 x BN tile (A tile + half a B tile per k-block and CTA, shared through multicast): per MAC it is proportional to
+  // (128 + BN/2) / (128 BN), so narrower tiles are only chosen when they avoid wave / N-padding waste. A model, not a
+  // measurement: eff = (128 BN / (128 + BN/2)) normalised to BN = 256.
   const int cands[7] = {256, 224, 192, 160, 128, 64, 32};
-  // round 2 (converged-warp MMA / TMA issue): 1617 / 1595 / 1559 / 1443 / 1337 / 780 / 405 TFLOP/s (profiles/r02_bn_sweep.txt)
-  const double eff[7] = {1.00, 0.985, 0.96, 0.89, 0.825, 0.48, 0.25};
+  double eff[7];
+  for (int i = 0; i < 7; ++i) eff[i] = (128.0 * cands[i] / (128.0 + cands[i] / 2.0)) / (128.0 * 256 / (128.0 + 128.0));
   double best = 1e30;
   int best_bn = 256;
   const int clusters = num_sms() / 2;
@@ -1193,29 +1140,30 @@ static int dispatch_igemm(const CUtensorMap& tmA, const void* W, long long ldw, 
   {
     uint64_t dims[2] = {(uint64_t)Ktot, (uint64_t)p.N};
     uint64_t strides[1] = {(uint64_t)ldw * 2};
-    uint32_t box[2] = {64, (uint32_t)(bn / 2)};  // each CTA of the cluster loads (and multicasts) one half
+    uint32_t box[2] = {64, (uint32_t)(bn / 2)};  // the B tile is loaded in two halves (one per CTA of a cluster)
     int rc = encode_tmap_bf16_sw128(&tmB, W, 2, dims, strides, box);
     if (rc) return rc;
   }
-  if (g_gemm_pair) {  // one 256 x BN MMA per CTA pair (the default)
+  // stage counts: as many as fit next to the epilogue buffers (IGemmCfg::EXTRA_BYTES) in 227 KB
+  if (g_gemm_pair) {
     switch (bn) {
-      case 256: return launch_igemm<256, 6, true>(tmA, tmB, p, stream);
-      case 224: return launch_igemm<224, 6, true>(tmA, tmB, p, stream);
-      case 192: return launch_igemm<192, 7, true>(tmA, tmB, p, stream);
-      case 160: return launch_igemm<160, 7, true>(tmA, tmB, p, stream);
-      case 128: return launch_igemm<128, 8, true>(tmA, tmB, p, stream);
-      case 64: return launch_igemm<64, 8, true>(tmA, tmB, p, stream);
+      case 256: return launch_igemm<256, 3, true>(tmA, tmB, p, stream);
+      case 224: return launch_igemm<224, 3, true>(tmA, tmB, p, stream);
+      case 192: return launch_igemm<192, 4, true>(tmA, tmB, p, stream);
+      case 160: return launch_igemm<160, 4, true>(tmA, tmB, p, stream);
+      case 128: return launch_igemm<128, 5, true>(tmA, tmB, p, stream);
+      case 64: return launch_igemm<64, 6, true>(tmA, tmB, p, stream);
       case 32: return launch_igemm<32, 8, true>(tmA, tmB, p, stream);
       default: set_error("unsupported BN %d", bn); return B200MIX_ERR_INVALID;
     }
   }
-  switch (bn) {  // two 128 x BN MMAs per cluster with a multicast B tile (kept for A/B measurements)
-    case 256: return launch_igemm<256, 4, false>(tmA, tmB, p, stream);
-    case 224: return launch_igemm<224, 4, false>(tmA, tmB, p, stream);
-    case 192: return launch_igemm<192, 5, false>(tmA, tmB, p, stream);
-    case 160: return launch_igemm<160, 5, false>(tmA, tmB, p, stream);
-    case 128: return launch_igemm<128, 6, false>(tmA, tmB, p, stream);
-    case 64: return launch_igemm<64, 8, false>(tmA, tmB, p, stream);
+  switch (bn) {
+    case 256: return launch_igemm<256, 3, false>(tmA, tmB, p, stream);
+    case 224: return launch_igemm<224, 3, false>(tmA, tmB, p, stream);
+    case 192: return launch_igemm<192, 4, false>(tmA, tmB, p, stream);
+    case 160: return launch_igemm<160, 4, false>(tmA, tmB, p, stream);
+    case 128: return launch_igemm<128, 5, false>(tmA, tmB, p, stream);
+    case 64: return launch_igemm<64, 6, false>(tmA, tmB, p, stream);
     case 32: return launch_igemm<32, 8, false>(tmA, tmB, p, stream);
     default: set_error("unsupported BN %d", bn); return B200MIX_ERR_INVALID;
   }

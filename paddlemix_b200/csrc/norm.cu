@@ -37,7 +37,7 @@ __device__ __forceinline__ float silu_f(float x) {
 // sum of squares: 2^16) so that the cross-CTA reduction is integer adds: exact, order-independent (bit-reproducible
 // without atomics-ordering concerns) and off the FP64 pipe. The first version kept the partials in double; on this
 // part ~100 dependent DADDs per CTA (one warp, one group per lane) cost more than streaming the CTA's pixels
-// (tools/ln_fold_probe.py measured ~40 cycles per warp-level FP64 instruction). Only the last three operations per
+// (FP64 issues at a fraction of the FP32 rate). Only the last three operations per
 // group (mean, variance from the int64 totals) are double. Block = PPB pixels x CV 8-channel vectors; each thread owns
 // a fixed channel vector, so every row is read with fully coalesced 16-byte loads.
 // ------------------------------------------------------------------------------------------------------------
@@ -138,8 +138,7 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x1, int C1, co
   long long su = 0, sq = 0;
   if (g < groups) {
     // L2 loads (the partials were published with __threadfence + the arrival counter), several in flight: a volatile
-    // loop here serialised ~28 L2 round trips and was half of the kernel's 15 us on the small slices (ncu: SMs active
-    // 49 % of the elapsed cycles, profiles/r02_ncu_full_norm.txt)
+    // loop here would serialise one L2 round trip per partial
     const longlong2* srcp = reinterpret_cast<const longlong2*>(partial + (static_cast<long long>(b) * gx * groups + g) * 2);
 #pragma unroll 4
     for (int i = j; i < gx; i += per) {
@@ -476,7 +475,7 @@ extern "C" int b200mix_groupnorm_nhwc(const void* x1, int64_t C1, const void* x2
 
 // Row softmax y = softmax(x * scale) for fp32 scores [M, N] -> bf16 probabilities: the attention of the VAE decoder's
 // mid block (ONE 512-wide head over H*W tokens, ppdiffusers/models/vae.py:232-241, attention_processor.py:673-735 with
-// upcast_softmax) runs as two GEMMs around this kernel because a 512-wide head does not fit the flash kernels' TMEM /
+// upcast_softmax) runs as two GEMMs around this kernel because a 512-wide head does not fit the flash kernel's register /
 // shared-memory budget. One CTA per row; the row is staged in shared memory (read once), fp32 math, exp2.
 __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y,
                                                           long long N, long long ldx, long long ldy, float scale_log2) {

@@ -1,4 +1,4 @@
-"""LLaVA on the sm_100a kernels: the Llama decoder prefill (PaddleNLP/paddlenlp/transformers/llama/modeling.py: RMSNorm
+"""LLaVA on the sm_90a kernels: the Llama decoder prefill (PaddleNLP/paddlenlp/transformers/llama/modeling.py: RMSNorm
 :386-420, rotary :534-555, attention :197-330, decoder layers, lm head) and the LLaVA composition around it
 (paddlemix/models/llava/modeling.py:47-120, base_model.py:136-330): CLIP vision tower -> feature_select
 (clip_encoder.py:49-57) -> mm_projector mlp2x_gelu (mm_projector.py:45-58) -> image features spliced in place of each

@@ -1,5 +1,5 @@
 """STDiT2 — host-side mirror of ppdiffusers/examples/Open-Sora/models/stdit/stdit2.py (STDiT2.forward :334-448,
-STDiT2Block.forward :119-191) on sm_100a kernels; inference path (x_mask = None).
+STDiT2Block.forward :119-191) on sm_90a kernels; inference path (x_mask = None).
 
 Device graph per block (tokens are [B, T*S, D] with row = (b*T + t)*S + s, never transposed):
   LN+modulate (one kernel) -> spatial qkv GEMM -> [q/k RMSNorm per head] -> flash attention over S per (b, t)

@@ -1,5 +1,5 @@
 """Tensor-level wrappers over the C ABI. torch is used for device memory and streams only: every function below
-enqueues hand-written sm_100a kernels from libb200mix.so on torch's current CUDA stream and raises if that fails.
+enqueues hand-written sm_90a kernels from libb200mix.so on torch's current CUDA stream and raises if that fails.
 """
 import ctypes
 from typing import Optional

@@ -1,4 +1,4 @@
-"""AutoencoderKL.decode on the sm_100a kernels — host-side mirror of ppdiffusers/models/autoencoder_kl.py:288-325 and
+"""AutoencoderKL.decode on the sm_90a kernels — host-side mirror of ppdiffusers/models/autoencoder_kl.py:288-325 and
 vae.py:182-282 (Decoder), the step that turns the denoising loop's latents into pixels
 (pipeline_stable_diffusion.py:910-917; SURVEY.md §8 f2).
 
@@ -7,7 +7,7 @@ conv_in (tiny-Cin kernel) -> mid block: ResnetBlock2D (GroupNorm+SiLU -> conv3x3
 one-head attention over H*W tokens, ResnetBlock2D -> 4 x UpDecoderBlock2D (3 resnets each, 1x1 shortcut GEMM where the
 width changes, nearest x2 + conv3x3) -> GroupNorm+SiLU -> conv_out -> NCHW fp32.
 The mid attention has ONE 512-wide head: it runs as score GEMM (fp32 out) -> row softmax kernel -> PV GEMM per image
-(a 512-wide head does not fit the flash kernels' TMEM / shared-memory budget; at 128x128 latents the score matrix is
+(a 512-wide head does not fit the flash kernel's register / shared-memory budget; at 128x128 latents the score matrix is
 16384^2 fp32 = 1 GB of scratch that is reused across the batch).
 """
 from dataclasses import dataclass

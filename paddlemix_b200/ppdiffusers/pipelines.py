@@ -1,7 +1,7 @@
 """The denoising loops of StableDiffusionPipeline / StableDiffusionXLPipeline / StableDiffusion3Pipeline
 (ppdiffusers/pipelines/stable_diffusion/pipeline_stable_diffusion.py:858-908,
  ppdiffusers/pipelines/stable_diffusion_xl/pipeline_stable_diffusion_xl.py:1040-1082,
- ppdiffusers/pipelines/stable_diffusion_3/pipeline_stable_diffusion_3.py:794-866) on the B200-native denoisers.
+ ppdiffusers/pipelines/stable_diffusion_3/pipeline_stable_diffusion_3.py:794-866) on the H100-native denoisers.
 
 Text encoders and the VAE run before / after the loop and are out of scope (SURVEY.md §8f): the pipelines here take
 `prompt_embeds` (and `negative_prompt_embeds`) exactly as the reference pipelines accept them and return latents

@@ -1,5 +1,5 @@
 """SD3Transformer2DModel — host-side mirror of ppdiffusers.models.transformer_sd3.SD3Transformer2DModel
-(ppdiffusers/models/transformer_sd3.py:44-122 constructor, :279-287 forward signature) on sm_100a kernels.
+(ppdiffusers/models/transformer_sd3.py:44-122 constructor, :279-287 forward signature) on sm_90a kernels.
 
 The reference offers two block stacks: 24 x JointTransformerBlock (attention.py:96-214) and its own fused
 replacement SimplifiedSD3 (simplified_sd3.py:43-160, Triton ops). This graph goes further along the same lines:

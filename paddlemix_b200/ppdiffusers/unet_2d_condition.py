@@ -1,11 +1,11 @@
 """UNet2DConditionModel — host-side mirror of ppdiffusers.models.unet_2d_condition.UNet2DConditionModel
 (ppdiffusers/models/unet_2d_condition.py:172-228 constructor arguments, :809-824 forward signature) whose forward
-runs entirely on hand-written sm_100a kernels through the C ABI (paddlemix_b200.ops).
+runs entirely on hand-written sm_90a kernels through the C ABI (paddlemix_b200.ops).
 
-Data layout on the device (B200-first, not the reference's NCHW nn.Layer graph):
+Data layout on the device (H100-first, not the reference's NCHW nn.Layer graph):
   * activations are NHWC bf16 end to end (the reference's own data_format="NHWC" switch makes this API-legal);
     [B,H,W,C] doubles as the [B*H*W, C] token matrix, so Transformer2DModel's two transposes disappear;
-  * every Linear / 1x1 conv / conv3x3 is one launch of the tcgen05 implicit-GEMM kernel with a fused epilogue
+  * every Linear / 1x1 conv / conv3x3 is one launch of the wgmma implicit-GEMM kernel with a fused epilogue
     (bias, temb broadcast, GEGLU, residual add);  q,k,v are one fused projection, cross-attention K/V of all blocks
     are one batched GEMM per forward; all resnet time_emb_proj layers are one batched GEMM per forward;
   * the skip-connection concat is never materialised: GroupNorm reads both sources, the 1x1 shortcut is two
@@ -62,7 +62,7 @@ def _pad_head(d):
     for p in (64, 128, 192):
         if d <= p:
             return p
-    raise ValueError(f"attention head size {d} > 192 is not supported by the sm_100a attention kernel")
+    raise ValueError(f"attention head size {d} > 192 is not supported by the sm_90a attention kernel")
 
 
 def _to_t(x):

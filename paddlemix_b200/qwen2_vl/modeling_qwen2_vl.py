@@ -1,5 +1,5 @@
 """Qwen2VLForConditionalGeneration — host-side mirror of paddlemix/models/qwen2_vl/modeling_qwen2_vl.py for the
-PREFILL path (forward signature :1382-1399; logits over all positions in fp32, :1474-1475) on sm_100a kernels.
+PREFILL path (forward signature :1382-1399; logits over all positions in fp32, :1474-1475) on sm_90a kernels.
 
 Device graph (one process per GPU, every arithmetic op is a libb200mix kernel):
   ViT (:916-986): PatchEmbed Conv3D == GEMM [T,1176]x[1176,E]; 32 x { LayerNorm -> fused qkv GEMM (+bias) -> 2-D RoPE

@@ -53,7 +53,7 @@ def ref_sdpa(q, k, v, scale, mask=None, kv_lens=None):
     (1, 64, 200, 8, 8),       # fewer query rows than one tile
     (1, 4250, 4250, 2, 2),    # SD3: 4096 image + 154 text tokens
     (2, 640, 1300, 6, 2),     # GQA, Sq != Sk
-    (2, 4096, 4096, 10, 10),  # SDXL top level: 320 items on 148 CTAs (persistent loop, Q ring reuse)
+    (2, 4096, 4096, 10, 10),  # SDXL top level
     (8, 1024, 1024, 20, 20),  # SDXL 32x32 level (the benched shape)
 ])
 def test_pingpong_matches_reference(ops, B, Sq, Sk, Hq, Hkv):
@@ -68,12 +68,12 @@ def test_pingpong_agrees_with_one_tile_kernel(ops, B, Sq, Sk, H):
     from paddlemix_b200._lib import lib
     q, k, v = rnd(B, Sq, H, 64, seed=4), rnd(B, Sk, H, 64, seed=5), rnd(B, Sk, H, 64, seed=6)
     out = ops.sdpa(q, k, v)
-    lib.b200mix_debug_attn_pingpong(0)
+    lib.b200mix_debug_attn_bn64(1)
     try:
         old = ops.sdpa(q, k, v)
     finally:
-        lib.b200mix_debug_attn_pingpong(1)
-    close(out, old, "pingpong vs attn_kernel<64>")
+        lib.b200mix_debug_attn_bn64(0)
+    close(out, old, "128-key vs 64-key blocks")
     assert torch.equal(out, ops.sdpa(q, k, v)), "the kernel must be deterministic"
 
 
@@ -120,7 +120,8 @@ def test_attn_mask(ops, kind, dtype, B, Sq, Sk, H, D, path):
     from paddlemix_b200._lib import lib
     q, k, v = rnd(B, Sq, H, D, seed=12), rnd(B, Sk, H, D, seed=13), rnd(B, Sk, H, D, seed=14)
     mask = _mask(kind, B, H, Sq, Sk, dtype)
-    hooks = {"one_tile": (lib.b200mix_debug_attn_pingpong, 0, 1), "general_short": (lib.b200mix_debug_no_shortkv, 1, 0)}
+    # one_tile / general_short: the 64-key-block configuration of the D = 64 kernel
+    hooks = {"one_tile": (lib.b200mix_debug_attn_bn64, 1, 0), "general_short": (lib.b200mix_debug_attn_bn64, 1, 0)}
     fn, on, off = hooks.get(path, (None, None, None))
     if fn:
         fn(on)
@@ -155,14 +156,12 @@ def test_kv_lens_zero_gives_zeros_and_does_not_hang(ops, D, Sk, general):
     B, Sq, H = 3, 200, 2
     q, k, v = rnd(B, Sq, H, D, seed=18), rnd(B, Sk, H, D, seed=19), rnd(B, Sk, H, D, seed=20)
     lens = [Sk, 0, 5]
-    lib.b200mix_debug_no_shortkv(1 if general else 0)
-    lib.b200mix_debug_attn_pingpong(0 if general else 1)
+    lib.b200mix_debug_attn_bn64(1 if general else 0)  # general: 64-key blocks
     try:
         out = ops.sdpa(q, k, v, kv_lens=torch.tensor(lens, dtype=torch.int32, device="cuda"))
         torch.cuda.synchronize()
     finally:
-        lib.b200mix_debug_no_shortkv(0)
-        lib.b200mix_debug_attn_pingpong(1)
+        lib.b200mix_debug_attn_bn64(0)
     assert (out[1] == 0).all()
     close(out, ref_sdpa(q, k, v, D ** -0.5, kv_lens=lens), f"kv_lens with an empty batch element D{D} Sk{Sk}")
 

@@ -13,7 +13,7 @@ tiny configurations:
 
 Stated tolerance (bf16 kernels vs fp32 oracle, every activation rounded to bf16 after each fused op): cosine >= 0.999
 and max |err| <= 4 % of the output's max magnitude -- the same bar as the tiny-config tests. Each test appends its
-(cosine, max-rel) to gpurun_out/parity_baseline.json so the numbers can be quoted (profiles/).
+(cosine, max-rel) to a JSON record (see _record) so the numbers can be quoted.
 The oracle needs 10-40 s per forward on the GPU box's host cores; marked `slow`.
 """
 import json

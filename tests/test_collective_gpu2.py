@@ -1,4 +1,4 @@
-"""The path's only collective through the C ABI, on 2 GPUs (run under `gpurun --gpus 2`): libb200mix creates its own NCCL
+"""The path's only collective through the C ABI, on 2 GPUs (needs a machine with 2 GPUs): libb200mix creates its own NCCL
 communicator (b200mix_nccl_unique_id / b200mix_comm_init) and b200mix_allgather_latents must return exactly what
 torch.distributed's all_gather returns. Spawns 2 ranks; skipped with fewer than 2 GPUs."""
 import os
@@ -37,7 +37,7 @@ print("rank", rank, "ok")
 """ % ROOT
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_allgather_latents_cabi_two_ranks(tmp_path):
     script = tmp_path / "worker.py"
     script.write_text(WORKER)

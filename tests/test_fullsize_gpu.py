@@ -37,7 +37,7 @@ def gelu_erf(x):
     return 0.5 * x * (1 + torch.erf(x * 0.7071067811865476))
 
 
-# (name, M, N, K, epilogue) of the SDXL forward's dominant Linear problems (tools/shape_profile.py)
+# (name, M, N, K, epilogue) of the SDXL forward's dominant Linear problems 
 LINEARS = [("ff1 GEGLU 1280", 8192, 10240, 1280, "geglu"), ("ff2 1280", 8192, 1280, 5120, "bias+res"),
            ("qkv 1280", 8192, 3840, 1280, "plain"), ("out 1280", 8192, 1280, 1280, "bias+res"),
            ("ff1 GEGLU 640", 32768, 5120, 640, "geglu"), ("ff2 640", 32768, 640, 2560, "bias+res"),

@@ -37,7 +37,7 @@ GEMM_RTOL, GEMM_ATOL = 1.0e-2, 2e-2
 @pytest.mark.parametrize("M,N,K", [(128, 128, 64), (256, 640, 320), (8, 1280, 320), (1000, 328, 200), (4096, 1920, 640),
                                    (77, 64, 2048), (300, 40, 1176)])
 @pytest.mark.parametrize("bn", [0, 32, 64, 128, 160, 192, 224, 256])
-@pytest.mark.parametrize("pair", [1, 0])  # 1: one 256-row MMA per CTA pair (default); 0: per-CTA MMA + multicast B
+@pytest.mark.parametrize("pair", [1, 0])  # 1: CTA pairs sharing the B tile through TMA multicast (default); 0: independent CTAs
 def test_linear_plain(ops, M, N, K, bn, pair):
     from paddlemix_b200._lib import lib
     a, w = rnd(M, K, seed=1), rnd(N, K, seed=2, scale=K ** -0.5)
@@ -54,7 +54,7 @@ def test_linear_plain(ops, M, N, K, bn, pair):
 
 
 def test_linear_persistent_many_tiles(ops):
-    M, N, K = 8192, 2560, 1280  # 64 x 10+ tiles: several tiles per CTA, both TMEM stages and all ring phases
+    M, N, K = 8192, 2560, 1280  # 64 x 10+ tiles: several tiles per CTA and all ring phases
     a, w = rnd(M, K, seed=4), rnd(N, K, seed=5, scale=K ** -0.5)
     out = ops.linear(a, w)
     ref = a.float() @ w.float().t()
@@ -70,7 +70,7 @@ def _streamk(lib, on, max_clusters=0):
 
 
 @pytest.mark.parametrize("M,N,K,clusters,bn", [
-    (8192, 1280, 1280, 0, 0),     # SDXL out-projection: 160 tile pairs on 74 clusters -> 86 stream-K tiles + 1 round
+    (8192, 1280, 1280, 0, 0),     # SDXL out-projection: 160 tile pairs on 66 clusters -> 94 stream-K tiles + 1 round
     (8192, 1280, 5120, 0, 0),     # FF2
     (2048, 512, 1024, 3, 256),    # 16 tile pairs on 3 clusters: 4 stream-K tiles, every cluster has a tail and / or a head
     (1536, 768, 576, 5, 128),     # 36 tile pairs on 5 clusters, 9 k-blocks: 6 stream-K tiles; ragged last n-tile
@@ -344,20 +344,20 @@ def test_sdpa(ops, B, Sq, Sk, Hq, Hkv, D, causal):
                                             (1, 130, 17, 3, 3), (5, 384, 96, 6, 2), (2, 256, 128, 4, 4),
                                             (1, 128, 33, 1, 1), (37, 200, 64, 9, 3)])
 def test_sdpa_short_kv_persistent(ops, B, Sq, Sk, Hq, Hkv):
-    """Sk <= 128, D = 64, non-causal takes the persistent short-KV kernel (K / V resident, Q ring, several
-    (batch, head) groups per CTA); it must agree with the general kernel and with the fp32 reference."""
+    """Sk <= 128, D = 64, non-causal (cross-attention against a short context): the default 128-key blocks (one block
+    covers every key) must agree with the 64-key-block configuration and with the fp32 reference."""
     from paddlemix_b200._lib import lib
     D = 64
     q, k, v = rnd(B, Sq, Hq, D, seed=90), rnd(B, Sk, Hkv, D, seed=91), rnd(B, Sk, Hkv, D, seed=92)
     lens = torch.tensor([max(1, Sk - 3 * b) for b in range(B)], dtype=torch.int32, device="cuda")
     for kv_lens in (None, lens):
         out = ops.sdpa(q, k, v, kv_lens=kv_lens)
-        lib.b200mix_debug_no_shortkv(1)
+        lib.b200mix_debug_attn_bn64(1)
         try:
             gen = ops.sdpa(q, k, v, kv_lens=kv_lens)
         finally:
-            lib.b200mix_debug_no_shortkv(0)
-        close(out, gen.float(), ATT_ATOL, ATT_RTOL, f"short-kv vs general B{B} Sq{Sq} Sk{Sk}")
+            lib.b200mix_debug_attn_bn64(0)
+        close(out, gen.float(), ATT_ATOL, ATT_RTOL, f"short-kv 128- vs 64-key blocks B{B} Sq{Sq} Sk{Sk}")
         for b in ([0, B - 1] if kv_lens is not None else [0]):
             n = int(lens[b]) if kv_lens is not None else Sk
             ref = ref_sdpa(q[b:b + 1], k[b:b + 1, :n], v[b:b + 1, :n], D ** -0.5)
@@ -366,7 +366,7 @@ def test_sdpa_short_kv_persistent(ops, B, Sq, Sk, Hq, Hkv):
 
 @pytest.mark.parametrize("B,Sq,Sk,H,causal", [(2, 1024, 1024, 4, False), (1, 300, 450, 3, False), (1, 333, 333, 2, True)])
 def test_sdpa_d64_64_key_blocks(ops, B, Sq, Sk, H, causal):
-    """The D = 64 kernel with 64-key blocks (3 CTAs per SM; not the default, kept for A/B runs) against the fp32 reference."""
+    """The D = 64 kernel with 64-key blocks (not the default, kept for A/B runs) against the fp32 reference."""
     from paddlemix_b200._lib import lib
     q, k, v = rnd(B, Sq, H, 64, seed=93), rnd(B, Sk, H, 64, seed=94), rnd(B, Sk, H, 64, seed=95)
     lib.b200mix_debug_attn_bn64(1)
@@ -379,17 +379,17 @@ def test_sdpa_d64_64_key_blocks(ops, B, Sq, Sk, H, causal):
 
 @pytest.mark.parametrize("B,Sq,Sk,H,causal,scale", [(2, 1024, 1024, 4, False, 1.0), (1, 300, 450, 3, False, 1.0),
                                                       (1, 333, 333, 2, True, 1.0), (1, 512, 512, 2, False, 4.0)])
-def test_sdpa_d64_p_in_tmem(ops, B, Sq, Sk, H, causal, scale):
-    """The D = 64 kernel variant that keeps P in TMEM (tcgen05.mma with the A operand in TMEM; not the default, kept
-    for A/B runs) against the fp32 reference, incl. masked tiles and the lazy-rescale path (large logits)."""
+def test_sdpa_d64_64_key_blocks_lazy_rescale(ops, B, Sq, Sk, H, causal, scale):
+    """The D = 64 kernel with 64-key blocks against the fp32 reference, incl. masked tiles and the lazy-rescale path
+    (large logits: the running max grows by more than 2^8 between blocks)."""
     from paddlemix_b200._lib import lib
     q, k, v = rnd(B, Sq, H, 64, seed=96, scale=scale), rnd(B, Sk, H, 64, seed=97, scale=scale), rnd(B, Sk, H, 64, seed=98)
-    lib.b200mix_debug_attn_ptmem(1)
+    lib.b200mix_debug_attn_bn64(1)
     try:
         out = ops.sdpa(q, k, v, causal=causal)
     finally:
-        lib.b200mix_debug_attn_ptmem(0)
-    close(out, ref_sdpa(q, k, v, 64 ** -0.5, causal), ATT_ATOL, ATT_RTOL, f"sdpa P-in-TMEM B{B} Sq{Sq} Sk{Sk} causal={causal}")
+        lib.b200mix_debug_attn_bn64(0)
+    close(out, ref_sdpa(q, k, v, 64 ** -0.5, causal), ATT_ATOL, ATT_RTOL, f"sdpa 64-key blocks B{B} Sq{Sq} Sk{Sk} causal={causal}")
 
 
 def test_sdpa_large_logits(ops):

@@ -1,4 +1,4 @@
-"""Model-level parity on the GPU: paddlemix_b200's UNet2DConditionModel (bf16, sm_100a kernels through the C ABI)
+"""Model-level parity on the GPU: paddlemix_b200's UNet2DConditionModel (bf16, sm_90a kernels through the C ABI)
 against the CPU fp32 oracle on identical seeded inputs and weights.
 
 Tolerance (stated, bf16 vs fp32): every activation is rounded to bf16 (2^-8 relative) after each of ~10^2 fused
