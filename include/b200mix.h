@@ -141,6 +141,13 @@ int b200mix_conv3x3_up2x(const void* x, const void* w4, void* y, int64_t B, int6
 int b200mix_conv3x3_small_cin(const void* x, int32_t x_fp32, const void* w, const float* bias, void* y, int64_t B,
                               int64_t H, int64_t W, int64_t Cin, int64_t Cout, void* stream);
 
+/* y[B,Ho,Wo,Cout] = act(conv3x3(x[B,H,W,Cin], w[Cout,3,3,Cin], padding 1, stride 1|2) + bias), NHWC bf16 in / out,
+ * 1 <= Cin <= 128, Cout % 8 == 0, Cout <= 256 (ControlNetConditioningEmbedding, controlnet.py:71-113). bias fp32 [Cout]
+ * or NULL; act B200MIX_ACT_NONE or B200MIX_ACT_SILU; stride 2 needs even H and W (Ho = H/2, Wo = W/2).
+ * Tensor-core implicit GEMM on mma.sync.m16n8k16 with K = 9 taps x Cin padded to 16 (csrc/conv_narrow.cu). */
+int b200mix_conv3x3_narrow(const void* x, const void* w, const float* bias, void* y, int64_t B, int64_t H, int64_t W,
+                           int64_t Cin, int64_t Cout, int32_t stride, int32_t act, void* stream);
+
 /* Scaled dot-product attention, flash-style on wgmma (S=QK^T and O+=PV in registers, online softmax in registers).
  * Full signature of scaled_dot_product_attention_(query, key, value, attn_mask, dropout_p=0, is_causal, scale)
  * (ppdiffusers/patches/paddle_patch.py:414-424), semantics of its `math` branch (:445-461):

@@ -66,6 +66,8 @@ SIGNATURES = {
                              POINTER(Epilogue), c_void_p],
     "b200mix_conv3x3_small_cin": [c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64,
                                   c_int64, c_void_p],
+    "b200mix_conv3x3_narrow": [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64,
+                               c_int32, c_int32, c_void_p],
     "b200mix_sdpa": [c_void_p, c_void_p, c_void_p, c_void_p] + [c_int64] * 6 + [c_int64] * 12 +
                     [c_float, c_int32, c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int64, c_int64, c_int64, c_void_p],
     "b200mix_groupnorm_nhwc": [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,

@@ -309,6 +309,25 @@ def conv3x3_small_cin(x: torch.Tensor, w: torch.Tensor, bias=None) -> torch.Tens
     return out
 
 
+def conv3x3_narrow(x: torch.Tensor, w: torch.Tensor, bias=None, *, stride=1, act=ACT_NONE, out=None) -> torch.Tensor:
+    """act(conv3x3(x) + bias) for 1 <= Cin <= 128 (the ControlNet conditioning embedding). x: bf16 NHWC [B,H,W,Cin]
+    contiguous; w: bf16 [Cout,3,3,Cin] contiguous; bias fp32 [Cout] or None; act ACT_NONE | ACT_SILU. Returns bf16 NHWC
+    [B,H/stride,W/stride,Cout]."""
+    _req(x, bf16, "x"), _req(w, bf16, "w")
+    B, H, W, Cin = x.shape
+    Cout = w.shape[0]
+    assert x.is_contiguous() and w.is_contiguous() and tuple(w.shape[1:]) == (3, 3, Cin)
+    if out is None:
+        out = torch.empty(B, H // stride, W // stride, Cout, device=x.device, dtype=bf16)
+    with _Timed("conv_narrow", 2.0 * B * (H // stride) * (W // stride) * Cout * 9 * Cin, "flop",
+                lambda: f"convn{stride} {B}x{H}x{W}x{Cin}->{Cout}"):
+        check(lib.b200mix_conv3x3_narrow(_p(x), _p(w), _p(None if bias is None else _req(bias, torch.float32, "bias")),
+                                         _p(out), B, H, W, Cin, Cout, int(stride), int(act), _stream()),
+              "b200mix_conv3x3_narrow")
+    _count()
+    return out
+
+
 def sdpa(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, *, scale: Optional[float] = None, causal=False,
          cu_seqlens: Optional[torch.Tensor] = None, kv_lens: Optional[torch.Tensor] = None,
          attn_mask: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:

@@ -12,10 +12,12 @@ in a device tensor) and replayed; the scheduler kernel, whose fp32 scalars chang
 Multi-GPU (data parallel over images, SURVEY.md §8e): each rank takes a contiguous slice of the batch, replicates the
 weights, runs the loop with zero per-step communication, and `all_gather`s the finished latents once over NCCL.
 """
-from typing import Any, Dict, Optional
+from types import SimpleNamespace
+from typing import Any, Dict, List, Optional, Union
 
 import torch
 
+from .controlnet import MultiControlNetModel, controlnet_keep
 from .schedulers import DDIMScheduler
 from .unet_2d_condition import UNet2DConditionModel
 
@@ -24,10 +26,15 @@ bf16 = torch.bfloat16
 
 class GraphedUNet:
     """Static-shape CUDA-graph wrapper around UNet2DConditionModel.forward_nhwc (+ NCHW<->NHWC conversion).
-    Inputs are copied into static device buffers; the timestep lives in a device tensor so it can change per replay."""
+    Inputs are copied into static device buffers; the timestep lives in a device tensor so it can change per replay.
+    With `controlnet` (a ControlNetModel or MultiControlNetModel) the graph runs the ControlNet(s) and hands their
+    residuals to the UNet; the conditioning embeddings and the fp32 scale tables are static buffers too
+    (`cond_embeddings` / `scale_tables` of __call__), so new scales need no new capture. `controlnet_rows` < rows:
+    the ControlNet runs on the last `controlnet_rows` rows only (guess mode with CFG) and the residuals of the other
+    rows stay zero."""
 
     def __init__(self, unet: UNet2DConditionModel, sample_shape, ctx_shape, added_cond_shapes: Optional[Dict[str, Any]] = None,
-                 warmup: int = 2):
+                 warmup: int = 2, controlnet=None, controlnet_rows: Optional[int] = None):
         from .. import ops
         dev = unet.device
         self.unet = unet
@@ -38,12 +45,18 @@ class GraphedUNet:
         if added_cond_shapes:
             self.added = {k: torch.zeros(s, device=dev, dtype=(bf16 if k == "text_embeds" else torch.float32))
                           for k, s in added_cond_shapes.items()}
+        self.cn = None
+        if controlnet is not None:
+            self.cn = controlnet_state(controlnet, sample_shape, controlnet_rows or sample_shape[0], dev)
         self.out = None
         self.launches_per_replay = 0
 
         def run():
             x = ops.nchw_to_nhwc(self.sample)
-            y = unet.forward_nhwc(x, self.t, self.ctx, self.added)
+            if controlnet is None:
+                y = unet.forward_nhwc(x, self.t, self.ctx, self.added)
+            else:
+                y = denoise_with_controlnet(unet, controlnet, x, self.t, self.ctx, self.added, self.cn)
             return ops.nhwc_to_nchw(y, out_dtype=bf16)
 
         s = torch.cuda.Stream(device=dev)
@@ -59,7 +72,7 @@ class GraphedUNet:
             self.out = run()
         self.launches_per_replay = ops.launches() - n0
 
-    def __call__(self, sample, timestep, ctx=None, added_cond_kwargs=None):
+    def __call__(self, sample, timestep, ctx=None, added_cond_kwargs=None, cond_embeddings=None, scale_tables=None):
         from .. import ops
         self.sample.copy_(sample, non_blocking=True)
         if ctx is not None:
@@ -71,9 +84,51 @@ class GraphedUNet:
         if added_cond_kwargs is not None and self.added is not None:
             for k, v in added_cond_kwargs.items():
                 self.added[k].copy_(v, non_blocking=True)
+        for src, dst in ((cond_embeddings, "embs"), (scale_tables, "tables")):
+            if src is not None:
+                for a, b in zip(getattr(self.cn, dst), src):
+                    a.copy_(b, non_blocking=True)
         self.graph.replay()
         ops._count(self.launches_per_replay)
         return self.out
+
+
+def _nets(controlnet):
+    return controlnet.nets if isinstance(controlnet, MultiControlNetModel) else [controlnet]
+
+
+def controlnet_state(controlnet, sample_shape, controlnet_rows, dev):
+    """Device buffers of the ControlNet part of one denoiser step for `sample_shape` latents: per net a conditioning
+    embedding [controlnet_rows, H, W, C0] and a scale table; with controlnet_rows < rows, zeroed residual buffers
+    [rows, ...] whose last controlnet_rows rows the zero convs overwrite (the first rows stay zero,
+    pipeline_controlnet.py:1093-1100)."""
+    rows, _, H, W = sample_shape
+    nets = _nets(controlnet)
+    cn = SimpleNamespace(lo=rows - controlnet_rows, out=None,
+                         embs=[torch.zeros(controlnet_rows, H, W, n.config.block_out_channels[0], device=dev, dtype=bf16)
+                               for n in nets],
+                         tables=[torch.zeros(n.num_residuals, n._scale_width, device=dev, dtype=torch.float32)
+                                 for n in nets])
+    if cn.lo:
+        bufs = [torch.zeros(rows, h, w, c, device=dev, dtype=bf16) for h, w, c in nets[0].residual_shapes(H, W)]
+        cn.out = (bufs[:-1], bufs[-1])
+    return cn
+
+
+def denoise_with_controlnet(unet, controlnet, x, t, ctx, added, cn):
+    """ControlNet(s) on rows [cn.lo:] of the NHWC model input, then the UNet on all rows with their residuals
+    (pipeline_controlnet.py:1063-1113). t: device fp32 [rows]. Returns the UNet's NHWC output."""
+    lo = cn.lo
+    cadded = None if added is None else {k: v[lo:] for k, v in added.items()}
+    out = None if cn.out is None else ([d[lo:] for d in cn.out[0]], cn.out[1][lo:])
+    if isinstance(controlnet, MultiControlNetModel):
+        down, mid = controlnet.forward_nhwc(x[lo:], t[lo:], ctx[lo:], cn.embs, cn.tables, cadded, out=out)
+    else:
+        down, mid = controlnet.forward_nhwc(x[lo:], t[lo:], ctx[lo:], cn.embs[0], cn.tables[0], cadded, out=out)
+    if cn.out is not None:
+        down, mid = cn.out
+    return unet.forward_nhwc(x, t, ctx, added, down_block_additional_residuals=down, mid_block_additional_residual=mid,
+                             residuals_nchw=False)
 
 
 class StableDiffusionPipeline:
@@ -102,6 +157,16 @@ class StableDiffusionPipeline:
             g = GraphedUNet(self.unet, sample_shape, ctx_shape, None if added is None else {k: v.shape for k, v in added.items()})
             self._graphed[key] = g
         return g
+
+    def _begin(self, sample_shape, ctx, added, B, do_cfg):
+        """Per-call set-up of the denoiser once the loop's inputs are known: the CUDA graph (or None = eager)."""
+        return self._denoiser(sample_shape, ctx.shape, added)
+
+    def _predict(self, den, i, t, model_in, ctx, added, first):
+        """The model output of step i for the NCHW fp32 model input (the static inputs are copied on the first step)."""
+        if den is not None:
+            return den(model_in, float(t), ctx if first else None, added if first else None)
+        return self.unet.forward(model_in, float(t), ctx, added_cond_kwargs=added, return_dict=False)[0]
 
     @torch.no_grad()
     def __call__(self, prompt=None, height: Optional[int] = None, width: Optional[int] = None,
@@ -148,7 +213,7 @@ class StableDiffusionPipeline:
             added = {k: (v.to(bf16) if k == "text_embeds" else v.to(torch.float32)).contiguous() for k, v in added.items()}
         rows = 2 * B if do_cfg else B
         sample_shape = (rows,) + tuple(latents.shape[1:])
-        den = self._denoiser(sample_shape, ctx.shape, added)
+        den = self._begin(sample_shape, ctx, added, B, do_cfg)
         model_in = torch.empty(sample_shape, device=dev, dtype=torch.float32)
         nxt = torch.empty_like(latents)
         first = True
@@ -161,10 +226,7 @@ class StableDiffusionPipeline:
                 model_in[B:].copy_(scaled)
             else:
                 model_in = scaled
-            if den is not None:
-                eps = den(model_in, float(t), ctx if first else None, added if first else None)
-            else:
-                eps = self.unet.forward(model_in, float(t), ctx, added_cond_kwargs=added, return_dict=False)[0]
+            eps = self._predict(den, i, t, model_in, ctx, added, first)
             first = False
             if do_cfg and guidance_rescale > 0.0:
                 # rescale_noise_cfg (pipeline_stable_diffusion.py:69-80, :886-888; SDXL :1061-1067): the guided
@@ -179,6 +241,133 @@ class StableDiffusionPipeline:
             if callback_on_step_end is not None:
                 callback_on_step_end(self, i, t, {"latents": latents})
         return latents if output_type == "latent" else self.decode_latents(latents)
+
+
+class StableDiffusionControlNetPipeline(StableDiffusionPipeline):
+    """Loop-only mirror of ppdiffusers.StableDiffusionControlNetPipeline / StableDiffusionXLControlNetPipeline.__call__
+    (pipeline_controlnet.py:1047-1130, pipeline_controlnet_sd_xl.py's loop): each step runs the ControlNet(s) and the
+    UNet with their residuals (one CUDA graph per shape), then the CFG combine + scheduler kernel. The control images'
+    conditioning embedding does not depend on the timestep, so it runs once per call. Steps whose keep is 0 run the
+    ControlNet with scale 0, as the reference does.
+    `controlnet`: a ControlNetModel, a MultiControlNetModel or a list of ControlNetModels."""
+
+    def __init__(self, unet: UNet2DConditionModel, controlnet, scheduler: DDIMScheduler, use_cuda_graph: bool = True,
+                 vae=None):
+        super().__init__(unet, scheduler, use_cuda_graph=use_cuda_graph, vae=vae)
+        if isinstance(controlnet, (list, tuple)):
+            controlnet = MultiControlNetModel(controlnet)
+        self.controlnet = controlnet
+        self._control = None  # the control arguments of the call in progress
+
+    @torch.no_grad()
+    def __call__(self, prompt=None, height: Optional[int] = None, width: Optional[int] = None,
+                 image: Union[torch.Tensor, List[torch.Tensor]] = None, num_inference_steps: int = 50,
+                 guidance_scale: float = 7.5, negative_prompt=None, eta: float = 0.0,
+                 latents: Optional[torch.Tensor] = None, prompt_embeds: Optional[torch.Tensor] = None,
+                 negative_prompt_embeds: Optional[torch.Tensor] = None, output_type: str = "latent",
+                 controlnet_conditioning_scale: Union[float, List[float]] = 1.0, guess_mode: bool = False,
+                 control_guidance_start: Union[float, List[float]] = 0.0,
+                 control_guidance_end: Union[float, List[float]] = 1.0,
+                 added_cond_kwargs: Optional[Dict[str, torch.Tensor]] = None,
+                 negative_added_cond_kwargs: Optional[Dict[str, torch.Tensor]] = None, callback_on_step_end=None,
+                 generator: Optional[torch.Generator] = None, guidance_rescale: float = 0.0):
+        """`image`: the control image, fp32 [B | 1, C, H, W] in [0, 1] (a list of them, one per net, for
+        Multi-ControlNet); loading and resizing images is the caller's job. Other arguments as
+        StableDiffusionPipeline.__call__ and the reference (pipeline_controlnet.py:905-1003)."""
+        multi = isinstance(self.controlnet, MultiControlNetModel)
+        nets = _nets(self.controlnet)
+        if image is None:
+            raise ValueError("`image` (the control image) is required")
+        images = list(image) if multi else [image]
+        if len(images) != len(nets):
+            raise ValueError(f"{len(nets)} ControlNets need {len(nets)} control images, got {len(images)}")
+        # pipeline_controlnet.py:951-965: align the guidance window (and the scale) with the number of nets
+        if not isinstance(control_guidance_start, list) and isinstance(control_guidance_end, list):
+            control_guidance_start = len(control_guidance_end) * [control_guidance_start]
+        elif not isinstance(control_guidance_end, list) and isinstance(control_guidance_start, list):
+            control_guidance_end = len(control_guidance_start) * [control_guidance_end]
+        elif not isinstance(control_guidance_start, list) and not isinstance(control_guidance_end, list):
+            control_guidance_start, control_guidance_end = [control_guidance_start] * len(nets), [control_guidance_end] * len(nets)
+        if len(control_guidance_start) != len(nets) or len(control_guidance_end) != len(nets):
+            raise ValueError(f"control_guidance_start / _end need one entry per ControlNet ({len(nets)})")
+        for s, e in zip(control_guidance_start, control_guidance_end):
+            # start == end is an empty window: the ControlNet runs at scale 0 on every step
+            if s > e or s < 0.0 or e > 1.0:
+                raise ValueError(f"control guidance window [{s}, {e}] must satisfy 0 <= start <= end <= 1")
+        if multi and isinstance(controlnet_conditioning_scale, (float, int)):
+            controlnet_conditioning_scale = [float(controlnet_conditioning_scale)] * len(nets)
+        self._control = dict(images=images, scale=controlnet_conditioning_scale, guess_mode=guess_mode,
+                             start=control_guidance_start, end=control_guidance_end,
+                             steps=num_inference_steps, guidance_scale=guidance_scale)
+        try:
+            return super().__call__(prompt=prompt, height=height, width=width, num_inference_steps=num_inference_steps,
+                                    guidance_scale=guidance_scale, negative_prompt=negative_prompt, eta=eta,
+                                    latents=latents, prompt_embeds=prompt_embeds,
+                                    negative_prompt_embeds=negative_prompt_embeds, output_type=output_type,
+                                    added_cond_kwargs=added_cond_kwargs,
+                                    negative_added_cond_kwargs=negative_added_cond_kwargs,
+                                    callback_on_step_end=callback_on_step_end, generator=generator,
+                                    guidance_rescale=guidance_rescale)
+        finally:
+            self._control = None
+
+    def _begin(self, sample_shape, ctx, added, B, do_cfg):
+        from .. import ops
+        c = self._control
+        dev = self.unet.device
+        rows = sample_shape[0]
+        # guess mode with CFG: the ControlNet sees the conditional rows only (pipeline_controlnet.py:1063-1068)
+        cn_rows = B if (c["guess_mode"] and do_cfg) else rows
+        nets = _nets(self.controlnet)
+        c["keep"] = controlnet_keep(len(self.scheduler.timesteps), c["start"], c["end"], len(nets) > 1)
+        embs = []
+        for net, img in zip(nets, c["images"]):
+            img = img.to(device=dev, dtype=torch.float32).contiguous()
+            if img.shape[0] not in (1, B):
+                raise ValueError(f"control image batch {img.shape[0]} must be 1 or the prompt batch {B}")
+            if tuple(img.shape[2:]) != (sample_shape[2] * net.cond_downscale, sample_shape[3] * net.cond_downscale):
+                raise ValueError(f"control image {tuple(img.shape[2:])} does not match the latents {tuple(sample_shape[2:])}")
+            e = net.embed_condition(ops.nchw_to_nhwc(img))  # once per call (prepare_image repeats the image, :985-1003)
+            embs.append(e if e.shape[0] == cn_rows else e.repeat(cn_rows // e.shape[0], 1, 1, 1))
+        c["embs"] = embs
+        if self.use_cuda_graph:
+            key = ("controlnet", id(self.controlnet), cn_rows, tuple(sample_shape), tuple(ctx.shape),
+                   None if added is None else tuple((k, tuple(v.shape)) for k, v in added.items()))
+            g = self._graphed.get(key)
+            if g is None:
+                g = GraphedUNet(self.unet, sample_shape, ctx.shape,
+                                None if added is None else {k: v.shape for k, v in added.items()},
+                                controlnet=self.controlnet, controlnet_rows=cn_rows)
+                self._graphed[key] = g
+            return g
+        c["state"] = controlnet_state(self.controlnet, sample_shape, cn_rows, dev)
+        c["state"].embs = embs
+        return None
+
+    def _scale_tables(self, i):
+        """Host scale tables of step i: controlnet_conditioning_scale x keep (pipeline_controlnet.py:1074-1080)."""
+        c = self._control
+        keep, scale = c["keep"][i], c["scale"]
+        if isinstance(keep, list):
+            cond_scale = [s * k for s, k in zip(scale, keep)]
+        else:
+            cond_scale = (scale[0] if isinstance(scale, list) else scale) * keep
+        nets = _nets(self.controlnet)
+        scales = cond_scale if len(nets) > 1 else [cond_scale]
+        return [n.scale_table(n.residual_scales(s, c["guess_mode"])) for n, s in zip(nets, scales)]
+
+    def _predict(self, den, i, t, model_in, ctx, added, first):
+        from .. import ops
+        c = self._control
+        tables = self._scale_tables(i)
+        if den is not None:
+            return den(model_in, float(t), ctx if first else None, added if first else None,
+                       cond_embeddings=c["embs"] if first else None, scale_tables=tables)
+        st = c["state"]
+        st.tables = [tab.to(self.unet.device) for tab in tables]
+        tt = torch.full((model_in.shape[0],), float(t), device=self.unet.device, dtype=torch.float32)
+        y = denoise_with_controlnet(self.unet, self.controlnet, ops.nchw_to_nhwc(model_in), tt, ctx, added, st)
+        return ops.nhwc_to_nchw(y, out_dtype=bf16)
 
 
 class StableDiffusion3Pipeline:

@@ -54,6 +54,22 @@ _REFERENCE_DEFAULTS = dict(
     reverse_transformer_layers_per_block=None, attention_type="default")
 
 
+def _check_reference_defaults(model, options, defaults):
+    """Constructor arguments outside the supported family are accepted only at their reference defaults: each is
+    compared with ITS OWN default by type and value (True == 1.0 must not pass)."""
+    for k, v in options.items():
+        if k.startswith("_"):  # _class_name / _ppdiffusers_version bookkeeping of config.json
+            continue
+        if k == "upcast_attention" and isinstance(v, bool):
+            continue  # scores are always accumulated and soft-maxed in fp32 here (attention.cu), i.e. "upcast"
+        if k not in defaults:
+            raise NotImplementedError(f"{model}(b200): unknown config option {k}={v!r}")
+        d = defaults[k]
+        if not (v is d or (type(v) is type(d) and v == d)):
+            raise NotImplementedError(f"{model}(b200): config option {k}={v!r} is outside the hot path "
+                                      f"(only the reference default {d!r} is supported)")
+
+
 def _tup(v, n):
     return tuple(v) if isinstance(v, (tuple, list)) else (v,) * n
 
@@ -441,18 +457,8 @@ class UNet2DConditionModel:
                              "https://github.com/huggingface/diffusers/issues/2011#issuecomment-1547958131. Passing "
                              "`num_attention_heads` will only be supported in diffusers v0.19.")
         # the remaining reference constructor arguments (unet_2d_condition.py:172-228) are accepted only at their
-        # reference defaults: each is compared with ITS OWN default by type and value (True == 1.0 must not pass)
-        for k, v in unsupported.items():
-            if k.startswith("_"):  # _class_name / _ppdiffusers_version bookkeeping of config.json
-                continue
-            if k == "upcast_attention" and isinstance(v, bool):
-                continue  # scores are always accumulated and soft-maxed in fp32 here (attention.cu), i.e. "upcast"
-            if k not in _REFERENCE_DEFAULTS:
-                raise NotImplementedError(f"UNet2DConditionModel(b200): unknown config option {k}={v!r}")
-            d = _REFERENCE_DEFAULTS[k]
-            if not (v is d or (type(v) is type(d) and v == d)):
-                raise NotImplementedError(f"UNet2DConditionModel(b200): config option {k}={v!r} is outside the hot path "
-                                          f"(only the reference default {d!r} is supported)")
+        # reference defaults
+        _check_reference_defaults("UNet2DConditionModel", unsupported, _REFERENCE_DEFAULTS)
         if len(down_block_types) != len(up_block_types):
             raise ValueError(f"Must provide the same number of `down_block_types` as `up_block_types`. "
                              f"`down_block_types`: {down_block_types}. `up_block_types`: {up_block_types}.")
@@ -483,6 +489,35 @@ class UNet2DConditionModel:
 
     # ------------------------------------------------------------------------------------------------------------
     def _build(self):
+        res, tr = self._build_encoder()
+        c = self.config
+        boc = c.block_out_channels
+        n = len(boc)
+        heads, tl = _tup(c.attention_head_dim, n), _tup(c.transformer_layers_per_block, n)
+        lpb, cad = _tup(c.layers_per_block, n), _tup(c.cross_attention_dim, n)
+        self.up = []
+        rboc, rheads, rtl, rlpb, rcad = [list(reversed(x)) for x in (boc, heads, tl, lpb, cad)]
+        out_ch = rboc[0]
+        for i, t in enumerate(c.up_block_types):
+            prev, out_ch = out_ch, rboc[i]
+            in_ch = rboc[min(i + 1, n - 1)]
+            blk = SimpleNamespace(resnets=[], attns=[], up=None)
+            for j in range(rlpb[i] + 1):
+                skip = in_ch if j == rlpb[i] else out_ch
+                rin = prev if j == 0 else out_ch
+                blk.resnets.append(res(f"up_blocks.{i}.resnets.{j}", rin + skip, out_ch))
+                if t == "CrossAttnUpBlock2D":
+                    blk.attns.append(tr(f"up_blocks.{i}.attentions.{j}", out_ch, rheads[i], rcad[i], rtl[i]))
+                elif t != "UpBlock2D":
+                    raise NotImplementedError(f"up block type {t}")
+            if i != n - 1:
+                blk.up = _Conv3x3(f"up_blocks.{i}.upsamplers.0.conv", out_ch, out_ch, upsample=True)
+            self.up.append(blk)
+        self.norm_out, self.conv_out = _Norm("conv_norm_out", boc[0]), _Conv3x3("conv_out", boc[0], c.out_channels)
+
+    def _build_encoder(self):
+        """conv_in, the time / added-condition embeddings, the down blocks and the mid block (the part a ControlNet
+        shares with the UNet). Returns the resnet / transformer constructors for the rest of the model."""
         c = self.config
         boc = c.block_out_channels
         n = len(boc)
@@ -499,7 +534,7 @@ class UNet2DConditionModel:
             self.add_lin2 = _Linear("add_embedding.linear_2", ted, ted)
             # pipelines read unet.add_embedding.linear_1.in_features (pipeline_stable_diffusion_xl.py:609-611)
             self.add_embedding = SimpleNamespace(linear_1=SimpleNamespace(in_features=c.projection_class_embeddings_input_dim))
-        self.down, self.up = [], []
+        self.down = []
         self.resnets, self.transformers = [], []
 
         def res(name, i, o):
@@ -530,33 +565,19 @@ class UNet2DConditionModel:
             res0=res("mid_block.resnets.0", boc[-1], boc[-1]),
             attn=tr("mid_block.attentions.0", boc[-1], heads[-1], cad[-1], tl[-1]),
             res1=res("mid_block.resnets.1", boc[-1], boc[-1]))
-        rboc, rheads, rtl, rlpb, rcad = [list(reversed(x)) for x in (boc, heads, tl, lpb, cad)]
-        out_ch = rboc[0]
-        for i, t in enumerate(c.up_block_types):
-            prev, out_ch = out_ch, rboc[i]
-            in_ch = rboc[min(i + 1, n - 1)]
-            blk = SimpleNamespace(resnets=[], attns=[], up=None)
-            for j in range(rlpb[i] + 1):
-                skip = in_ch if j == rlpb[i] else out_ch
-                rin = prev if j == 0 else out_ch
-                blk.resnets.append(res(f"up_blocks.{i}.resnets.{j}", rin + skip, out_ch))
-                if t == "CrossAttnUpBlock2D":
-                    blk.attns.append(tr(f"up_blocks.{i}.attentions.{j}", out_ch, rheads[i], rcad[i], rtl[i]))
-                elif t != "UpBlock2D":
-                    raise NotImplementedError(f"up block type {t}")
-            if i != n - 1:
-                blk.up = _Conv3x3(f"up_blocks.{i}.upsamplers.0.conv", out_ch, out_ch, upsample=True)
-            self.up.append(blk)
-        self.norm_out, self.conv_out = _Norm("conv_norm_out", boc[0]), _Conv3x3("conv_out", boc[0], c.out_channels)
+        return res, tr
+
+    def _leaves(self):
+        """Every weight-holding layer: each has shapes() and load(P, dev)."""
+        leaves = [self.conv_in, self.time_lin1, self.time_lin2, self.add_lin1, self.add_lin2, self.norm_out, self.conv_out,
+                  *self.resnets, *self.transformers, *(b.down for b in self.down), *(b.up for b in self.up)]
+        return [m for m in leaves if m is not None]
 
     def state_dict_shapes(self) -> Dict[str, tuple]:
         """Names and shapes of the reference state dict this model consumes (Paddle layouts)."""
         out = {}
-        leaves = [self.conv_in, self.time_lin1, self.time_lin2, self.add_lin1, self.add_lin2, self.norm_out, self.conv_out,
-                  *self.resnets, *self.transformers, *(b.down for b in self.down), *(b.up for b in self.up)]
-        for m in leaves:
-            if m is not None:
-                out.update(m.shapes())
+        for m in self._leaves():
+            out.update(m.shapes())
         return out
 
     def init_synthetic_weights(self, seed: int = 1, device: Union[int, str] = 0):
@@ -615,20 +636,8 @@ class UNet2DConditionModel:
         missing = [k for k in self.state_dict_shapes() if k not in P]
         if missing:
             raise KeyError(f"state dict is missing {len(missing)} parameters, e.g. {missing[:3]}")
-        for m in (self.conv_in, self.time_lin1, self.time_lin2, self.norm_out, self.conv_out):
+        for m in self._leaves():
             m.load(P, dev)
-        if self.add_lin1 is not None:
-            self.add_lin1.load(P, dev), self.add_lin2.load(P, dev)
-        for r in self.resnets:
-            r.load(P, dev)
-        for t in self.transformers:
-            t.load(P, dev)
-        for blk in self.down:
-            if blk.down is not None:
-                blk.down.load(P, dev)
-        for blk in self.up:
-            if blk.up is not None:
-                blk.up.load(P, dev)
         # batched time_emb_proj: one GEMM [B, ted] x [sum(cout), ted]^T per forward
         off = 0
         ws, bs = [], []
