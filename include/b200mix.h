@@ -342,6 +342,30 @@ int b200mix_decode_rope_cache(void* qkv, int64_t ld_row, int64_t B, int64_t head
                               const float* cos, const float* sin, const int64_t* rows, void* cache_k, void* cache_v,
                               void* stream);
 
+/* ---- Token sampling (PaddleNLP GenerationMixin.greedy_search / sample, generation/utils.py:1028-1271) ------------- */
+
+/* One generation step for B rows of fp32 logits (row b at logits + b * ld, V <= 2^20 columns), one CTA per row:
+ *   1. repetition penalty (logits_process.py:104-110): l = l < 0 ? l * penalty : l / penalty for every id whose bit is
+ *      set in the row's presence bitmap (uint32 [B, ceil(V / 32)], bit i of word i / 32);
+ *   2. do_sample == 0: argmax of the penalised logits, lowest id on ties (temperature, top_k, top_p are ignored);
+ *   3. do_sample != 0: p = softmax(l / temperature) in fp32 (IEEE division, accurate expf); top_k > 0 keeps
+ *      p >= the k-th largest p (ties kept); top_p < 1 then keeps, in order of descending p with lower ids first among
+ *      equal p, every id whose preceding mass is <= top_p (the top-k output is not renormalised; the first id is always
+ *      kept); masses are summed as floor(p * 2^48) integers. Draw: Philox4x32-10 with key = seed and counter =
+ *      (step, b, 0, 0), u = (x0 >> 8) * 2^-24; the token is the first kept id, in ascending id order, whose inclusive
+ *      prefix mass exceeds u * (kept mass);
+ *   4. (utils.py:1239-1259) a row already finished emits pad_id instead; finished[b] |= (token in eos_ids). The token
+ *      is written to out[b * ld_out + step] (when step < max_new) and to next_ids[b], and its presence bit is set.
+ * state (uint64 [4], zeroed before the first step): [0] = step, [1] = arrival counter (left at 0), [2] = 1 once every
+ * row has finished, [3] = the step at which the last row finished. The kernel advances state[0], so the call can be
+ * replayed in a CUDA graph. finished int32 [B]; eos_ids int64 [n_eos] (n_eos = 0: rows never finish); pad_id in
+ * [0, V) when n_eos > 0. Requires temperature > 0, 0 < top_p <= 1, top_k >= 0, penalty > 0; 4-byte aligned logits /
+ * presence / finished and 8-byte aligned state / out / next_ids / eos_ids. */
+int b200mix_sample_tokens(const float* logits, int64_t ld, int64_t B, int64_t V, uint32_t* presence, int32_t* finished,
+                          uint64_t* state, int64_t* out, int64_t ld_out, int64_t max_new, int64_t* next_ids,
+                          const int64_t* eos_ids, int32_t n_eos, int64_t pad_id, int32_t do_sample, float temperature,
+                          int32_t top_k, float top_p, float penalty, uint64_t seed, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

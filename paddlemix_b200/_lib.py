@@ -5,7 +5,7 @@ missing, importing this module raises, and every entry point returns B200MIX_ERR
 """
 import ctypes
 import os
-from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int64, c_void_p
+from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int64, c_uint64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # B200MIX_LIB selects an alternative build of the same library (A/B kernel experiments); never a different backend
@@ -109,6 +109,9 @@ SIGNATURES = {
     "b200mix_rope_inplace": [c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p],
     "b200mix_decode_rope_cache": [c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p,
                                   c_void_p, c_void_p, c_void_p],
+    "b200mix_sample_tokens": [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
+                              c_int64, c_void_p, c_void_p, c_int32, c_int64, c_int32, c_float, c_int32, c_float,
+                              c_float, c_uint64, c_void_p],
 }
 STRING_GETTERS = ("b200mix_last_error", "b200mix_version")
 

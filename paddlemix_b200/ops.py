@@ -639,6 +639,37 @@ def decode_rope_cache(qkv: torch.Tensor, heads: int, kv_heads: int, head_dim: in
     _count()
 
 
+def sample_tokens(logits: torch.Tensor, presence: torch.Tensor, finished: torch.Tensor, state: torch.Tensor,
+                  out: torch.Tensor, next_ids: torch.Tensor, eos_ids: Optional[torch.Tensor] = None, pad_token_id=0, *,
+                  do_sample=False, temperature=1.0, top_k=0, top_p=1.0, repetition_penalty=1.0, seed=0):
+    """One generation step (b200mix_sample_tokens, see include/b200mix.h): logits fp32 [B, V] view with a contiguous
+    vocabulary axis (any row stride: logits[:, -1] of prefill logits [B, S, V] is read in place); presence int32
+    [B, ceil(V/32)] bitmap of the ids seen so far; finished int32 [B]; state int64 [4] (step, arrivals, all finished,
+    step of the last finish; zero before the first step); out int64 [B, max_new]; next_ids int64 [B]; eos_ids int64
+    [n] on the device or None. Every buffer except logits is updated on the device."""
+    _req(logits, torch.float32, "logits"), _req(presence, torch.int32, "presence"), _req(finished, torch.int32, "finished")
+    _req(state, torch.int64, "state"), _req(out, torch.int64, "out"), _req(next_ids, torch.int64, "next_ids")
+    B, V = logits.shape
+    if logits.stride(1) != 1 and V > 1:
+        raise ValueError("logits must have a contiguous vocabulary axis")
+    words = (V + 31) // 32
+    if tuple(presence.shape) != (B, words) or not presence.is_contiguous():
+        raise ValueError(f"presence must be a contiguous int32 [{B}, {words}] bitmap, got {tuple(presence.shape)}")
+    if finished.numel() != B or next_ids.numel() != B or state.numel() != 4 or out.shape[0] != B or out.stride(1) != 1:
+        raise ValueError("finished / next_ids must have B entries, state 4, out [B, max_new] with contiguous rows")
+    n_eos = 0
+    if eos_ids is not None:
+        _req(eos_ids, torch.int64, "eos_ids")
+        n_eos = eos_ids.numel()
+    with _Timed("sampling", 4.0 * B * V, "byte", lambda: f"sample {B}x{V}"):
+        check(lib.b200mix_sample_tokens(_p(logits), logits.stride(0), B, V, _p(presence), _p(finished), _p(state),
+                                        _p(out), out.stride(0), out.shape[1], _p(next_ids), _p(eos_ids), n_eos,
+                                        int(pad_token_id), 1 if do_sample else 0, float(temperature), int(top_k),
+                                        float(top_p), float(repetition_penalty), int(seed) & (2 ** 64 - 1), _stream()),
+              "b200mix_sample_tokens")
+    _count()
+
+
 def gather_rows(table: torch.Tensor, ids: torch.Tensor) -> torch.Tensor:
     """table bf16 [V, D], ids int64 [n] (device) -> bf16 [n, D]."""
     _req(table, bf16, "table"), _req(ids, torch.int64, "ids")

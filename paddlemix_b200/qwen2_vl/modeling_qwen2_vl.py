@@ -77,11 +77,13 @@ class GraphedDecodeStep:
     Static device state: newest token ids, the cache row to write and the key count per sequence (both advance INSIDE the
     graph), the 1-D rotary position per sequence (after the prompt all three M-RoPE axes carry the same position,
     cache_position + rope_delta, modeling_qwen2_vl.py:1413-1441) with cos / sin gathered from device tables.
-    step(ids) = one small H2D copy (or none, with device ids) + one graph replay; logits stay on the device."""
+    step(ids) = one small H2D copy (or none, with device ids) + one graph replay; logits stay on the device.
+    With a `sampler` (sampling.TokenSampler) the graph also runs b200mix_sample_tokens on the step's logits, which writes
+    the next ids straight into the static ids buffer (sampler.ids): step() is then a replay only."""
 
-    def __init__(self, model, cache: KVCache, rope_deltas, warmup: int = 2):
+    def __init__(self, model, cache: KVCache, rope_deltas, warmup: int = 2, sampler=None):
         from .. import ops
-        self.model, self.cache = model, cache
+        self.model, self.cache, self.sampler = model, cache, sampler
         dev, B, hd = model.device, cache.batch, model.head_dim
         c = model.config
         P = cache.length
@@ -91,7 +93,7 @@ class GraphedDecodeStep:
         fr = torch.arange(n_pos, dtype=torch.float32)[:, None] * inv_freq[None]
         emb = torch.cat([fr, fr], -1)
         self.cos_table, self.sin_table = emb.cos().contiguous().to(dev), emb.sin().contiguous().to(dev)
-        self.ids = torch.zeros(B, dtype=torch.long, device=dev)
+        self.ids = torch.zeros(B, dtype=torch.long, device=dev) if sampler is None else sampler.ids
         self.pos = (P + deltas).clamp(min=0).to(dev)
         self.rows = (torch.arange(B) * cache.max_len + P).to(dev)
         self.kv_lens = torch.full((B,), P + 1, dtype=torch.int32, device=dev)
@@ -118,16 +120,22 @@ class GraphedDecodeStep:
         n0 = ops.launches()
         with torch.cuda.graph(self.graph):
             self.logits = body()
+            if sampler is not None:
+                sampler(self.logits)
         self.launches_per_step = ops.launches() - n0
         for t, t0 in zip((self.pos, self.rows, self.kv_lens), self._state0):
             t.copy_(t0)
 
-    def step(self, ids):
-        """ids: int64 [B] (host or device) newest token of each sequence -> fp32 logits [B, vocab] (device, reused)."""
+    def step(self, ids=None):
+        """ids: int64 [B] (host or device) newest token of each sequence -> fp32 logits [B, vocab] (device, reused).
+        With a sampler, ids is None: the previous step's sampler output is already in place."""
         from .. import ops
         if self.cache.length + 1 > self.cache.max_len:
             raise ValueError(f"KV cache is full ({self.cache.max_len} positions)")
-        self.ids.copy_(ids.reshape(-1), non_blocking=True)
+        if ids is not None:
+            self.ids.copy_(ids.reshape(-1), non_blocking=True)
+        elif self.sampler is None:
+            raise ValueError("step() needs the newest ids when the graph has no sampler")
         self.graph.replay()
         ops._count(self.launches_per_step)
         self.cache.length += 1
@@ -560,13 +568,32 @@ class Qwen2VLForConditionalGeneration:
 
     @torch.no_grad()
     def generate(self, input_ids, pixel_values=None, image_grid_thw=None, max_new_tokens: int = 16, eos_token_id=None,
-                 attention_mask=None):
-        """Greedy decoding (generation_utils' default `do_sample=False`): prefill with use_cache, then one decode step per
-        token; returns [B, S + n_new] token ids (generation stops early when every sequence has produced EOS). Prompts of
-        different lengths are LEFT-padded (attention_mask zeros in front), so that every prompt ends at column S - 1."""
+                 attention_mask=None, *, decode_strategy: str = "greedy_search", do_sample: bool = False,
+                 temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, repetition_penalty: float = 1.0,
+                 pad_token_id: Optional[int] = None, generator: Optional[torch.Generator] = None):
+        """PaddleNLP GenerationMixin.generate for greedy search and sampling (generation/utils.py): prefill with
+        use_cache, then one decode step per token; returns [B, S + n_new] token ids. Prompts of different lengths are
+        LEFT-padded (attention_mask zeros in front), so that every prompt ends at column S - 1.
+
+        Greedy search (the default) takes the argmax. do_sample=True or decode_strategy="sampling" draws from
+        softmax(logits / temperature) after top_k / top_p filtering; repetition_penalty applies to both. eos_token_id is
+        an int or a list of ints; a sequence that has produced one of them is continued with pad_token_id (default: an
+        int eos_token_id) and generation stops at the step where the last sequence finished. The random numbers come
+        from a Philox key drawn from `generator` (torch's default CPU generator when None): the same generator state
+        gives the same tokens. Everything after the prefill runs as CUDA-graph replays with next-token selection on
+        the device (b200mix_sample_tokens).
+
+        Calls that use none of penalty, sampling, an eos list or pad_token_id keep plain greedy decoding, which does
+        not pad sequences that have finished."""
+        from ..sampling import resolve_generation_args, seed_from
+        args = resolve_generation_args(decode_strategy, do_sample, temperature, top_k, top_p, repetition_penalty,
+                                       eos_token_id, pad_token_id)
         B, S = input_ids.shape
         if attention_mask is not None and not bool((attention_mask[:, -1] == 1).all()):
             raise ValueError("generate(): pad on the left (the last column of attention_mask must be all ones)")
+        if args.on_device:
+            return self._generate_on_device(input_ids, pixel_values, image_grid_thw, max_new_tokens, attention_mask,
+                                            args, seed_from(generator) if args.do_sample else 0)
         self.cache_headroom = max_new_tokens
         out = self.forward(input_ids=input_ids, attention_mask=attention_mask, pixel_values=pixel_values,
                            image_grid_thw=image_grid_thw, use_cache=True)
@@ -588,5 +615,26 @@ class Qwen2VLForConditionalGeneration:
             out = self.forward(input_ids=seq[-1], past_key_values=cache, rope_deltas=deltas, use_cache=True)
             seq.append(out.logits[:, -1].argmax(-1).cpu().unsqueeze(1))
         return torch.cat(seq, 1)
+
+    def _generate_on_device(self, input_ids, pixel_values, image_grid_thw, max_new_tokens, attention_mask, args, seed):
+        """generate() with b200mix_sample_tokens: the prefill's last logits row gives the first token, then every
+        decode step and its token selection is one graph replay; the host reads the all-finished flag once every
+        FINISH_CHECK_INTERVAL steps."""
+        from ..sampling import FINISH_CHECK_INTERVAL, TokenSampler
+        if max_new_tokens < 1:
+            raise ValueError(f"max_new_tokens must be >= 1, got {max_new_tokens}")
+        self.cache_headroom = max_new_tokens
+        out = self.forward(input_ids=input_ids, attention_mask=attention_mask, pixel_values=pixel_values,
+                           image_grid_thw=image_grid_thw, use_cache=True)
+        sampler = TokenSampler(input_ids, self.config.vocab_size, max_new_tokens, args, seed, self.device)
+        sampler(out.logits[:, -1])
+        if max_new_tokens > 1:
+            stepper = GraphedDecodeStep(self, out.past_key_values, out.rope_deltas, sampler=sampler)
+            for i in range(1, max_new_tokens):
+                if i % FINISH_CHECK_INTERVAL == 0 and sampler.all_finished():
+                    break
+                stepper.step()
+        n = sampler.n_generated()
+        return torch.cat([input_ids.cpu(), sampler.out[:, :n].cpu()], 1)
 
     __call__ = forward
