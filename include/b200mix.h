@@ -366,6 +366,62 @@ int b200mix_sample_tokens(const float* logits, int64_t ld, int64_t B, int64_t V,
                           const int64_t* eos_ids, int32_t n_eos, int64_t pad_id, int32_t do_sample, float temperature,
                           int32_t top_k, float top_p, float penalty, uint64_t seed, void* stream);
 
+/* ---- Beam search (PaddleNLP GenerationMixin.beam_search, generation/utils.py:1484-1649) -------------------------- */
+
+/* Device state of one beam-search call over B items of nb beams (rows = B * nb, row b * nb + j is beam j of item b).
+ * Every buffer lives on the device; the step kernel reads and updates them, so a call can be replayed in a CUDA graph. */
+typedef struct b200mix_beam_state {
+  uint64_t* state;      /* [4] zeroed before step 0: [0] step, [1] arrival counter (left at 0), [2] 1 once every item is
+                           done, [3] generated cache positions the following b200mix_kv_reorder moves (0: none,
+                           also after the selection at step max_new - 1, whose cache no decode step reads) */
+  int64_t* next_ids;    /* [rows] the chosen token per beam slot (what the next decode step embeds) */
+  float* beam_scores;   /* [rows] running beam scores: 0 for beam 0, -1e6 for the others before step 0 (:1523-1526) */
+  int64_t* tokens;      /* [max_new, rows] token chosen per slot at each step */
+  int32_t* parents;     /* [max_new, rows] parent beam (within the item) of each slot at each step */
+  double* hyp_score;    /* [B, nb] BeamHypotheses in insertion order: score (GNMT length penalty applied), */
+  int32_t* hyp_step;    /* [B, nb]   number of generated tokens of the hypothesis (the step its eos was chosen), */
+  int32_t* hyp_slot;    /* [B, nb]   beam slot whose history it ends, at that step */
+  int32_t* hyp_count;   /* [B] entries in use */
+  double* hyp_worst;    /* [B] worst_score, 1e6 before step 0 (:107) */
+  int32_t* done;        /* [B] BeamSearchScorer._done */
+  uint32_t* presence;   /* [2, rows, ceil(V / 32)] ping-pong bitmaps of the ids in each beam (buffer step & 1 is read,
+                           the other written); NULL when penalty == 1 */
+} b200mix_beam_state;
+
+/* Bytes of the scratch buffer b200mix_beam_search_step needs for B items of nb beams over V tokens (into *bytes). */
+int b200mix_beam_search_workspace_size(int64_t B, int64_t nb, int64_t V, int64_t* bytes);
+
+/* One beam-search step (beam_search :1555-1621 with BeamSearchScorer.process :196-262 and BeamHypotheses :98-143) for
+ * fp32 logits of B * nb rows (row r at logits + r * ld):
+ *   1. score = log(exp(x - max) / sum) in fp32 (:1561-1562), repetition penalty (logits_process.py:104-110: score < 0 ?
+ *      score * penalty : score / penalty on the ids present in the beam), + the running beam score (:1564);
+ *   2. diversity_rate == 0: the item's top 2 * nb of its nb * V scores (:1569-1574); diversity_rate > 0: each row's top
+ *      2 * nb, minus rank * diversity_rate (rank 1 .. 2 * nb, fp32), top 2 * nb of those (:1576-1598), whose
+ *      undiversified scores go on. Ties: lower flat index (beam * V + token, or beam * 2 * nb + rank - 1) first;
+ *   3. process in fp64: an eos_id candidate at rank < nb adds a hypothesis with score / ((step + 5) / 6)^length_penalty,
+ *      one at rank >= nb is skipped, any other candidate fills the next slot; a done item emits pad_id, score 0, parent
+ *      0; is_done with early_stopping or worst_score >= best candidate / ((step + 5) / 6)^length_penalty.
+ * Writes next_ids, beam_scores, column `step` of tokens / parents, the hypothesis store, done, the child presence
+ * bitmaps and advances state (steps at or past max_new, or after every item is done, change nothing but state[3]).
+ * Scores are rounded after every operation (no fused multiply-add), as the reference rounds them.
+ * eos_id = -1: no eos. Requires 2 <= nb <= 16, 2 * nb <= V <= 2^20, penalty > 0, finite diversity_rate >= 0 and
+ * length_penalty, pad_id in [0, V), the workspace of b200mix_beam_search_workspace_size (16-byte aligned). */
+int b200mix_beam_search_step(const float* logits, int64_t ld, int64_t B, int64_t nb, int64_t V,
+                             const b200mix_beam_state* st, void* workspace, int64_t workspace_bytes, int64_t max_new,
+                             int64_t eos_id, int64_t pad_id, float penalty, float diversity_rate, double length_penalty,
+                             int32_t early_stopping, void* stream);
+
+/* reorder_cache (:1480-1482, index_select of every cache tensor by the chosen parents) for the generated region only,
+ * in place, all layers in one launch. layer_kv: device array [2 * n_layers] of bf16 cache bases (K_0, V_0, K_1, ...),
+ * each [B * nb, max_len, row_elems]. Moves positions [S, S + state[3]) of every beam whose parent (column state[0] - 1 of
+ * parents [max_new, B * nb]) is not itself; items with done[b] set are left alone. Prompt positions [0, S) are never
+ * touched: they are the same in every beam of an item. Launched for max_new positions (CTAs past state[3] exit), so it
+ * can be captured once and replayed. Requires row_elems a multiple of 8, nb * row_elems * 2 <= 32768 and every base in
+ * layer_kv 16-byte aligned (rows are moved as 16-byte vectors; the table lives on the device, so this is not checked). */
+int b200mix_kv_reorder(void* const* layer_kv, int64_t n_layers, int64_t B, int64_t nb, int64_t max_len,
+                       int64_t row_elems, int64_t S, int64_t max_new, const int32_t* parents, const uint64_t* state,
+                       const int32_t* done, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

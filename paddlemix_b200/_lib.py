@@ -5,7 +5,7 @@ missing, importing this module raises, and every entry point returns B200MIX_ERR
 """
 import ctypes
 import os
-from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int64, c_uint64, c_void_p
+from ctypes import POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_uint64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # B200MIX_LIB selects an alternative build of the same library (A/B kernel experiments); never a different backend
@@ -38,6 +38,13 @@ class Epilogue(Structure):
         ("ln_rms", c_int32),
         ("ln_eps", c_float),
     ]
+
+
+class BeamState(Structure):
+    """Mirror of `b200mix_beam_state` (include/b200mix.h): device pointers."""
+
+    _fields_ = [(name, c_void_p) for name in ("state", "next_ids", "beam_scores", "tokens", "parents", "hyp_score",
+                                              "hyp_step", "hyp_slot", "hyp_count", "hyp_worst", "done", "presence")]
 
 
 ACT_NONE, ACT_SILU, ACT_GELU_ERF, ACT_GELU_TANH, ACT_QUICK_GELU = 0, 1, 2, 3, 4
@@ -112,6 +119,11 @@ SIGNATURES = {
     "b200mix_sample_tokens": [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
                               c_int64, c_void_p, c_void_p, c_int32, c_int64, c_int32, c_float, c_int32, c_float,
                               c_float, c_uint64, c_void_p],
+    "b200mix_beam_search_workspace_size": [c_int64, c_int64, c_int64, POINTER(c_int64)],
+    "b200mix_beam_search_step": [c_void_p, c_int64, c_int64, c_int64, c_int64, POINTER(BeamState), c_void_p, c_int64,
+                                 c_int64, c_int64, c_int64, c_float, c_float, c_double, c_int32, c_void_p],
+    "b200mix_kv_reorder": [c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p,
+                           c_void_p, c_void_p],
 }
 STRING_GETTERS = ("b200mix_last_error", "b200mix_version")
 

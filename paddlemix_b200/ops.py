@@ -670,6 +670,73 @@ def sample_tokens(logits: torch.Tensor, presence: torch.Tensor, finished: torch.
     _count()
 
 
+def beam_search_workspace_bytes(B: int, num_beams: int, V: int) -> int:
+    n = ctypes.c_int64(0)
+    check(lib.b200mix_beam_search_workspace_size(B, num_beams, V, ctypes.byref(n)), "b200mix_beam_search_workspace_size")
+    return n.value
+
+
+def beam_search_step(logits: torch.Tensor, num_beams: int, workspace: torch.Tensor, *, state, next_ids, beam_scores,
+                     tokens, parents, hyp_score, hyp_step, hyp_slot, hyp_count, hyp_worst, done, presence=None,
+                     eos_token_id=-1, pad_token_id=0, repetition_penalty=1.0, diversity_rate=0.0, length_penalty=1.0,
+                     early_stopping=False):
+    """One beam-search step (b200mix_beam_search_step, see include/b200mix.h): logits fp32 [B * nb, V] view with a
+    contiguous vocabulary axis (any row stride); state int64 [4]; next_ids int64 [B*nb]; beam_scores fp32 [B*nb]; tokens
+    int64 / parents int32 [max_new, B*nb]; hyp_score fp64 / hyp_step, hyp_slot int32 [B, nb]; hyp_count int32 [B];
+    hyp_worst fp64 [B]; done int32 [B]; presence int32 [2, B*nb, ceil(V/32)] or None (penalty 1); workspace uint8 of
+    beam_search_workspace_bytes(B, nb, V). Everything but logits is updated on the device; eos_token_id -1 = none."""
+    _req(logits, torch.float32, "logits")
+    rows, V = logits.shape
+    nb = int(num_beams)
+    if logits.stride(1) != 1 or rows % nb:
+        raise ValueError(f"logits must be [B * {nb}, V] with a contiguous vocabulary axis, got {tuple(logits.shape)}")
+    B = rows // nb
+    for t, dt, n, name in ((state, torch.int64, 4, "state"), (next_ids, torch.int64, rows, "next_ids"),
+                           (beam_scores, torch.float32, rows, "beam_scores"), (hyp_score, torch.float64, B * nb, "hyp_score"),
+                           (hyp_step, torch.int32, B * nb, "hyp_step"), (hyp_slot, torch.int32, B * nb, "hyp_slot"),
+                           (hyp_count, torch.int32, B, "hyp_count"), (hyp_worst, torch.float64, B, "hyp_worst"),
+                           (done, torch.int32, B, "done")):
+        _req(t, dt, name)
+        if t.numel() != n or not t.is_contiguous():
+            raise ValueError(f"{name} must be a contiguous tensor of {n} elements, got {tuple(t.shape)}")
+    _req(tokens, torch.int64, "tokens"), _req(parents, torch.int32, "parents"), _req(workspace, torch.uint8, "workspace")
+    max_new = tokens.shape[0]
+    if tuple(tokens.shape) != (max_new, rows) or tuple(parents.shape) != (max_new, rows) or not (
+            tokens.is_contiguous() and parents.is_contiguous()):
+        raise ValueError(f"tokens / parents must be contiguous [max_new, {rows}]")
+    if presence is not None:
+        _req(presence, torch.int32, "presence")
+        if tuple(presence.shape) != (2, rows, (V + 31) // 32) or not presence.is_contiguous():
+            raise ValueError(f"presence must be a contiguous int32 [2, {rows}, {(V + 31) // 32}] bitmap pair")
+    st = _lib.BeamState(*(t.data_ptr() for t in (state, next_ids, beam_scores, tokens, parents, hyp_score, hyp_step,
+                                                 hyp_slot, hyp_count, hyp_worst, done)),
+                        None if presence is None else presence.data_ptr())
+    with _Timed("beam_search", 4.0 * rows * V, "byte", lambda: f"beam {B}x{nb}x{V}"):
+        check(lib.b200mix_beam_search_step(_p(logits), logits.stride(0), B, nb, V, ctypes.byref(st), _p(workspace),
+                                           workspace.numel(), max_new, int(eos_token_id), int(pad_token_id),
+                                           float(repetition_penalty), float(diversity_rate), float(length_penalty),
+                                           1 if early_stopping else 0, _stream()), "b200mix_beam_search_step")
+    _count(3)
+
+
+def kv_reorder(layer_kv: torch.Tensor, cache_k, num_beams: int, prompt_len: int, parents: torch.Tensor,
+               state: torch.Tensor, done: torch.Tensor):
+    """b200mix_kv_reorder: layer_kv int64 [2 * L] device table of the K / V base pointers (K_0, V_0, K_1, ...) of caches
+    shaped like cache_k (bf16 [B * nb, max_len, kv_heads, head_dim], contiguous); moves the generated positions
+    [prompt_len, prompt_len + state[3]) from parent beam to child (parents int32 [max_new, B * nb], column state[0] - 1)
+    for every item whose done flag is 0."""
+    _req(layer_kv, torch.int64, "layer_kv"), _req(cache_k, bf16, "cache_k"), _req(parents, torch.int32, "parents")
+    _req(state, torch.int64, "state"), _req(done, torch.int32, "done")
+    rows, max_len = cache_k.shape[:2]
+    nb = int(num_beams)
+    if rows % nb or not cache_k.is_contiguous() or layer_kv.numel() % 2 or parents.shape[1] != rows:
+        raise ValueError("kv_reorder: cache / parents shapes do not match num_beams")
+    check(lib.b200mix_kv_reorder(_p(layer_kv), layer_kv.numel() // 2, rows // nb, nb, max_len,
+                                 cache_k[0, 0].numel(), int(prompt_len), parents.shape[0], _p(parents), _p(state),
+                                 _p(done), _stream()), "b200mix_kv_reorder")
+    _count()
+
+
 def gather_rows(table: torch.Tensor, ids: torch.Tensor) -> torch.Tensor:
     """table bf16 [V, D], ids int64 [n] (device) -> bf16 [n, D]."""
     _req(table, bf16, "table"), _req(ids, torch.int64, "ids")

@@ -78,8 +78,9 @@ class GraphedDecodeStep:
     graph), the 1-D rotary position per sequence (after the prompt all three M-RoPE axes carry the same position,
     cache_position + rope_delta, modeling_qwen2_vl.py:1413-1441) with cos / sin gathered from device tables.
     step(ids) = one small H2D copy (or none, with device ids) + one graph replay; logits stay on the device.
-    With a `sampler` (sampling.TokenSampler) the graph also runs b200mix_sample_tokens on the step's logits, which writes
-    the next ids straight into the static ids buffer (sampler.ids): step() is then a replay only."""
+    With a `sampler` (sampling.TokenSampler or beam_search.BeamSearcher) the graph also runs its token selection on the
+    step's logits, which writes the next ids straight into the static ids buffer (sampler.ids): step() is then a replay
+    only."""
 
     def __init__(self, model, cache: KVCache, rope_deltas, warmup: int = 2, sampler=None):
         from .. import ops
@@ -570,10 +571,13 @@ class Qwen2VLForConditionalGeneration:
     def generate(self, input_ids, pixel_values=None, image_grid_thw=None, max_new_tokens: int = 16, eos_token_id=None,
                  attention_mask=None, *, decode_strategy: str = "greedy_search", do_sample: bool = False,
                  temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, repetition_penalty: float = 1.0,
-                 pad_token_id: Optional[int] = None, generator: Optional[torch.Generator] = None):
-        """PaddleNLP GenerationMixin.generate for greedy search and sampling (generation/utils.py): prefill with
-        use_cache, then one decode step per token; returns [B, S + n_new] token ids. Prompts of different lengths are
-        LEFT-padded (attention_mask zeros in front), so that every prompt ends at column S - 1.
+                 pad_token_id: Optional[int] = None, generator: Optional[torch.Generator] = None,
+                 num_beams: int = 1, length_penalty: float = 1.0, early_stopping: bool = False,
+                 num_return_sequences: int = 1, diversity_rate: float = 0.0, num_beam_groups: int = 1,
+                 return_scores: bool = False):
+        """PaddleNLP GenerationMixin.generate for greedy search, sampling and beam search (generation/utils.py): prefill
+        with use_cache, then one decode step per token; returns [B, S + n_new] token ids. Prompts of different lengths
+        are LEFT-padded (attention_mask zeros in front), so that every prompt ends at column S - 1.
 
         Greedy search (the default) takes the argmax. do_sample=True or decode_strategy="sampling" draws from
         softmax(logits / temperature) after top_k / top_p filtering; repetition_penalty applies to both. eos_token_id is
@@ -584,7 +588,31 @@ class Qwen2VLForConditionalGeneration:
         the device (b200mix_sample_tokens).
 
         Calls that use none of penalty, sampling, an eos list or pad_token_id keep plain greedy decoding, which does
-        not pad sequences that have finished."""
+        not pad sequences that have finished.
+
+        decode_strategy="beam_search" keeps num_beams (2 .. 16) beams per prompt (BeamSearchScorer, GNMT length penalty
+        ((len + 5) / 6) ** length_penalty, early_stopping, diversity_rate for diverse sibling search) and returns the
+        num_return_sequences best hypotheses of prompt b in rows b * num_return_sequences ... (b + 1) *
+        num_return_sequences - 1, each ended by eos_token_id (one int or None) when it fits and padded with
+        pad_token_id (default eos_token_id); return_scores=True also returns their fp32 scores [B *
+        num_return_sequences]. Beam search applies repetition_penalty and ignores do_sample, temperature, top_k, top_p
+        and generator, as the reference's beam branch does. The prompt is prefilled once per prompt; after that, token
+        selection and KV-cache reordering run on the device inside the graphed decode step
+        (b200mix_beam_search_step, b200mix_kv_reorder)."""
+        if decode_strategy == "beam_search" or num_beams != 1:
+            from ..beam_search import resolve_beam_search_args
+            if decode_strategy != "beam_search":
+                raise ValueError(f"num_beams={num_beams} needs decode_strategy='beam_search'")
+            bargs = resolve_beam_search_args(num_beams, num_return_sequences, length_penalty, early_stopping,
+                                             diversity_rate, num_beam_groups, repetition_penalty, eos_token_id,
+                                             pad_token_id)
+            if attention_mask is not None and not bool((attention_mask[:, -1] == 1).all()):
+                raise ValueError("generate(): pad on the left (the last column of attention_mask must be all ones)")
+            ids, scores = self._generate_beam_search(input_ids, pixel_values, image_grid_thw, max_new_tokens,
+                                                     attention_mask, bargs)
+            return (ids, scores) if return_scores else ids
+        if return_scores:
+            raise ValueError("return_scores=True needs decode_strategy='beam_search'")
         from ..sampling import resolve_generation_args, seed_from
         args = resolve_generation_args(decode_strategy, do_sample, temperature, top_k, top_p, repetition_penalty,
                                        eos_token_id, pad_token_id)
@@ -636,5 +664,30 @@ class Qwen2VLForConditionalGeneration:
                 stepper.step()
         n = sampler.n_generated()
         return torch.cat([input_ids.cpu(), sampler.out[:, :n].cpu()], 1)
+
+    def _generate_beam_search(self, input_ids, pixel_values, image_grid_thw, max_new_tokens, attention_mask, args):
+        """generate() with beam search: one prefill at B rows, the cache, key mask and rope deltas expanded to B * nb
+        rows, selection step 0 on the expanded last logits row, then graph replays of decode + selection + cache
+        reorder; the host reads the all-done flag once every FINISH_CHECK_INTERVAL steps."""
+        from ..beam_search import BeamSearcher, expand_cache
+        from ..sampling import FINISH_CHECK_INTERVAL
+        if max_new_tokens < 1:
+            raise ValueError(f"max_new_tokens must be >= 1, got {max_new_tokens}")
+        nb = args.num_beams
+        self.cache_headroom = max_new_tokens
+        out = self.forward(input_ids=input_ids, attention_mask=attention_mask, pixel_values=pixel_values,
+                           image_grid_thw=image_grid_thw, use_cache=True)
+        cache = expand_cache(out.past_key_values, nb)
+        deltas = out.rope_deltas.repeat_interleave(nb, 0)
+        searcher = BeamSearcher(input_ids, self.config.vocab_size, max_new_tokens, args, cache, self.device)
+        searcher(out.logits[:, -1].repeat_interleave(nb, 0))
+        del out
+        if max_new_tokens > 1:
+            stepper = GraphedDecodeStep(self, cache, deltas, sampler=searcher)
+            for i in range(1, max_new_tokens):
+                if i % FINISH_CHECK_INTERVAL == 0 and searcher.all_done():
+                    break
+                stepper.step()
+        return searcher.finalize()
 
     __call__ = forward
