@@ -1,0 +1,142 @@
+"""The Llama-family causal decoder shared by Qwen2-VL's LLM (with a qkv bias) and Llama (without): parameter names, the
+device weight layout, the 1-D RoPE table and one layer loop on the sm_90a kernels.
+
+Per layer: RMSNorm -> fused q|k|v GEMM (+bias) -> attention -> o_proj GEMM (+residual) -> RMSNorm -> gate|up GEMM with
+SwiGLU epilogue (interleaved rows) -> down GEMM (+residual); then the final RMSNorm and the lm_head GEMM with fp32
+output. Only the attention differs between prefill() (RoPE in place, optional KV-cache fill, causal or masked flash
+attention) and decode() (one token per sequence, every position on the device: CUDA-graph capturable).
+"""
+from typing import Dict
+
+import torch
+
+from .ppdiffusers.unet_2d_condition import _to_t
+
+bf16 = torch.bfloat16
+
+
+def rope_cos_sin(theta: float, head_dim: int, n_positions: int):
+    """Rotary table (rotate_half convention) for positions 0 .. n_positions - 1: fp32 host cos, sin
+    [n_positions, head_dim], each row cat([f, f]) of position * inv_freq."""
+    inv_freq = 1.0 / (theta ** (torch.arange(0, head_dim, 2, dtype=torch.float32) / head_dim))
+    freqs = torch.arange(n_positions, dtype=torch.float32)[:, None] * inv_freq[None]
+    emb = torch.cat([freqs, freqs], -1)
+    return emb.cos(), emb.sin()
+
+
+class CausalDecoder:
+    """Embedding table, decoder layers, final norm and lm_head. Parameters are `{prefix}.embed_tokens`,
+    `{prefix}.layers.{i}.*`, `{prefix}.norm` and `lm_head` in the Paddle Linear layout ([in, out]); on the device q|k|v
+    rows are fused, up / gate rows interleaved, GEMM weights bf16 [N, K], norm weights and biases fp32."""
+
+    def __init__(self, config, prefix: str, qkv_bias: bool):
+        self.config, self.prefix, self.qkv_bias = config, prefix, qkv_bias
+        self.head_dim = config.hidden_size // config.num_attention_heads
+
+    def state_dict_shapes(self) -> Dict[str, tuple]:
+        c, p = self.config, self.prefix
+        H, I = c.hidden_size, c.intermediate_size
+        kv = c.num_key_value_heads * self.head_dim
+        S = {f"{p}.embed_tokens.weight": (c.vocab_size, H)}
+        for i in range(c.num_hidden_layers):
+            b = f"{p}.layers.{i}"
+            S[b + ".input_layernorm.weight"] = S[b + ".post_attention_layernorm.weight"] = (H,)
+            for name, out in (("q_proj", H), ("k_proj", kv), ("v_proj", kv)):
+                S[f"{b}.self_attn.{name}.weight"] = (H, out)
+                if self.qkv_bias:
+                    S[f"{b}.self_attn.{name}.bias"] = (out,)
+            S[b + ".self_attn.o_proj.weight"] = (H, H)
+            S[b + ".mlp.gate_proj.weight"] = S[b + ".mlp.up_proj.weight"] = (H, I)
+            S[b + ".mlp.down_proj.weight"] = (I, H)
+        S[f"{p}.norm.weight"] = (H,)
+        S["lm_head.weight"] = (H, c.vocab_size)
+        return S
+
+    def load_state_dict(self, P: Dict[str, object], dev: torch.device):
+        c, p = self.config, self.prefix
+
+        def W(name):  # Paddle [in, out] -> [out, in] fp32
+            return _to_t(P[name + ".weight"]).t().contiguous()
+
+        def vec(name):
+            return _to_t(P[name]).contiguous().to(dev)
+
+        self.embed = _to_t(P[f"{p}.embed_tokens.weight"]).contiguous().to(dev, bf16)
+        self.layers = []
+        for i in range(c.num_hidden_layers):
+            b = f"{p}.layers.{i}"
+            qkv = [f"{b}.self_attn.{n}_proj" for n in "qkv"]
+            gate, up = W(b + ".mlp.gate_proj"), W(b + ".mlp.up_proj")  # [I, H] each
+            gu = torch.stack([up, gate], 1).reshape(2 * up.shape[0], -1)  # interleave: 2j = up (value), 2j+1 = gate
+            self.layers.append(dict(
+                ln1=vec(b + ".input_layernorm.weight"), ln2=vec(b + ".post_attention_layernorm.weight"),
+                qkv=torch.cat([W(n) for n in qkv], 0).to(dev, bf16),
+                qkv_bias=torch.cat([_to_t(P[n + ".bias"]) for n in qkv], 0).to(dev) if self.qkv_bias else None,
+                o=W(b + ".self_attn.o_proj").to(dev, bf16), gu=gu.to(dev, bf16), down=W(b + ".mlp.down_proj").to(dev, bf16)))
+        self.norm_w = vec(f"{p}.norm.weight")
+        self.lm_head = W("lm_head").to(dev, bf16)
+        return self
+
+    def _layers(self, x, attention):
+        """x bf16 [M, hidden] -> fp32 logits [M, vocab]; attention(layer index, qkv [M, q|k|v]) -> bf16 [M, heads *
+        head_dim]. Kernel launches only."""
+        from . import ops
+        from ._lib import GLU_SWIGLU
+        eps = self.config.rms_norm_eps
+        for li, L in enumerate(self.layers):
+            h1 = ops.layernorm(x, L["ln1"], None, eps=eps, rms=True)
+            a = attention(li, ops.linear(h1, L["qkv"], L["qkv_bias"]))
+            x = ops.linear(a, L["o"], residual=x)
+            h2 = ops.layernorm(x, L["ln2"], None, eps=eps, rms=True)
+            x = ops.linear(ops.linear(h2, L["gu"], glu=GLU_SWIGLU), L["down"], residual=x)  # silu(gate) * up
+        hN = ops.layernorm(x, self.norm_w, None, eps=eps, rms=True)
+        return ops.linear(hN, self.lm_head, out_fp32=True)
+
+    def prefill(self, x, B, S, cos, sin, cache=None, attn_bias=None):
+        """x bf16 [B*S, hidden] input embeddings, cos / sin fp32 [B*S, head_dim]; cache: a KVCache to fill with the RoPE'd
+        K and V (its length becomes S); attn_bias: additive [B, 1, S, S] mask of a padded batch (causality included) or
+        None for the causal mask. Returns fp32 logits [B, S, vocab]."""
+        from . import ops
+        c, hd = self.config, self.head_dim
+        nh, nkv = c.num_attention_heads, c.num_key_value_heads
+        qd, kvd = nh * hd, nkv * hd
+        if cache is not None:
+            if cache.batch != B or cache.max_len < S:
+                raise ValueError(f"KV cache [{cache.batch}, {cache.max_len}] cannot hold a [{B}, {S}] prefill")
+            cache.length = S
+
+        def attention(li, qkv):
+            q = qkv[:, :qd].unflatten(-1, (nh, hd))
+            k = qkv[:, qd:qd + kvd].unflatten(-1, (nkv, hd))
+            v = qkv[:, qd + kvd:].unflatten(-1, (nkv, hd))
+            ops.rope_inplace(q, cos, sin)
+            ops.rope_inplace(k, cos, sin)
+            if cache is not None:
+                cache.k[li][:, :S].copy_(k.unflatten(0, (B, S)))
+                cache.v[li][:, :S].copy_(v.unflatten(0, (B, S)))
+            a = ops.sdpa(q.unflatten(0, (B, S)), k.unflatten(0, (B, S)), v.unflatten(0, (B, S)), scale=hd ** -0.5,
+                         causal=attn_bias is None, attn_mask=attn_bias)
+            return a.reshape(B * S, qd)
+        return self._layers(x, attention).reshape(B, S, c.vocab_size)
+
+    def decode(self, ids, cos, sin, cache, rows, kv_lens):
+        """One token per sequence against `cache`: ids int64 [B], cos / sin fp32 [B, head_dim] for its position, rows
+        int64 [B] = b * max_len + position (the flattened cache row its K / V go to), kv_lens int32 [B] = position + 1,
+        all on the device. The G = heads / kv_heads query heads that share a KV head are presented to the attention
+        kernel as G query rows of ONE head (Sq = G, Hq = Hkv): one K / V stream per KV head instead of one per query
+        head. Returns fp32 logits [B, vocab]; advancing cache.length is the caller's job."""
+        from . import ops
+        c, hd = self.config, self.head_dim
+        nh, nkv = c.num_attention_heads, c.num_key_value_heads
+        G, qd, kvd = nh // nkv, nh * hd, nkv * hd
+        B = ids.shape[0]
+        kb = None if cache.key_bias is None else cache.key_bias[:, None, None, :]
+
+        def attention(li, qkv):
+            ops.decode_rope_cache(qkv, nh, nkv, hd, cos, sin, rows, cache.k[li].view(-1, kvd), cache.v[li].view(-1, kvd))
+            a = torch.empty(B, qd, device=qkv.device, dtype=bf16)
+            qg = qkv.as_strided((B, G, nkv, hd), (qkv.stride(0), hd, G * hd, 1), qkv.storage_offset())
+            ag = a.as_strided((B, G, nkv, hd), (qd, hd, G * hd, 1))
+            ops.sdpa(qg, cache.k[li], cache.v[li], scale=hd ** -0.5, kv_lens=kv_lens, attn_mask=kb, out=ag)
+            return a
+        return self._layers(ops.gather_rows(self.embed, ids), attention)

@@ -4,16 +4,18 @@
 (clip_encoder.py:49-57) -> mm_projector mlp2x_gelu (mm_projector.py:45-58) -> image features spliced in place of each
 sample's IMAGE_TOKEN_INDEX placeholder -> causal prefill -> fp32 logits.
 
-Device graph per decoder layer: RMSNorm -> fused q|k|v GEMM (no bias) -> RoPE in place (rotate_half, fp32 math) ->
-causal GQA flash attention (d = 128) -> o_proj GEMM (+residual) -> RMSNorm -> gate|up GEMM with the SwiGLU epilogue
-(interleaved rows) -> down GEMM (+residual). SURVEY.md §8 row a19.
+The decoder is paddlemix_b200.decoder.CausalDecoder without the qkv bias, run as its prefill. Device graph per decoder
+layer: RMSNorm -> fused q|k|v GEMM -> RoPE in place (rotate_half, fp32 math) -> causal GQA flash attention (d = 128) ->
+o_proj GEMM (+residual) -> RMSNorm -> gate|up GEMM with the SwiGLU epilogue (interleaved rows) -> down GEMM
+(+residual). SURVEY.md §8 row a19.
 """
 from types import SimpleNamespace
-from typing import Any, Dict, Optional, Union
+from typing import Any, Dict, Union
 
 import torch
 
 from ..clip import CLIPVisionModel
+from ..decoder import CausalDecoder, rope_cos_sin
 from ..ppdiffusers.unet_2d_condition import FrozenDict, _to_t
 
 bf16 = torch.bfloat16
@@ -37,23 +39,13 @@ class LlamaForCausalLM:
                              f"`num_heads`: {c.num_attention_heads}).")
         if self.head_dim not in (64, 128):
             raise NotImplementedError("Llama(b200): head_dim must be 64 or 128")
+        self.decoder = CausalDecoder(c, self.PREFIX, qkv_bias=False)
         self.device, self.dtype = None, bf16
 
     EMBEDDING_KEYS = ("embed_tokens.weight",)
 
     def state_dict_shapes(self) -> Dict[str, tuple]:
-        c, p = self.config, self.PREFIX
-        H, I = c.hidden_size, c.intermediate_size
-        kv = c.num_key_value_heads * self.head_dim
-        S = {f"{p}.embed_tokens.weight": (c.vocab_size, H), f"{p}.norm.weight": (H,), "lm_head.weight": (H, c.vocab_size)}
-        for i in range(c.num_hidden_layers):
-            b = f"{p}.layers.{i}"
-            S[b + ".input_layernorm.weight"] = S[b + ".post_attention_layernorm.weight"] = (H,)
-            S[b + ".self_attn.q_proj.weight"], S[b + ".self_attn.o_proj.weight"] = (H, H), (H, H)
-            S[b + ".self_attn.k_proj.weight"] = S[b + ".self_attn.v_proj.weight"] = (H, kv)
-            S[b + ".mlp.gate_proj.weight"] = S[b + ".mlp.up_proj.weight"] = (H, I)
-            S[b + ".mlp.down_proj.weight"] = (I, H)
-        return S
+        return self.decoder.state_dict_shapes()
 
     def load_state_dict(self, P: Dict[str, Any], device: Union[int, str] = 0):
         from .. import ops
@@ -63,63 +55,24 @@ class LlamaForCausalLM:
         missing = [k for k in self.state_dict_shapes() if k not in P]
         if missing:
             raise KeyError(f"state dict is missing {len(missing)} parameters, e.g. {missing[:3]}")
-        c, p = self.config, self.PREFIX
-
-        def W(n):
-            return _to_t(P[n + ".weight"]).t().contiguous()
-
-        self.embed = _to_t(P[f"{p}.embed_tokens.weight"]).to(dev, bf16).contiguous()
-        self.layers = []
-        for i in range(c.num_hidden_layers):
-            b = f"{p}.layers.{i}"
-            wqkv = torch.cat([W(b + ".self_attn.q_proj"), W(b + ".self_attn.k_proj"), W(b + ".self_attn.v_proj")], 0)
-            gate, up = W(b + ".mlp.gate_proj"), W(b + ".mlp.up_proj")
-            gu = torch.stack([up, gate], 1).reshape(2 * up.shape[0], -1)  # interleave: 2j = up (value), 2j+1 = gate
-            self.layers.append(dict(ln1=_to_t(P[b + ".input_layernorm.weight"]).to(dev),
-                                    ln2=_to_t(P[b + ".post_attention_layernorm.weight"]).to(dev),
-                                    qkv=wqkv.to(dev, bf16).contiguous(), o=W(b + ".self_attn.o_proj").to(dev, bf16),
-                                    gu=gu.to(dev, bf16).contiguous(), down=W(b + ".mlp.down_proj").to(dev, bf16)))
-        self.norm_w = _to_t(P[f"{p}.norm.weight"]).to(dev)
-        self.lm_head = W("lm_head").to(dev, bf16)
+        self.decoder.load_state_dict(P, dev)
         return self
 
     def _rope_tables(self, S):
         """LlamaRotaryEmbedding: cos / sin fp32 [S, head_dim] for positions 0..S-1 (host index math)."""
-        hd = self.head_dim
-        inv = 1.0 / (self.config.rope_theta ** (torch.arange(0, hd, 2, dtype=torch.float32) / hd))
-        fr = torch.arange(S, dtype=torch.float32)[:, None] * inv[None]
-        emb = torch.cat([fr, fr], -1)
-        return emb.cos().contiguous().to(self.device), emb.sin().contiguous().to(self.device)
+        cos, sin = rope_cos_sin(self.config.rope_theta, self.head_dim, S)
+        return cos.to(self.device), sin.to(self.device)
 
     def prefill_embeds(self, x):
         """x: bf16 [B, S, H] input embeddings -> fp32 logits [B, S, vocab] (causal, positions 0..S-1)."""
-        from .. import ops
-        from .._lib import GLU_SWIGLU
-        c, hd = self.config, self.head_dim
         B, S, H = x.shape
-        nh, nkv = c.num_attention_heads, c.num_key_value_heads
-        qd, kvd = nh * hd, nkv * hd
         cos, sin = self._rope_tables(S)
-        cos, sin = cos.repeat(B, 1), sin.repeat(B, 1)  # one row per token of the flattened [B*S] axis
-        x = x.reshape(B * S, H).contiguous()
-        for L in self.layers:
-            h1 = ops.layernorm(x, L["ln1"], None, eps=c.rms_norm_eps, rms=True)
-            qkv = ops.linear(h1, L["qkv"])
-            q = qkv[:, :qd].unflatten(-1, (nh, hd))
-            k = qkv[:, qd:qd + kvd].unflatten(-1, (nkv, hd))
-            v = qkv[:, qd + kvd:].unflatten(-1, (nkv, hd))
-            ops.rope_inplace(q, cos, sin)
-            ops.rope_inplace(k, cos, sin)
-            a = ops.sdpa(q.unflatten(0, (B, S)), k.unflatten(0, (B, S)), v.unflatten(0, (B, S)), scale=hd ** -0.5, causal=True)
-            x = ops.linear(a.reshape(B * S, qd), L["o"], residual=x)
-            h2 = ops.layernorm(x, L["ln2"], None, eps=c.rms_norm_eps, rms=True)
-            x = ops.linear(ops.linear(h2, L["gu"], glu=GLU_SWIGLU), L["down"], residual=x)
-        hN = ops.layernorm(x, self.norm_w, None, eps=c.rms_norm_eps, rms=True)
-        return ops.linear(hN, self.lm_head, out_fp32=True).reshape(B, S, c.vocab_size)
+        # one cos / sin row per token of the flattened [B*S] axis
+        return self.decoder.prefill(x.reshape(B * S, H).contiguous(), B, S, cos.repeat(B, 1), sin.repeat(B, 1))
 
     def embed_tokens(self, ids_dev):
         from .. import ops
-        return ops.gather_rows(self.embed, ids_dev.reshape(-1))
+        return ops.gather_rows(self.decoder.embed, ids_dev.reshape(-1))
 
     def forward(self, input_ids=None, inputs_embeds=None, attention_mask=None, return_dict=True):
         if self.device is None:

@@ -6,9 +6,11 @@ Device graph (one process per GPU, every arithmetic op is a libb200mix kernel):
   in place (fp32 math, rotate_half) -> varlen block-diagonal flash attention (cu_seqlens) -> proj GEMM (+bias,
   +residual) -> LayerNorm -> fc1 GEMM + quick_gelu -> fc2 GEMM (+residual) }; PatchMerger LN -> GEMM+GELU -> GEMM.
   ViT heads are 80 wide: q/k/v rows and proj columns are zero-padded to 128 once at load time (exact).
-  LLM (:813-889): 28 x { RMSNorm -> fused q|k|v GEMM (+bias) -> M-RoPE in place -> causal GQA flash attention
-  (28 q heads / 4 kv heads, d=128) -> o_proj GEMM (+residual) -> RMSNorm -> gate|up GEMM with SwiGLU epilogue
-  (interleaved rows) -> down GEMM (+residual) }; final RMSNorm; lm_head GEMM with fp32 output.
+  LLM (:813-889): paddlemix_b200.decoder.CausalDecoder with the qkv bias: 28 x { RMSNorm -> fused q|k|v GEMM (+bias)
+  -> M-RoPE in place -> causal GQA flash attention (28 q heads / 4 kv heads, d=128) -> o_proj GEMM (+residual) ->
+  RMSNorm -> gate|up GEMM with SwiGLU epilogue (interleaved rows) -> down GEMM (+residual) }; final RMSNorm; lm_head
+  GEMM with fp32 output. Prefill, eager decode and the CUDA-graph decode step all run that one layer loop; both decode
+  paths run the same single-token body (fused RoPE + cache write, GQA-folded attention over the cache).
 Host side (pure index math, no arithmetic on activations): get_rope_index (:1217-1360), rot_pos_emb (:940-971),
 the cos/sin tables of both rotary embeddings.
 """
@@ -18,6 +20,7 @@ from typing import Any, Dict, List, Optional, Union
 
 import torch
 
+from ..decoder import CausalDecoder, rope_cos_sin
 from ..ppdiffusers.unet_2d_condition import FrozenDict, _to_t
 
 bf16 = torch.bfloat16
@@ -84,16 +87,15 @@ class GraphedDecodeStep:
 
     def __init__(self, model, cache: KVCache, rope_deltas, warmup: int = 2, sampler=None):
         from .. import ops
+        if cache.length + warmup > cache.max_len:  # the warm-up steps write cache rows length .. length + warmup - 1
+            raise ValueError(f"KV cache has {cache.max_len - cache.length} free positions, the graph's warm-up needs {warmup}")
         self.model, self.cache, self.sampler = model, cache, sampler
         dev, B, hd = model.device, cache.batch, model.head_dim
-        c = model.config
         P = cache.length
         deltas = torch.zeros(B, dtype=torch.long) if rope_deltas is None else rope_deltas.reshape(B).cpu().long()
         n_pos = cache.max_len + int(deltas.max().clamp(min=0)) + 2
-        inv_freq = 1.0 / (c.rope_theta ** (torch.arange(0, hd, 2, dtype=torch.float32) / hd))
-        fr = torch.arange(n_pos, dtype=torch.float32)[:, None] * inv_freq[None]
-        emb = torch.cat([fr, fr], -1)
-        self.cos_table, self.sin_table = emb.cos().contiguous().to(dev), emb.sin().contiguous().to(dev)
+        cos, sin = rope_cos_sin(model.config.rope_theta, hd, n_pos)
+        self.cos_table, self.sin_table = cos.to(dev), sin.to(dev)
         self.ids = torch.zeros(B, dtype=torch.long, device=dev) if sampler is None else sampler.ids
         self.pos = (P + deltas).clamp(min=0).to(dev)
         self.rows = (torch.arange(B) * cache.max_len + P).to(dev)
@@ -104,7 +106,7 @@ class GraphedDecodeStep:
         def body():
             torch.index_select(self.cos_table, 0, self.pos, out=self.cos)  # row gathers (no arithmetic on activations)
             torch.index_select(self.sin_table, 0, self.pos, out=self.sin)
-            logits = model.decode_body_static(self.ids, self.cos, self.sin, cache, self.rows, self.kv_lens)
+            logits = model.decoder.decode(self.ids, self.cos, self.sin, cache, self.rows, self.kv_lens)
             self.pos.add_(1), self.rows.add_(1), self.kv_lens.add_(1)  # index bookkeeping advances on the device
             return logits
 
@@ -171,13 +173,14 @@ class Qwen2VLForConditionalGeneration:
             raise NotImplementedError("Qwen2VL(b200): LLM head_dim must be 64 or 128")
         self.v_head = c.vision["embed_dim"] // c.vision["num_heads"]
         self.v_pad = 64 if self.v_head <= 64 else 128
+        self.decoder = CausalDecoder(c, "model", qkv_bias=True)
         self.dtype = bf16
         self.device = None
 
     # ------------------------------------------------------------------------------------------------------------
     def state_dict_shapes(self) -> Dict[str, tuple]:
         c, v = self.config, self.config.vision
-        E, H, I = v["embed_dim"], c.hidden_size, c.intermediate_size
+        E, H = v["embed_dim"], c.hidden_size
         S: Dict[str, tuple] = {}
 
         def lin(name, i, o, bias=True):
@@ -195,18 +198,7 @@ class Qwen2VLForConditionalGeneration:
         m = E * v["spatial_merge_size"] ** 2
         S["visual.merger.ln_q.weight"], S["visual.merger.ln_q.bias"] = (E,), (E,)
         lin("visual.merger.mlp.0", m, m), lin("visual.merger.mlp.2", m, H)
-        S["model.embed_tokens.weight"] = (c.vocab_size, H)
-        kv = c.num_key_value_heads * self.head_dim
-        for i in range(c.num_hidden_layers):
-            b = f"model.layers.{i}"
-            S[b + ".input_layernorm.weight"] = (H,)
-            S[b + ".post_attention_layernorm.weight"] = (H,)
-            lin(b + ".self_attn.q_proj", H, H), lin(b + ".self_attn.k_proj", H, kv), lin(b + ".self_attn.v_proj", H, kv)
-            lin(b + ".self_attn.o_proj", H, H, bias=False)
-            lin(b + ".mlp.gate_proj", H, I, bias=False), lin(b + ".mlp.up_proj", H, I, bias=False)
-            lin(b + ".mlp.down_proj", I, H, bias=False)
-        S["model.norm.weight"] = (H,)
-        lin("lm_head", H, c.vocab_size, bias=False)
+        S.update(self.decoder.state_dict_shapes())
         return S
 
     def default_missing_parameters(self, sd) -> Dict[str, Any]:
@@ -241,7 +233,7 @@ class Qwen2VLForConditionalGeneration:
         missing = [k for k in self.state_dict_shapes() if k not in P]
         if missing:
             raise KeyError(f"state dict is missing {len(missing)} parameters, e.g. {missing[:3]}")
-        c, v = self.config, self.config.vision
+        v = self.config.vision
         E, nh = v["embed_dim"], v["num_heads"]
         d, dp = self.v_head, self.v_pad
 
@@ -273,19 +265,7 @@ class Qwen2VLForConditionalGeneration:
         self.merger = dict(ln=(dv(_to_t(P["visual.merger.ln_q.weight"])), dv(Bv("visual.merger.ln_q"))),
                            m0=(dv(W("visual.merger.mlp.0"), bf16), dv(Bv("visual.merger.mlp.0"))),
                            m2=(dv(W("visual.merger.mlp.2"), bf16), dv(Bv("visual.merger.mlp.2"))))
-        self.embed = dv(_to_t(P["model.embed_tokens.weight"]), bf16)
-        self.layers = []
-        for i in range(c.num_hidden_layers):
-            b = f"model.layers.{i}"
-            wqkv = torch.cat([W(b + ".self_attn.q_proj"), W(b + ".self_attn.k_proj"), W(b + ".self_attn.v_proj")], 0)
-            bqkv = torch.cat([Bv(b + ".self_attn.q_proj"), Bv(b + ".self_attn.k_proj"), Bv(b + ".self_attn.v_proj")], 0)
-            gate, up = W(b + ".mlp.gate_proj"), W(b + ".mlp.up_proj")  # [I, H] each
-            gu = torch.stack([up, gate], 1).reshape(2 * up.shape[0], -1)  # interleave: 2j = up (value), 2j+1 = gate
-            self.layers.append(dict(ln1=dv(_to_t(P[b + ".input_layernorm.weight"])), ln2=dv(_to_t(P[b + ".post_attention_layernorm.weight"])),
-                                    qkv=(dv(wqkv, bf16), dv(bqkv)), o=dv(W(b + ".self_attn.o_proj"), bf16),
-                                    gu=dv(gu, bf16), down=dv(W(b + ".mlp.down_proj"), bf16)))
-        self.norm_w = dv(_to_t(P["model.norm.weight"]))
-        self.lm_head = dv(W("lm_head"), bf16)
+        self.decoder.load_state_dict(P, dev)
         return self
 
     # ------------------------------------------------------------------------------------------------------------
@@ -356,11 +336,8 @@ class Qwen2VLForConditionalGeneration:
     def _mrope_tables(self, position_ids):
         """Qwen2RotaryEmbedding (:136-166) + section gather (:212-220) -> cos, sin fp32 [B*S, head_dim] on device."""
         c, hd = self.config, self.head_dim
-        inv_freq = 1.0 / (c.rope_theta ** (torch.arange(0, hd, 2, dtype=torch.float32) / hd))
-        n = int(position_ids.max()) + 1
-        freqs = torch.einsum("i,j->ij", torch.arange(n, dtype=torch.float32), inv_freq)
-        emb = torch.cat([freqs, freqs], -1)
-        cos, sin = emb.cos()[position_ids], emb.sin()[position_ids]
+        cos, sin = rope_cos_sin(c.rope_theta, hd, int(position_ids.max()) + 1)
+        cos, sin = cos[position_ids], sin[position_ids]
         sec = list(c.mrope_section) * 2
         cos = torch.cat([x[i % 3] for i, x in enumerate(cos.split(sec, -1))], -1)
         sin = torch.cat([x[i % 3] for i, x in enumerate(sin.split(sec, -1))], -1)
@@ -425,16 +402,24 @@ class Qwen2VLForConditionalGeneration:
         B, S = ids_host.shape
         ids_dev = ids_host.to(dev).reshape(-1).contiguous()
         if past_key_values is not None and past_key_values.length > 0:
-            # ---- decode: one new token per sequence against the cache ----
+            # ---- decode: one new token per sequence against the cache, the body GraphedDecodeStep captures ----
+            cache, P = past_key_values, past_key_values.length
             if S != 1 or pixel_values is not None:
                 raise NotImplementedError("decode takes exactly one new token per sequence and no new images")
+            if B != cache.batch:
+                raise ValueError(f"decode got {B} sequences for a KV cache of {cache.batch}")
             if position_ids is None:
                 if rope_deltas is None:
                     raise ValueError("decode needs the rope_deltas returned by the prefill call (or explicit position_ids)")
-                pos = past_key_values.length + rope_deltas.reshape(B, 1).cpu().long()  # arange(1) + cache_position + delta
+                pos = P + rope_deltas.reshape(B, 1).cpu().long()  # arange(1) + cache_position + delta
                 position_ids = pos.unsqueeze(0).expand(3, -1, -1)
+            if P + 1 > cache.max_len:
+                raise ValueError(f"KV cache is full ({cache.max_len} positions)")
             cos, sin = self._mrope_tables(position_ids.cpu())
-            logits = self.decode_device(ids_dev, B, cos, sin, past_key_values).reshape(B, 1, c.vocab_size)
+            rows = (torch.arange(B) * cache.max_len + P).to(dev)
+            kv_lens = torch.full((B,), P + 1, dtype=torch.int32, device=dev)
+            logits = self.decoder.decode(ids_dev, cos, sin, cache, rows, kv_lens).reshape(B, 1, c.vocab_size)
+            cache.length = P + 1
             if return_dict is False:
                 return (logits, past_key_values)
             return Qwen2VLCausalLMOutputWithPast(logits=logits, past_key_values=past_key_values, rope_deltas=rope_deltas)
@@ -470,102 +455,16 @@ class Qwen2VLForConditionalGeneration:
         ids_dev int64 [B*S]; cos/sin fp32 [B*S, head_dim] (M-RoPE tables); image_idx int64 [n_image_tokens]; attn_bias =
         additive [B, 1, S, S] mask of a padded batch (causality included) or None for the plain causal mask."""
         from .. import ops
-        from .._lib import GLU_SWIGLU
-        c, hd = self.config, self.head_dim
-        nh, nkv = c.num_attention_heads, c.num_key_value_heads
-        x = ops.gather_rows(self.embed, ids_dev)  # [B*S, H]  (embed_tokens, :1443)
+        x = ops.gather_rows(self.decoder.embed, ids_dev)  # [B*S, H]  (embed_tokens, :1443)
         if pixel_values is not None:
             image_embeds = self.visual(pixel_values, image_grid_thw)
             if image_idx.numel() != image_embeds.shape[0]:
                 raise ValueError(f"Image features and image tokens do not match: tokens: {image_idx.numel()}, "
                                  f"features {image_embeds.shape[0]}")
             ops.scatter_rows(image_embeds, image_idx, x)  # inputs_embeds[image_mask] = image_embeds (:1449-1452)
-        qd, kvd = nh * hd, nkv * hd
-        if cache is not None:
-            if cache.batch != B or cache.max_len < S:
-                raise ValueError(f"KV cache [{cache.batch}, {cache.max_len}] cannot hold a [{B}, {S}] prefill")
-            cache.length = S
-        for li, L in enumerate(self.layers):
-            h1 = ops.layernorm(x, L["ln1"], None, eps=c.rms_norm_eps, rms=True)
-            qkv = ops.linear(h1, *L["qkv"])  # [B*S, qd + 2*kvd]
-            q = qkv[:, :qd].unflatten(-1, (nh, hd))
-            k = qkv[:, qd:qd + kvd].unflatten(-1, (nkv, hd))
-            vv = qkv[:, qd + kvd:].unflatten(-1, (nkv, hd))
-            ops.rope_inplace(q, cos, sin)
-            ops.rope_inplace(k, cos, sin)
-            if cache is not None:  # key_states / value_states after RoPE are what the reference caches (:591-596)
-                cache.k[li][:, :S].copy_(k.unflatten(0, (B, S)))
-                cache.v[li][:, :S].copy_(vv.unflatten(0, (B, S)))
-            a = ops.sdpa(q.unflatten(0, (B, S)), k.unflatten(0, (B, S)), vv.unflatten(0, (B, S)), scale=hd ** -0.5,
-                         causal=attn_bias is None, attn_mask=attn_bias)
-            x = ops.linear(a.reshape(B * S, qd), L["o"], residual=x)
-            h2 = ops.layernorm(x, L["ln2"], None, eps=c.rms_norm_eps, rms=True)
-            g = ops.linear(h2, L["gu"], glu=GLU_SWIGLU)  # silu(gate) * up
-            x = ops.linear(g, L["down"], residual=x)
-        hN = ops.layernorm(x, self.norm_w, None, eps=c.rms_norm_eps, rms=True)
-        return ops.linear(hN, self.lm_head, out_fp32=True).reshape(B, S, c.vocab_size)  # fp32 logits (:1474-1475)
-
-    def decode_device(self, ids_dev, B, cos, sin, cache: KVCache):
-        """One decode step (Qwen2VLDecoderLayer.forward :829-889 with a cache): ids_dev int64 [B] = the newest token of each
-        sequence, cos / sin fp32 [B, head_dim] for its position. Appends K / V at cache.length, attends over the
-        cache.length + 1 cached positions (GQA, no mask needed: everything cached is in the past), returns fp32 logits
-        [B, vocab] and advances the cache. Kernel launches only."""
-        from .. import ops
-        from .._lib import GLU_SWIGLU
-        c, hd = self.config, self.head_dim
-        nh, nkv = c.num_attention_heads, c.num_key_value_heads
-        P = cache.length
-        if P + 1 > cache.max_len:
-            raise ValueError(f"KV cache is full ({cache.max_len} positions)")
-        x = ops.gather_rows(self.embed, ids_dev)  # [B, H]
-        qd, kvd = nh * hd, nkv * hd
-        for li, L in enumerate(self.layers):
-            h1 = ops.layernorm(x, L["ln1"], None, eps=c.rms_norm_eps, rms=True)
-            qkv = ops.linear(h1, *L["qkv"])  # [B, qd + 2*kvd]
-            q = qkv[:, :qd].unflatten(-1, (nh, hd))
-            k = qkv[:, qd:qd + kvd].unflatten(-1, (nkv, hd))
-            vv = qkv[:, qd + kvd:].unflatten(-1, (nkv, hd))
-            ops.rope_inplace(q, cos, sin)
-            ops.rope_inplace(k, cos, sin)
-            cache.k[li][:, P].copy_(k)
-            cache.v[li][:, P].copy_(vv)
-            kb = None if cache.key_bias is None else cache.key_bias[:, None, None, :P + 1]
-            a = ops.sdpa(q.unsqueeze(1), cache.k[li][:, :P + 1], cache.v[li][:, :P + 1], scale=hd ** -0.5, attn_mask=kb)  # [B,1,nh,hd]
-            x = ops.linear(a.reshape(B, qd), L["o"], residual=x)
-            h2 = ops.layernorm(x, L["ln2"], None, eps=c.rms_norm_eps, rms=True)
-            g = ops.linear(h2, L["gu"], glu=GLU_SWIGLU)
-            x = ops.linear(g, L["down"], residual=x)
-        cache.length = P + 1
-        hN = ops.layernorm(x, self.norm_w, None, eps=c.rms_norm_eps, rms=True)
-        return ops.linear(hN, self.lm_head, out_fp32=True)
-
-    def decode_body_static(self, ids_dev, cos, sin, cache: KVCache, rows, kv_lens):
-        """decode_device with every position-dependent quantity on the DEVICE (CUDA-graph capturable): `rows` int64 [B] =
-        b * max_len + position of the new token (row of the flattened cache to write), `kv_lens` int32 [B] = keys to attend
-        to (position + 1). The G = heads / kv_heads query heads that share a KV head are presented to the attention kernel
-        as G query rows of ONE head (Sq = G, Hq = Hkv): one K / V stream per KV head instead of one per query head."""
-        from .. import ops
-        from .._lib import GLU_SWIGLU
-        c, hd = self.config, self.head_dim
-        nh, nkv = c.num_attention_heads, c.num_key_value_heads
-        G = nh // nkv
-        B = ids_dev.shape[0]
-        x = ops.gather_rows(self.embed, ids_dev)
-        qd, kvd = nh * hd, nkv * hd
-        for li, L in enumerate(self.layers):
-            h1 = ops.layernorm(x, L["ln1"], None, eps=c.rms_norm_eps, rms=True)
-            qkv = ops.linear(h1, *L["qkv"])
-            ops.decode_rope_cache(qkv, nh, nkv, hd, cos, sin, rows, cache.k[li].view(-1, kvd), cache.v[li].view(-1, kvd))
-            a = torch.empty(B, qd, device=x.device, dtype=bf16)
-            qg = qkv.as_strided((B, G, nkv, hd), (qkv.stride(0), hd, G * hd, 1), qkv.storage_offset())
-            ag = a.as_strided((B, G, nkv, hd), (qd, hd, G * hd, 1))
-            kb = None if cache.key_bias is None else cache.key_bias[:, None, None, :]
-            ops.sdpa(qg, cache.k[li], cache.v[li], scale=hd ** -0.5, kv_lens=kv_lens, attn_mask=kb, out=ag)
-            x = ops.linear(a, L["o"], residual=x)
-            h2 = ops.layernorm(x, L["ln2"], None, eps=c.rms_norm_eps, rms=True)
-            x = ops.linear(ops.linear(h2, L["gu"], glu=GLU_SWIGLU), L["down"], residual=x)
-        hN = ops.layernorm(x, self.norm_w, None, eps=c.rms_norm_eps, rms=True)
-        return ops.linear(hN, self.lm_head, out_fp32=True)
+        # the cache holds key_states / value_states after RoPE, as the reference's does (:591-596); fp32 logits over all
+        # positions (:1474-1475)
+        return self.decoder.prefill(x, B, S, cos, sin, cache=cache, attn_bias=attn_bias)
 
     @torch.no_grad()
     def generate(self, input_ids, pixel_values=None, image_grid_thw=None, max_new_tokens: int = 16, eos_token_id=None,
@@ -613,36 +512,33 @@ class Qwen2VLForConditionalGeneration:
             return (ids, scores) if return_scores else ids
         if return_scores:
             raise ValueError("return_scores=True needs decode_strategy='beam_search'")
-        from ..sampling import resolve_generation_args, seed_from
+        from ..sampling import FINISH_CHECK_INTERVAL, resolve_generation_args, seed_from
         args = resolve_generation_args(decode_strategy, do_sample, temperature, top_k, top_p, repetition_penalty,
                                        eos_token_id, pad_token_id)
-        B, S = input_ids.shape
         if attention_mask is not None and not bool((attention_mask[:, -1] == 1).all()):
             raise ValueError("generate(): pad on the left (the last column of attention_mask must be all ones)")
         if args.on_device:
             return self._generate_on_device(input_ids, pixel_values, image_grid_thw, max_new_tokens, attention_mask,
                                             args, seed_from(generator) if args.do_sample else 0)
+        # plain greedy: graph replays with a device argmax. With an int eos the host reads the tokens back once every
+        # FINISH_CHECK_INTERVAL steps; the result ends at the first step by which every row has produced the eos
         self.cache_headroom = max_new_tokens
         out = self.forward(input_ids=input_ids, attention_mask=attention_mask, pixel_values=pixel_values,
                            image_grid_thw=image_grid_thw, use_cache=True)
-        cache, deltas = out.past_key_values, out.rope_deltas
-        nxt = out.logits[:, -1].argmax(-1)
-        seq = [input_ids.cpu(), nxt.cpu().unsqueeze(1)]
-        done = torch.zeros(B, dtype=torch.bool)
-        if eos_token_id is None:
-            # no early stop: the whole continuation stays on the device (graph replays, device argmax, ONE final D2H)
-            stepper = GraphedDecodeStep(self, cache, deltas)
-            toks = [nxt]
-            for _ in range(max_new_tokens - 1):
+        toks = [out.logits[:, -1].argmax(-1)]
+        if max_new_tokens > 1:
+            stepper = GraphedDecodeStep(self, out.past_key_values, out.rope_deltas)
+            for i in range(1, max_new_tokens):
+                if (eos_token_id is not None and i % FINISH_CHECK_INTERVAL == 0
+                        and bool((torch.stack(toks, 1) == eos_token_id).any(1).all())):
+                    break
                 toks.append(stepper.step(toks[-1]).argmax(-1))
-            return torch.cat([input_ids.cpu(), torch.stack(toks, 1).cpu()], 1)
-        for _ in range(max_new_tokens - 1):
-            done |= seq[-1].squeeze(1) == eos_token_id
-            if bool(done.all()):
-                break
-            out = self.forward(input_ids=seq[-1], past_key_values=cache, rope_deltas=deltas, use_cache=True)
-            seq.append(out.logits[:, -1].argmax(-1).cpu().unsqueeze(1))
-        return torch.cat(seq, 1)
+        new = torch.stack(toks, 1).cpu()
+        if eos_token_id is not None:
+            all_seen = ((new == eos_token_id).cumsum(1) > 0).all(0)  # [n]: every row has an eos among its first j + 1
+            if bool(all_seen.any()):
+                new = new[:, :int(all_seen.nonzero()[0, 0]) + 1]
+        return torch.cat([input_ids.cpu(), new], 1)
 
     def _generate_on_device(self, input_ids, pixel_values, image_grid_thw, max_new_tokens, attention_mask, args, seed):
         """generate() with b200mix_sample_tokens: the prefill's last logits row gives the first token, then every

@@ -87,6 +87,28 @@ def test_qwen2vl_structure_and_rope_index_match_oracle():
     assert torch.equal(m.rot_pos_emb(grid), OQ.rot_pos_emb(cfg, grid))
 
 
+def test_llama_structure_matches_oracle():
+    from oracle import llama as OL
+    from paddlemix_b200.llava import LlamaForCausalLM
+    for name in ("tiny", "vicuna_7b"):
+        cfg = OL.LLAMA_CONFIGS[name]
+        assert LlamaForCausalLM(cfg).state_dict_shapes() == OL.llama_param_shapes(cfg)
+
+
+def test_graphed_decode_step_needs_room_for_its_warmup():
+    """The warm-up steps write cache rows length .. length + warmup - 1: a cache without that room is refused before
+    any device work (the stand-in cache has no tensors and the model no weights, so nothing could be launched)."""
+    from types import SimpleNamespace
+
+    from oracle import qwen2vl as OQ
+    from paddlemix_b200.qwen2_vl import GraphedDecodeStep, Qwen2VLForConditionalGeneration
+    model = Qwen2VLForConditionalGeneration(OQ.QWEN2VL_CONFIGS["tiny"])
+    for length, max_len, warmup in ((9, 10, 2), (10, 10, 2), (10, 10, 1), (3, 5, 3)):
+        cache = SimpleNamespace(length=length, max_len=max_len, batch=2, key_bias=None, k=None, v=None)
+        with pytest.raises(ValueError, match="warm-up"):
+            GraphedDecodeStep(model, cache, None, warmup=warmup)
+
+
 def test_stdit2_structure_matches_oracle():
     from oracle import stdit2 as OS2
     from paddlemix_b200.opensora import STDiT2

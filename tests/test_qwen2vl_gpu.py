@@ -108,16 +108,19 @@ def test_graphed_decode_step_matches_eager_and_oracle():
         eager = model(input_ids=new, past_key_values=out_a.past_key_values, rope_deltas=out_a.rope_deltas, use_cache=True).logits[:, 0]
         graphed = stepper.step(new.reshape(-1)).clone()
         assert out_b.past_key_values.get_seq_length() == S + step + 1
-        scale = eager.abs().max().item()
-        assert (graphed - eager).abs().max().item() <= 2e-2 * scale, (step, (graphed - eager).abs().max().item(), scale)
+        assert torch.equal(graphed, eager), step  # one decode body: the same kernels on the same inputs
         ref = O.qwen2vl_prefill(cfg, P, ids, pv, grid)[:, -1]
         o = graphed.cpu()
         cos = torch.nn.functional.cosine_similarity(o.flatten(), ref.flatten(), dim=0).item()
         assert cos >= 0.999 and (o - ref).abs().max().item() <= 0.04 * ref.abs().max().item(), (step, cos)
-    # greedy generate (no eos): the graphed continuation equals the eager one token for token
+    # greedy generate (no eos): the graphed continuation equals a host loop of eager decode steps token for token
     gen = model.generate(input_ids, pixel_values=pv.cuda(), image_grid_thw=torch.tensor(grid), max_new_tokens=6)
-    gen_e = model.generate(input_ids, pixel_values=pv.cuda(), image_grid_thw=torch.tensor(grid), max_new_tokens=6, eos_token_id=-1)
-    assert gen.shape == (B, S + 6) and torch.equal(gen, gen_e)
+    out = model(input_ids=input_ids, pixel_values=pv.cuda(), image_grid_thw=torch.tensor(grid), use_cache=True)
+    toks = [out.logits[:, -1].argmax(-1).cpu()]
+    for _ in range(5):
+        toks.append(model(input_ids=toks[-1][:, None], past_key_values=out.past_key_values, rope_deltas=out.rope_deltas,
+                          use_cache=True).logits[:, 0].argmax(-1).cpu())
+    assert gen.shape == (B, S + 6) and torch.equal(gen, torch.cat([input_ids, torch.stack(toks, 1)], 1))
 
 
 def _padded(cfg, grid, n_text, side, seed=7):
