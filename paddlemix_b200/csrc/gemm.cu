@@ -18,6 +18,7 @@
 #include <algorithm>
 #include <cstdlib>
 #include <mutex>
+#include <type_traits>
 
 namespace b200 {
 
@@ -59,13 +60,13 @@ struct IGemmParams {
   float ln_inv_k;             // 2^-24 / K
   // stream-K head (see SegIter): the first sk_tiles super-tiles are cut into equal k-block ranges, one per cluster
   int sk_tiles;
-  float4* sk_ws;          // [cluster][cta rank][chunk][8][128 rows] fp32 partial accumulators
+  float4* sk_ws;          // [cluster][cta rank][n8 block][consumer thread] fp32 partial accumulators (fragment layout)
   unsigned int* sk_flags; // [cluster][cta rank]: 1 = the partial of that CTA's tail piece is in sk_ws
 };
 
 // ---- work schedule -------------------------------------------------------------------------------------------------
 // A problem of T super-tiles (256 x BN) on C clusters needs ceil(T / C) rounds; SDXL's 8192 x 1280 projections have
-// T = 160 on C = 74: 2.16 rounds of work in 3 rounds of time. The schedule therefore starts with a STREAM-K head: the
+// T = 160 on the C = 66 clusters of 132 SMs: 2.42 rounds of work in 3 rounds of time. The schedule therefore starts with a STREAM-K head: the
 // first sk_tiles = C + (T mod C) tiles are laid end to end in units of one 64-deep k-block and cluster c takes the
 // contiguous unit range [c, c+1) * units / C (>= one whole tile, so a tile is shared by at most two clusters: its k
 // range splits into a HEAD piece = the last piece of cluster c and a TAIL piece = the first piece of cluster c + 1).
@@ -73,7 +74,7 @@ struct IGemmParams {
 // the head piece's epilogue - which runs (1 + T mod C / C) tiles later - adds them to its own accumulators and finishes
 // the tile (fixed split and fixed order: results are reproducible run to run). The remaining T - sk_tiles tiles (a
 // multiple of C) follow round-robin as before. Every cluster thus gets T / C tiles' worth of k-blocks.
-constexpr int SK_WS_FLOAT4_PER_CTA = 8 * 8 * 128;  // 8 chunks x 8 float4 x 128 rows = 128 KB
+constexpr int SK_WS_FLOAT4_PER_CTA = 32 * 256;  // <= 32 n8 blocks x 256 consumer threads x float4 = 128 KB
 enum { SEG_FULL = 0, SEG_TAIL = 1, SEG_HEAD = 2 };
 struct SegIter {
   int u, u1;        // stream-K unit range still to do
@@ -179,241 +180,22 @@ __device__ __forceinline__ float act_eval(float x, const ActCoef& a) {
   return x_sigmoid_neg_log2(x, x * fmaf(fmaf(a.c2, x2, a.c1), x2, a.c0));
 }
 
-// Global-memory operands of one 32-column chunk of one accumulator row.
-struct EpiOperands {  // direct (row-per-thread) path: GLU / fp32 output / unaligned or partial chunks
-  float4 bias[8];
-  bool vec;
-};
-
-__device__ __forceinline__ void epilogue_prefetch(const IGemmParams& p, EpiOperands& eo, const float* bias_c, int n_abs) {
-  eo.vec = (n_abs + 32 <= p.N) && p.vec_ok;
-  if (p.bias) {  // staged in shared memory by this warp (zeros past N)
-    const float4* b4 = reinterpret_cast<const float4*>(bias_c);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) eo.bias[j] = b4[j];
-  }
-}
-
-// One 32-column chunk of one accumulator row -> global memory.
-__device__ __forceinline__ void epilogue_chunk(const IGemmParams& p, const ActCoef& ac, const uint32_t (&r)[32],
-                                               const EpiOperands& eo, long long c_off, long long r_off, long long g,
-                                               int n_abs) {
-  float v[32];
-#pragma unroll
-  for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-  const bool full = (n_abs + 32 <= p.N);
-  const bool vec = eo.vec;
-
-  if (p.bias) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      v[4 * j + 0] += eo.bias[j].x, v[4 * j + 1] += eo.bias[j].y, v[4 * j + 2] += eo.bias[j].z,
-          v[4 * j + 3] += eo.bias[j].w;
-    }
-  }
-  if (p.row_add) {
-    const float* ra = p.row_add + g * p.ld_row + n_abs;
-#pragma unroll
-    for (int j = 0; j < 32; ++j)
-      if (full || n_abs + j < p.N) v[j] += __ldg(ra + j);
-  }
-  if (p.act != B200MIX_ACT_NONE && !p.glu) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = act_eval(v[j], ac);
-  }
-
-  if (p.glu) {
-    float o[16];
-#pragma unroll
-    for (int j = 0; j < 16; ++j) o[j] = v[2 * j] * act_eval(v[2 * j + 1], ac);
-    const int ncol = n_abs >> 1;
-    const int nout = p.N >> 1;
-    if (p.out_fp32) {
-      float* dst = reinterpret_cast<float*>(p.C) + c_off + ncol;
-#pragma unroll
-      for (int j = 0; j < 16; ++j)
-        if (ncol + j < nout) dst[j] = o[j];
-    } else {
-      __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.C) + c_off + ncol;
-      if (vec) {
-        uint4 w0 = make_uint4(pack_bf16x2(o[0], o[1]), pack_bf16x2(o[2], o[3]), pack_bf16x2(o[4], o[5]),
-                              pack_bf16x2(o[6], o[7]));
-        uint4 w1 = make_uint4(pack_bf16x2(o[8], o[9]), pack_bf16x2(o[10], o[11]), pack_bf16x2(o[12], o[13]),
-                              pack_bf16x2(o[14], o[15]));
-        reinterpret_cast<uint4*>(dst)[0] = w0;
-        reinterpret_cast<uint4*>(dst)[1] = w1;
-      } else {
-#pragma unroll
-        for (int j = 0; j < 16; ++j)
-          if (ncol + j < nout) dst[j] = __float2bfloat16(o[j]);
-      }
-    }
-    return;
-  }
-
-  if (p.row_gate) {
-    const float* rg = p.row_gate + g * p.ld_row + n_abs;
-#pragma unroll
-    for (int j = 0; j < 32; ++j)
-      if (full || n_abs + j < p.N) v[j] *= __ldg(rg + j);
-  }
-  if (p.residual) {
-    if (vec) {
-      const uint4* rs4 = reinterpret_cast<const uint4*>(p.residual + r_off + n_abs);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const uint4 w = __ldg(rs4 + j);
-        v[8 * j + 0] += bf16_lo(w.x), v[8 * j + 1] += bf16_hi(w.x);
-        v[8 * j + 2] += bf16_lo(w.y), v[8 * j + 3] += bf16_hi(w.y);
-        v[8 * j + 4] += bf16_lo(w.z), v[8 * j + 5] += bf16_hi(w.z);
-        v[8 * j + 6] += bf16_lo(w.w), v[8 * j + 7] += bf16_hi(w.w);
-      }
-    } else {
-      const __nv_bfloat16* rs = p.residual + r_off + n_abs;
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (n_abs + j < p.N) v[j] += __bfloat162float(rs[j]);
-    }
-  }
-  if (p.out_scale != 1.0f) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] *= p.out_scale;
-  }
-
-  if (p.out_fp32) {
-    float* dst = reinterpret_cast<float*>(p.C) + c_off + n_abs;
-    if (vec) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        reinterpret_cast<float4*>(dst)[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-    } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (n_abs + j < p.N) dst[j] = v[j];
-    }
-  } else {
-    __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.C) + c_off + n_abs;
-    if (vec) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        uint4 w = make_uint4(pack_bf16x2(v[8 * j], v[8 * j + 1]), pack_bf16x2(v[8 * j + 2], v[8 * j + 3]),
-                             pack_bf16x2(v[8 * j + 4], v[8 * j + 5]), pack_bf16x2(v[8 * j + 6], v[8 * j + 7]));
-        reinterpret_cast<uint4*>(dst)[j] = w;
-      }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (n_abs + j < p.N) dst[j] = __float2bfloat16(v[j]);
-    }
-  }
-}
-
-// ---- coalesced epilogue (bf16 output, no GLU, aligned full chunk) -------------------------------------------------
-// The epilogue hands every thread one accumulator ROW (32 consecutive columns = 64 bytes of bf16). Writing / reading
-// global memory in that shape makes each lane of a 16-byte access hit a different 128-byte line (32 L1 wavefronts per
-// instruction). The chunk is therefore transposed through a 2 KB per-warp shared-memory buffer so that a warp's
-// global access covers 8 rows x 64 contiguous bytes (8 wavefronts): 4 lanes per row, lane L -> row s*8 + L/4,
-// 16-byte piece L%4. The buffer is XOR-swizzled (piece ^ ((row >> 1) & 3)) so both access patterns are conflict-free.
-struct RowMap {          // global offsets (16-byte units) of the 4 rows this lane touches in the transposed pattern
-  uint32_t c16[4];
-  uint32_t r16[4];
-  uint32_t valid;        // bit s4 set = row s4 exists
-};
-
+// ---- epilogue staging buffer ------------------------------------------------------------------------------------------
+// The epilogue works on the wgmma accumulator fragments where they are: per n8 block a thread owns columns
+// (2 (lane % 4), + 1) of rows (lane / 4) and (lane / 4 + 8) of its warp's 16 rows. Global memory wants whole rows, so
+// the bf16 results (and, the other way, the residual) of 64 columns cross a 2 KB per-warp buffer: 16 rows x 8 pieces
+// of 16 bytes, XOR-swizzled so that the 4-byte fragment accesses and the 16-byte row accesses (8 lanes = one row's
+// 128 contiguous bytes) are both conflict-free.
 __device__ __forceinline__ uint32_t stage_addr(int row, int piece) {
-  return static_cast<uint32_t>(row * 64 + ((piece ^ ((row >> 1) & 3)) << 4));
+  return static_cast<uint32_t>(row * 128 + ((piece ^ (row & 7)) << 4));
 }
+constexpr uint32_t ROW_ABSENT = 0xFFFFFFFFu;  // row table entry of a row outside the problem
 
-__device__ __forceinline__ void epilogue_prefetch_staged(const IGemmParams& p, uint4 (&resv)[4], const RowMap& rm,
-                                                         int lane, int n_abs) {
-  if (p.residual) {
-    const uint4* base = reinterpret_cast<const uint4*>(p.residual + n_abs) + (lane & 3);
-#pragma unroll
-    for (int s4 = 0; s4 < 4; ++s4)
-      resv[s4] = ((rm.valid >> s4) & 1u) ? __ldg(base + rm.r16[s4]) : make_uint4(0u, 0u, 0u, 0u);
-  }
-}
-
-template <bool STATS>
-__device__ __forceinline__ void epilogue_chunk_staged(const IGemmParams& p, const ActCoef& ac, const uint32_t (&r)[32],
-                                                      const uint4 (&resv)[4], const float* bias_c, const RowMap& rm,
-                                                      uint8_t* stage, int lane, long long g, int n_abs, uint64_t (&st)[2]) {
-  float v[32];
-#pragma unroll
-  for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-  if (p.bias) {
-    const float4* b4 = reinterpret_cast<const float4*>(bias_c);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float4 a = b4[j];
-      v[4 * j + 0] += a.x, v[4 * j + 1] += a.y, v[4 * j + 2] += a.z, v[4 * j + 3] += a.w;
-    }
-  }
-  if (p.row_add) {
-    const float4* ra = reinterpret_cast<const float4*>(p.row_add + g * p.ld_row + n_abs);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float4 a = __ldg(ra + j);
-      v[4 * j + 0] += a.x, v[4 * j + 1] += a.y, v[4 * j + 2] += a.z, v[4 * j + 3] += a.w;
-    }
-  }
-  if (p.act != B200MIX_ACT_NONE) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = act_eval(v[j], ac);
-  }
-  if (p.row_gate) {
-    const float4* rg = reinterpret_cast<const float4*>(p.row_gate + g * p.ld_row + n_abs);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float4 a = __ldg(rg + j);
-      v[4 * j + 0] *= a.x, v[4 * j + 1] *= a.y, v[4 * j + 2] *= a.z, v[4 * j + 3] *= a.w;
-    }
-  }
-  const int piece = lane & 3;
-  if (p.residual) {
-    // transposed (coalesced) residual pieces -> smem -> this thread's own row
-#pragma unroll
-    for (int s4 = 0; s4 < 4; ++s4)
-      *reinterpret_cast<uint4*>(stage + stage_addr(s4 * 8 + (lane >> 2), piece)) = resv[s4];
-    __syncwarp();
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const uint4 w = *reinterpret_cast<const uint4*>(stage + stage_addr(lane, j));
-      v[8 * j + 0] += bf16_lo(w.x), v[8 * j + 1] += bf16_hi(w.x);
-      v[8 * j + 2] += bf16_lo(w.y), v[8 * j + 3] += bf16_hi(w.y);
-      v[8 * j + 4] += bf16_lo(w.z), v[8 * j + 5] += bf16_hi(w.z);
-      v[8 * j + 6] += bf16_lo(w.w), v[8 * j + 7] += bf16_hi(w.w);
-    }
-    __syncwarp();
-  }
-  if (p.out_scale != 1.0f) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] *= p.out_scale;
-  }
-  // own row -> smem -> transposed (coalesced) global stores
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const uint4 w = make_uint4(pack_bf16x2(v[8 * j], v[8 * j + 1]), pack_bf16x2(v[8 * j + 2], v[8 * j + 3]),
-                               pack_bf16x2(v[8 * j + 4], v[8 * j + 5]), pack_bf16x2(v[8 * j + 6], v[8 * j + 7]));
-    *reinterpret_cast<uint4*>(stage + stage_addr(lane, j)) = w;
-    if (STATS) {  // row statistics of the ROUNDED values (what the consumer of this tensor reads), packed fp32 pairs
-      const uint32_t ww[4] = {w.x, w.y, w.z, w.w};
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const uint64_t ab = pack_f32x2(bf16_lo(ww[u]), bf16_hi(ww[u]));
-        st[0] = fadd2(st[0], ab);
-        st[1] = ffma2(ab, ab, st[1]);
-      }
-    }
-  }
-  __syncwarp();
-  uint4* cbase = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.C) + n_abs) + piece;
-#pragma unroll
-  for (int s4 = 0; s4 < 4; ++s4) {
-    const uint4 w = *reinterpret_cast<const uint4*>(stage + stage_addr(s4 * 8 + (lane >> 2), piece));
-    if ((rm.valid >> s4) & 1u) cbase[rm.c16[s4]] = w;
-  }
-  __syncwarp();
+// two adjacent values of a per-group / per-row fp32 vector; the scalar form serves unaligned tables and the ragged
+// last columns (in0 / in1: the column exists)
+__device__ __forceinline__ float2 load_pair(const float* ptr, bool vec, bool in0, bool in1) {
+  if (vec) return in0 ? __ldg(reinterpret_cast<const float2*>(ptr)) : make_float2(0.0f, 0.0f);
+  return make_float2(in0 ? __ldg(ptr) : 0.0f, in1 ? __ldg(ptr + 1) : 0.0f);
 }
 
 // MCAST = the two CTAs of a cluster work on the same n-tile and each loads one half of the B tile with TMA multicast into
@@ -424,21 +206,22 @@ struct IGemmCfg {
   static constexpr int A_BYTES = 128 * 128;  // 128 rows x 64 bf16 (128 B per row, SW128)
   static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  // fp32 staging of 64 accumulator columns of one warpgroup's 64 rows; the row stride of 68 floats makes the row-wise
-  // float4 reads of the epilogue conflict-free
-  static constexpr int ACC_LD = 68;
-  static constexpr int ACC_BYTES = 2 * 64 * ACC_LD * 4;
-  // barriers | accumulator staging | 8 epilogue warps x 2 KB transpose buffers | 8 x 128 bias + 8 x 128 column sums
-  static constexpr int EXTRA_BYTES = 1024 + 256 + ACC_BYTES + 8 * 2048 + 2 * 8 * 512;
+  // alignment slack | barriers | 8 epilogue warps x 2 KB staging | per consumer warpgroup 256 bias + 256 column sums |
+  // 8 epilogue warps x 16-row offset tables
+  static constexpr int EXTRA_BYTES = 1024 + 256 + 8 * 2048 + 2 * 2 * 1024 + 8 * 128;
 };
 
-// Roles (288 threads): warps 0-7 = two consumer warpgroups, warp 8 = TMA producer (one elected lane). Consumer
-// warpgroup g multiplies rows [64 g, 64 g + 64) of the 128-row tile (wgmma m64 x BN x k16, accumulators in registers)
-// and then runs the epilogue of those rows: 64 accumulator columns at a time go through shared memory so that every
-// thread owns 32 consecutive columns of one row (warp w of the group: rows 32 (w & 1) + lane, chunk parity w >> 1).
-constexpr int IG_THREADS = 288;
-constexpr int IG_WARP_TMA = 8;
+// Roles (384 threads = three warpgroups): warpgroup 0 = producer (warp 0 issues the TMA loads from one elected lane,
+// warps 1-3 idle), warpgroups 1-2 = consumers. The producer warpgroup gives its registers back (setmaxnreg 40) and each
+// consumer warpgroup takes 232: 128 fp32 accumulators at BN = 256 plus the epilogue's operands fit without spilling.
+// Consumer warpgroup g multiplies rows [64 g, 64 g + 64) of the 128-row tile (wgmma m64 x BN x k16, accumulators in
+// registers) and then runs the epilogue of those rows on the fragments in place (see stage_addr).
+constexpr int IG_THREADS = 384;
+constexpr int IG_PRODUCER_REGS = 40, IG_CONSUMER_REGS = 232;
 
+// Epilogue families (see the dispatch in the kernel): bias / residual / statistics only, GLU, everything else on the
+// row-wise path, and the element-wise path (fp32 output, rows that are not whole 16-byte pieces).
+enum { EPI_PLAIN = 0, EPI_GLU = 1, EPI_GENERAL = 2, EPI_DIRECT = 3 };
 // LNM: the folded-LayerNorm epilogues are separate instantiations - the plain kernel carries none of their code.
 enum { LNM_NONE = 0, LNM_CONSUMER = 1, LNM_PRODUCER = 2 };
 template <int BN, int STAGES, bool MCAST, int LNM>
@@ -450,10 +233,10 @@ __global__ void __launch_bounds__(IG_THREADS, 1)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  float* acc_all = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES + 256);
-  uint8_t* stage_all = reinterpret_cast<uint8_t*>(acc_all) + Cfg::ACC_BYTES;
-  float* bias_all = reinterpret_cast<float*>(stage_all + 8 * 2048);  // 8 epilogue warps x 128 floats (their 4 chunks)
-  float* colsum_all = bias_all + 8 * 128;                            // same layout: folded-LayerNorm column sums
+  uint8_t* stage_all = smem + STAGES * Cfg::STAGE_BYTES + 256;
+  float* bias_all = reinterpret_cast<float*>(stage_all + 8 * 2048);  // per consumer warpgroup: the tile's BN bias values
+  float* colsum_all = bias_all + 2 * 256;                            // same layout: folded-LayerNorm column sums
+  uint2* rows_all = reinterpret_cast<uint2*>(colsum_all + 2 * 256);  // per epilogue warp: 16 x (C offset, residual offset)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -481,68 +264,75 @@ __global__ void __launch_bounds__(IG_THREADS, 1)
   const int total_super = tiles_m2 * p.tiles_n;
   const int kblocks = p.ntaps * p.kchunks;
 
-  if (warp == IG_WARP_TMA) {
-    // ===== TMA producer (whole warp runs the loop, one elected lane issues: see elect_one_sync) =====
-    int stage = 0;
-    uint32_t phase = 0;
-    for (SegIter seg(p.sk_tiles, total_super, kblocks, cluster_id, num_clusters); seg.next();) {
-      const int st = seg.st;
-      const int mp = st / p.tiles_n, nt = st - mp * p.tiles_n;
-      int mt = mp * 2 + (int)cta_rank;  // may be == tiles_m (phantom): its A box is out of bounds -> zeros
-      int tap_base = 0;
-      if (p.up) {  // phantom tiles of a parity (index >= tiles of the grid) get b0 >= Bn: zeros as well
-        const int par = mt / p.par_tiles;
-        mt -= par * p.par_tiles, tap_base = par * 4;
-      }
-      const int tx = mt % p.tiles_x;
-      const int ty = (mt / p.tiles_x) % p.tiles_y;
-      const int tb = mt / (p.tiles_x * p.tiles_y);
-      const int x0 = tx * p.TW, y0 = ty * p.TH, b0 = tb * p.TB, n0 = nt * BN;
-      int tap = seg.kb0 / p.kchunks, kc = seg.kb0 - tap * p.kchunks;
-      for (int kb = seg.kb0; kb < seg.kb1; ++kb) {
-        const int tg = tap_base + tap;
-        const int dc = p.tap_dc[tg], dx = p.tap_dx[tg], pp = p.tap_p[tg], dy = p.tap_dy[tg];
-        // MCAST: the peer CTA's consumers release this stage too (remote arrivals)
-        if (MCAST) mbar_wait_cluster(&empty_bar[stage], phase ^ 1);
-        else mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
-        uint8_t* sB = sA + Cfg::A_BYTES;
-        if (elect_one_sync()) {
-          mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-          tma_load_5d(sA, &tmA, &full_bar[stage], kc * 64 + dc, x0 + dx, pp, y0 + dy, b0);
-          if (MCAST) {
-            // my half of the weight tile, delivered to both CTAs of the cluster
-            tma_load_2d_mcast(sB + cta_rank * (Cfg::B_BYTES / 2), &tmB, &full_bar[stage], tg * p.Kc + kc * 64,
-                              n0 + (int)cta_rank * (BN / 2), (uint16_t)0x3);
-          } else {
-            tma_load_2d(sB, &tmB, &full_bar[stage], tg * p.Kc + kc * 64, n0);
-            tma_load_2d(sB + Cfg::B_BYTES / 2, &tmB, &full_bar[stage], tg * p.Kc + kc * 64, n0 + BN / 2);
-          }
+  if (warp < 4) {
+    setmaxnreg_dec<IG_PRODUCER_REGS>();
+    if (warp == 0) {
+      // ===== TMA producer (whole warp runs the loop, one elected lane issues: see elect_one_sync) =====
+      int stage = 0;
+      uint32_t phase = 0;
+      for (SegIter seg(p.sk_tiles, total_super, kblocks, cluster_id, num_clusters); seg.next();) {
+        const int st = seg.st;
+        const int mp = st / p.tiles_n, nt = st - mp * p.tiles_n;
+        int mt = mp * 2 + (int)cta_rank;  // may be == tiles_m (phantom): its A box is out of bounds -> zeros
+        int tap_base = 0;
+        if (p.up) {  // phantom tiles of a parity (index >= tiles of the grid) get b0 >= Bn: zeros as well
+          const int par = mt / p.par_tiles;
+          mt -= par * p.par_tiles, tap_base = par * 4;
         }
-        __syncwarp();
-        if (++stage == STAGES) stage = 0, phase ^= 1;
-        if (++kc == p.kchunks) kc = 0, ++tap;
+        const int tx = mt % p.tiles_x;
+        const int ty = (mt / p.tiles_x) % p.tiles_y;
+        const int tb = mt / (p.tiles_x * p.tiles_y);
+        const int x0 = tx * p.TW, y0 = ty * p.TH, b0 = tb * p.TB, n0 = nt * BN;
+        int tap = seg.kb0 / p.kchunks, kc = seg.kb0 - tap * p.kchunks;
+        for (int kb = seg.kb0; kb < seg.kb1; ++kb) {
+          const int tg = tap_base + tap;
+          const int dc = p.tap_dc[tg], dx = p.tap_dx[tg], pp = p.tap_p[tg], dy = p.tap_dy[tg];
+          // MCAST: the peer CTA's consumers release this stage too (remote arrivals)
+          if (MCAST) mbar_wait_cluster(&empty_bar[stage], phase ^ 1);
+          else mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
+          uint8_t* sB = sA + Cfg::A_BYTES;
+          if (elect_one_sync()) {
+            mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+            tma_load_5d(sA, &tmA, &full_bar[stage], kc * 64 + dc, x0 + dx, pp, y0 + dy, b0);
+            if (MCAST) {
+              // my half of the weight tile, delivered to both CTAs of the cluster
+              tma_load_2d_mcast(sB + cta_rank * (Cfg::B_BYTES / 2), &tmB, &full_bar[stage], tg * p.Kc + kc * 64,
+                                n0 + (int)cta_rank * (BN / 2), (uint16_t)0x3);
+            } else {
+              tma_load_2d(sB, &tmB, &full_bar[stage], tg * p.Kc + kc * 64, n0);
+              tma_load_2d(sB + Cfg::B_BYTES / 2, &tmB, &full_bar[stage], tg * p.Kc + kc * 64, n0 + BN / 2);
+            }
+          }
+          __syncwarp();
+          if (++stage == STAGES) stage = 0, phase ^= 1;
+          if (++kc == p.kchunks) kc = 0, ++tap;
+        }
       }
     }
   } else {
+    setmaxnreg_inc<IG_CONSUMER_REGS>();
     // ===== consumers: MMA of 64 rows, then their epilogue =====
-    const int grp = warp >> 2, w = warp & 3;
-    const int q = 2 * grp + (w & 1);  // 32-row quarter of the tile this warp's epilogue owns
-    const int wg = w >> 1;            // its 32-column chunks are c == wg (mod 2)
-    uint8_t* stage = stage_all + warp * 2048;
-    float* bias_s = bias_all + warp * 128;
-    float* colsum_s = colsum_all + warp * 128;
-    float* sacc = acc_all + grp * 64 * Cfg::ACC_LD;
+    const int cwarp = warp - 4;             // consumer warp 0-7
+    const int grp = cwarp >> 2, w = cwarp & 3;
+    const int l4 = lane >> 2, lm = lane & 3;
+    const int ctid = threadIdx.x - 128;     // consumer thread 0-255
+    uint8_t* stage = stage_all + cwarp * 2048;
+    float* bias_s = bias_all + grp * 256;
+    float* colsum_s = colsum_all + grp * 256;
+    uint2* rows_s = rows_all + cwarp * 16;
     const ActCoef ac = act_coef(p.act, p.glu);
-    const bool staged_ok = p.vec_ok && !p.glu && !p.out_fp32 && ((p.c_bstride | p.r_bstride) & 7) == 0;
-    const int row = q * 32 + lane;
-    const int tw = row % p.TW;
-    const int th = (row / p.TW) % p.TH;
-    const int tbb = row / (p.TW * p.TH);
+    const bool staged_ok = p.vec_ok && !p.out_fp32 && ((p.c_bstride | p.r_bstride) & 7) == 0;
+    // this thread's two rows of the tile: position inside the tile box
+    int tw[2], th[2], tbb[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = grp * 64 + w * 16 + l4 + 8 * h;
+      tw[h] = row % p.TW, th[h] = (row / p.TW) % p.TH, tbb[h] = row / (p.TW * p.TH);
+    }
     const uint32_t peer_empty = MCAST ? mapa_smem(&empty_bar[0], cta_rank ^ 1u) : 0u;
     int kstage = 0;
     uint32_t kphase = 0;
-    const int epi_tid = warp * 32 + lane;
     auto release = [&](int s) {  // this warp's wgmma reads of stage s are complete
       if (lane == 0) {
         mbar_arrive(&empty_bar[s]);
@@ -577,88 +367,20 @@ __global__ void __launch_bounds__(IG_THREADS, 1)
       const int st = seg.st;
       const int seg_mode = seg.mode();
       // stream-K pieces: the tail piece (my first) goes to MY workspace slot; the head piece (my last) is completed with
-      // the tail piece of the same tile, which the NEXT cluster produced at its very start
+      // the tail piece of the same tile, which the NEXT cluster produced at its very start. A partial travels in the
+      // fragment layout (n8 block j of consumer thread t at [j][t]: 512 contiguous bytes per warp and access).
       const int sk_slot = (seg_mode == SEG_TAIL ? cluster_id : cluster_id + 1) * 2 + (int)cta_rank;
-      float4* sk_ws = p.sk_ws + static_cast<size_t>(sk_slot) * SK_WS_FLOAT4_PER_CTA + (q * 32 + lane);
-      const int mp = st / p.tiles_n, nt = st - mp * p.tiles_n;
-      int mt = mp * 2 + (int)cta_rank;
-      const bool in_range = mt < tiles_m;
-      int par = 0;
-      if (p.up) par = mt / p.par_tiles, mt -= par * p.par_tiles;
-      const int tx = mt % p.tiles_x;
-      const int ty = (mt / p.tiles_x) % p.tiles_y;
-      const int tb = mt / (p.tiles_x * p.tiles_y);
-      const int x = tx * p.TW + tw, y = ty * p.TH + th, b = tb * p.TB + tbb;
-      const bool valid = in_range && (x < p.Wo) && (y < p.Ho) && (b < p.Bn);
-      const long long gm = p.up ? (static_cast<long long>(b) * (2 * p.Ho) + (2 * y + (par >> 1))) * (2 * p.Wo) + (2 * x + (par & 1))
-                                : (static_cast<long long>(b) * p.Ho + y) * p.Wo + x;
-      long long g, c_off, r_off;
-      if (p.c_bstride) {  // batched-strided: group == batch
-        g = b;
-        c_off = static_cast<long long>(b) * p.c_bstride + static_cast<long long>(x) * p.ldc;
-        r_off = static_cast<long long>(b) * p.r_bstride + static_cast<long long>(x) * p.ldr;
-      } else {
-        g = gm / p.rows_per_group;
-        c_off = gm * p.ldc;
-        r_off = (p.res_row_mod > 0 ? gm % p.res_row_mod : gm) * p.ldr;
-      }
-      // rows outside the problem (phantom m-tile of an odd pair, rows past M) still run the warp-collective epilogue:
-      // give them group 0 so their row_add / row_gate reads stay inside the [groups, N] tables (nothing is stored)
-      if (!valid) g = 0;
-      const int n0 = nt * BN;
-      RowMap rm;  // offsets are multiples of 8 elements whenever staged_ok (vec_ok: 16-byte aligned rows)
-      rm.valid = 0;
+      float4* sk_ws = p.sk_ws + static_cast<size_t>(sk_slot) * SK_WS_FLOAT4_PER_CTA + ctid;
+      if (seg_mode == SEG_TAIL) {
 #pragma unroll
-      for (int s4 = 0; s4 < 4; ++s4) {
-        const int src = s4 * 8 + (lane >> 2);
-        rm.c16[s4] = __shfl_sync(0xffffffffu, static_cast<uint32_t>(c_off >> 3), src);
-        rm.r16[s4] = __shfl_sync(0xffffffffu, static_cast<uint32_t>(r_off >> 3), src);
-        rm.valid |= (__shfl_sync(0xffffffffu, valid ? 1u : 0u, src) & 1u) << s4;
+        for (int j = 0; j < BN / 8; ++j)
+          __stcg(sk_ws + j * 256, make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]));
+        // all 256 consumer threads' partials are visible device-wide before the flag goes up
+        __threadfence();
+        named_bar_sync(1, 256);
+        if (ctid == 0) st_release_gpu(p.sk_flags + sk_slot, 1u);
+        continue;
       }
-      // this warp's bias values (its <= 4 chunks of the tile) go to shared memory, read back as broadcast float4s.
-      // Folded LayerNorm (consumer side): y = rstd * (acc - mean * colsum[n]) + bias'[n] needs the column sums the same
-      // way plus this row's fixed-point totals. ALL of these loads are issued before any of them is consumed, so a tile's
-      // preparation costs one L2 round trip, not three.
-      constexpr int NI = (BN / 32 + 1) / 2;
-      float bias_r[NI], cs_r[NI];
-      longlong2 t_stats = make_longlong2(0ll, 0ll);
-      if (p.bias) {
-#pragma unroll
-        for (int i = 0; i < NI; ++i) {
-          const int col = n0 + (wg + 2 * i) * 32 + lane;
-          bias_r[i] = (wg + 2 * i < BN / 32 && col < p.N) ? __ldg(p.bias + col) : 0.0f;
-        }
-      }
-      if (LNM == LNM_CONSUMER) {
-#pragma unroll
-        for (int i = 0; i < NI; ++i) {
-          const int col = n0 + (wg + 2 * i) * 32 + lane;
-          cs_r[i] = (wg + 2 * i < BN / 32 && col < p.N) ? __ldg(p.ln_colsum + col) : 0.0f;
-        }
-        t_stats = __ldg(reinterpret_cast<const longlong2*>(p.ln_stats) + (valid ? gm : 0ll));
-      }
-      if (p.bias) {
-#pragma unroll
-        for (int i = 0; i < NI; ++i) bias_s[i * 32 + lane] = bias_r[i];
-      }
-      if (LNM == LNM_CONSUMER) {
-#pragma unroll
-        for (int i = 0; i < NI; ++i) colsum_s[i * 32 + lane] = cs_r[i];
-      }
-      __syncwarp();
-      float ln_rstd = 1.0f, ln_shift = 0.0f;
-      if (LNM == LNM_CONSUMER) {  // mean / rstd of my row from the totals the producing GEMM's epilogues accumulated
-        // fp32 on purpose (FP64 is slow on the epilogue's critical path). E[x^2] - mean^2 in fp32 is good to
-        // ~1e-7 * mean^2 / var relative: below the bf16 resolution of the inputs themselves for any row bf16 can
-        // represent (|mean| / std < 2^8).
-        const float mean = p.ln_rms ? 0.0f : __ll2float_rn(t_stats.x) * p.ln_inv_k;
-        const float var = fmaxf(fmaf(-mean, mean, __ll2float_rn(t_stats.y) * p.ln_inv_k), 0.0f);
-        ln_rstd = rsqrtf(var + p.ln_eps);
-        ln_shift = -ln_rstd * mean;
-      }
-      uint64_t st_acc[2] = {0ull, 0ull};  // producer side: packed (even, odd column) sum / sum of squares of my row over my chunks
-      uint4 res_cur[4];
-      bool st_cur = staged_ok && n0 + wg * 32 + 32 <= p.N;
       if (seg_mode == SEG_HEAD) {
         // the partner's partial was published ~a tile ago; a bounded spin (2^35 cycles, ~18 s: far beyond any time slice
         // the context can lose) turns a scheduling accident (the partner cluster never resident) into an error instead
@@ -668,95 +390,245 @@ __global__ void __launch_bounds__(IG_THREADS, 1)
         while (ld_acquire_gpu(flag) == 0u) {
           if (clock64() - t_start > (1ll << 35)) __trap();
         }
-      }
-      const int l4 = lane >> 2, lm = lane & 3;
 #pragma unroll
-      for (int i = 0; i < (BN + 63) / 64; ++i) {
-        // columns [64 i, 64 i + 64) of the warpgroup's 64 rows: fragments -> shared memory -> one row per thread
-        named_bar_sync(2 + grp, 128);  // the previous pair of chunks has been read
-#pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
-          const int j = 8 * i + jj;  // n8 block of the accumulator fragment
-          if (j < BN / 8) {
-            float* d0 = sacc + (w * 16 + l4) * Cfg::ACC_LD + jj * 8 + 2 * lm;
-            *reinterpret_cast<float2*>(d0) = make_float2(acc[4 * j], acc[4 * j + 1]);
-            *reinterpret_cast<float2*>(d0 + 8 * Cfg::ACC_LD) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-          }
+        for (int j = 0; j < BN / 8; ++j) {
+          const float4 part = __ldcg(sk_ws + j * 256);
+          acc[4 * j] += part.x, acc[4 * j + 1] += part.y, acc[4 * j + 2] += part.z, acc[4 * j + 3] += part.w;
         }
-        named_bar_sync(2 + grp, 128);
-        const int c = 2 * i + wg;
-        if (c >= BN / 32) continue;
-        uint32_t r[32];
-        {
-          const float4* src = reinterpret_cast<const float4*>(sacc + (32 * (w & 1) + lane) * Cfg::ACC_LD + wg * 32);
-#pragma unroll
-          for (int t = 0; t < 8; ++t) {
-            const float4 v4 = src[t];
-            r[4 * t] = __float_as_uint(v4.x), r[4 * t + 1] = __float_as_uint(v4.y);
-            r[4 * t + 2] = __float_as_uint(v4.z), r[4 * t + 3] = __float_as_uint(v4.w);
-          }
-        }
-        const int n_abs = n0 + c * 32;
-        if (seg_mode == SEG_TAIL) {  // partial accumulators -> workspace (512 contiguous bytes per warp and store)
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            __stcg(sk_ws + (c * 8 + j) * 128, make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]),
-                                                          __uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3])));
-          continue;
-        }
-        if (seg_mode == SEG_HEAD) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 part = __ldcg(sk_ws + (c * 8 + j) * 128);
-            r[4 * j + 0] = __float_as_uint(__uint_as_float(r[4 * j + 0]) + part.x);
-            r[4 * j + 1] = __float_as_uint(__uint_as_float(r[4 * j + 1]) + part.y);
-            r[4 * j + 2] = __float_as_uint(__uint_as_float(r[4 * j + 2]) + part.z);
-            r[4 * j + 3] = __float_as_uint(__uint_as_float(r[4 * j + 3]) + part.w);
-          }
-        }
-        if (LNM == LNM_CONSUMER) {
-          const float4* c4 = reinterpret_cast<const float4*>(colsum_s + (c >> 1) * 32);
-          const uint64_t rstd2 = pack_f32x2(ln_rstd, ln_rstd), shift2 = pack_f32x2(ln_shift, ln_shift);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 cs = c4[j];
-            float a, bb;
-            unpack_f32x2(ffma2(pack_f32x2(__uint_as_float(r[4 * j + 0]), __uint_as_float(r[4 * j + 1])), rstd2,
-                               fmul2(shift2, pack_f32x2(cs.x, cs.y))), a, bb);
-            r[4 * j + 0] = __float_as_uint(a), r[4 * j + 1] = __float_as_uint(bb);
-            unpack_f32x2(ffma2(pack_f32x2(__uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3])), rstd2,
-                               fmul2(shift2, pack_f32x2(cs.z, cs.w))), a, bb);
-            r[4 * j + 2] = __float_as_uint(a), r[4 * j + 3] = __float_as_uint(bb);
-          }
-        }
-        if (st_cur) {  // warp-uniform: coalesced path through the transpose buffer
-          epilogue_prefetch_staged(p, res_cur, rm, lane, n_abs);
-          epilogue_chunk_staged<LNM == LNM_PRODUCER>(p, ac, r, res_cur, bias_s + (c >> 1) * 32, rm, stage, lane, g, n_abs, st_acc);
-          st_cur = (c + 2 < BN / 32) && (n_abs + 96 <= p.N);
-        } else {
-          const bool active = valid && n_abs < p.N;
-          EpiOperands eo;
-          if (active) epilogue_prefetch(p, eo, bias_s + (c >> 1) * 32, n_abs);
-          if (active) epilogue_chunk(p, ac, r, eo, c_off, r_off, g, n_abs);
-        }
-      }
-      if (LNM == LNM_PRODUCER && seg_mode != SEG_TAIL && valid) {
-        // 2^24 fixed point: integer adds commute, so the row totals are the same bits whatever order the tiles finish in
-        float s0, s1, q0, q1;
-        unpack_f32x2(st_acc[0], s0, s1);
-        unpack_f32x2(st_acc[1], q0, q1);
-        unsigned long long* dst = reinterpret_cast<unsigned long long*>(p.stats_out + 2 * gm);
-        atomicAdd(dst, static_cast<unsigned long long>(__float2ll_rn((s0 + s1) * 16777216.0f)));
-        atomicAdd(dst + 1, static_cast<unsigned long long>(__float2ll_rn((q0 + q1) * 16777216.0f)));
-      }
-      if (seg_mode != SEG_FULL) {
-        // tail: all 256 consumer threads' partials are visible device-wide before the flag goes up;
-        // head: everybody has read the partial before the flag is lowered for the next launch
-        if (seg_mode == SEG_TAIL) __threadfence();
+        // everybody has read the partial before the flag is lowered for the next launch
         named_bar_sync(1, 256);
-        if (epi_tid == 0) {
-          if (seg_mode == SEG_TAIL) st_release_gpu(p.sk_flags + sk_slot, 1u);
-          else p.sk_flags[sk_slot] = 0u;
+        if (ctid == 0) p.sk_flags[sk_slot] = 0u;
+      }
+
+      const int mp = st / p.tiles_n, nt = st - mp * p.tiles_n;
+      int mt = mp * 2 + (int)cta_rank;
+      const bool in_range = mt < tiles_m;
+      int par = 0;
+      if (p.up) par = mt / p.par_tiles, mt -= par * p.par_tiles;
+      const int tx = mt % p.tiles_x;
+      const int ty = (mt / p.tiles_x) % p.tiles_y;
+      const int tb = mt / (p.tiles_x * p.tiles_y);
+      const int n0 = nt * BN;
+      // my two rows: rows outside the problem (phantom m-tile of an odd pair, rows past M) still run the warp-collective
+      // epilogue; they get group 0 so their row_add / row_gate reads stay inside the [groups, N] tables (nothing is stored)
+      bool valid[2];
+      long long gm[2], g[2], c_off[2], r_off[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int x = tx * p.TW + tw[h], y = ty * p.TH + th[h], b = tb * p.TB + tbb[h];
+        valid[h] = in_range && (x < p.Wo) && (y < p.Ho) && (b < p.Bn);
+        gm[h] = p.up ? (static_cast<long long>(b) * (2 * p.Ho) + (2 * y + (par >> 1))) * (2 * p.Wo) + (2 * x + (par & 1))
+                     : (static_cast<long long>(b) * p.Ho + y) * p.Wo + x;
+        if (p.c_bstride) {  // batched-strided: group == batch
+          g[h] = b;
+          c_off[h] = static_cast<long long>(b) * p.c_bstride + static_cast<long long>(x) * p.ldc;
+          r_off[h] = static_cast<long long>(b) * p.r_bstride + static_cast<long long>(x) * p.ldr;
+        } else {
+          g[h] = gm[h] / p.rows_per_group;
+          c_off[h] = gm[h] * p.ldc;
+          r_off[h] = (p.res_row_mod > 0 ? gm[h] % p.res_row_mod : gm[h]) * p.ldr;
+        }
+        if (!valid[h]) g[h] = 0, gm[h] = 0;
+        // offsets in 16-byte units for the row-wise accesses (multiples of 8 elements whenever staged_ok)
+        if (lm == 0)
+          rows_s[l4 + 8 * h] = make_uint2(valid[h] ? static_cast<uint32_t>(c_off[h] >> 3) : ROW_ABSENT,
+                                          static_cast<uint32_t>(r_off[h] >> 3));
+      }
+      // The tile's bias values go to shared memory once per warpgroup. Folded LayerNorm (consumer side):
+      // y = rstd * (acc - mean * colsum[n]) + bias'[n] needs the column sums the same way plus my rows' fixed-point
+      // totals. ALL of these loads are issued before any of them is consumed: one L2 round trip per tile, not three.
+      constexpr int NI = (BN + 127) / 128;
+      const int gt = ctid & 127;
+      float bias_r[NI], cs_r[NI];
+      longlong2 t_stats[2] = {make_longlong2(0ll, 0ll), make_longlong2(0ll, 0ll)};
+#pragma unroll
+      for (int i = 0; i < NI; ++i) {
+        const int col = n0 + i * 128 + gt;
+        bias_r[i] = (p.bias && col < p.N) ? __ldg(p.bias + col) : 0.0f;
+        if (LNM == LNM_CONSUMER) cs_r[i] = col < p.N ? __ldg(p.ln_colsum + col) : 0.0f;
+      }
+      if (LNM == LNM_CONSUMER) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) t_stats[h] = __ldg(reinterpret_cast<const longlong2*>(p.ln_stats) + gm[h]);
+      }
+      named_bar_sync(2 + grp, 128);  // every warp of the group has finished reading the previous tile's values
+#pragma unroll
+      for (int i = 0; i < NI; ++i) {
+        if (i * 128 + gt < BN) {
+          bias_s[i * 128 + gt] = bias_r[i];
+          if (LNM == LNM_CONSUMER) colsum_s[i * 128 + gt] = cs_r[i];
+        }
+      }
+      named_bar_sync(2 + grp, 128);
+      float ln_rstd[2] = {1.0f, 1.0f}, ln_shift[2] = {0.0f, 0.0f};
+      if (LNM == LNM_CONSUMER) {  // mean / rstd of my rows from the totals the producing GEMM's epilogues accumulated
+        // fp32 on purpose (FP64 is slow on the epilogue's critical path). E[x^2] - mean^2 in fp32 is good to
+        // ~1e-7 * mean^2 / var relative: below the bf16 resolution of the inputs themselves for any row bf16 can
+        // represent (|mean| / std < 2^8).
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float mean = p.ln_rms ? 0.0f : __ll2float_rn(t_stats[h].x) * p.ln_inv_k;
+          const float var = fmaxf(fmaf(-mean, mean, __ll2float_rn(t_stats[h].y) * p.ln_inv_k), 0.0f);
+          ln_rstd[h] = rsqrtf(var + p.ln_eps);
+          ln_shift[h] = -ln_rstd[h] * mean;
+        }
+      }
+      float st_sum[2] = {0.0f, 0.0f}, st_sq[2] = {0.0f, 0.0f};  // producer side: my rows' sum / sum of squares over my columns
+      const int n_end = p.glu ? p.N >> 1 : p.N;  // output columns
+      const int srow = lane >> 3, spiece = lane & 7;  // row-wise pattern: row 4 s + srow, 16-byte piece spiece
+      // residual pieces of one 64-column group, row-wise (coalesced); fetched one group ahead of their use
+      uint4 resv[4];
+      auto residual_fetch = [&](int n_abs, int nb) {
+#pragma unroll
+        for (int s = 0; s < 4; ++s) {
+          const uint2 ro = rows_s[4 * s + srow];
+          const bool ok = ro.x != ROW_ABSENT && spiece < nb && n_abs + 8 * spiece < p.N;
+          resv[s] = ok ? __ldg(reinterpret_cast<const uint4*>(p.residual + n_abs) + ro.y + spiece) : make_uint4(0u, 0u, 0u, 0u);
+        }
+      };
+      __syncwarp();  // rows_s
+      constexpr int NG = (BN + 63) / 64;
+      // The tile takes the row-wise path when every output row splits into whole 16-byte pieces. The loop over the
+      // fragment is fully unrolled, so it is instantiated per epilogue family with the other families' code left out:
+      // what a tile executes stays a few thousand instructions, inside the instruction cache.
+      const bool tile_staged = staged_ok && p.N % (p.glu ? 16 : 8) == 0;
+      auto epilogue = [&](auto mode_c) {
+        constexpr int MODE = decltype(mode_c)::value;
+        constexpr bool staged = MODE != EPI_DIRECT;
+        constexpr bool general = MODE == EPI_GENERAL || MODE == EPI_DIRECT;
+        const bool glu_on = MODE == EPI_GLU || (MODE == EPI_DIRECT && p.glu);
+        const bool radd_on = MODE != EPI_PLAIN && p.row_add;
+        const bool act_on = general && p.act != B200MIX_ACT_NONE;
+        const bool gate_on = general && p.row_gate;
+        const bool scale_on = general && p.out_scale != 1.0f;
+        const bool res_on = MODE != EPI_GLU && p.residual;
+        const bool fp32_on = MODE == EPI_DIRECT && p.out_fp32;
+        if (staged && res_on) residual_fetch(n0, BN / 8 < 8 ? BN / 8 : 8);
+  #pragma unroll
+        for (int i = 0; i < NG; ++i) {
+          // columns [64 i, 64 i + 64) of the tile: nb n8 blocks of the fragment
+          const int nb = BN / 8 - 8 * i < 8 ? BN / 8 - 8 * i : 8;
+          const int n_abs = n0 + 64 * i;
+          if (n_abs >= p.N) break;
+          if (staged && res_on) {
+  #pragma unroll
+            for (int s = 0; s < 4; ++s) *reinterpret_cast<uint4*>(stage + stage_addr(4 * s + srow, spiece)) = resv[s];
+            __syncwarp();
+            if (i + 1 < NG) {
+              const int nb1 = BN / 8 - 8 * (i + 1) < 8 ? BN / 8 - 8 * (i + 1) : 8;
+              if (n_abs + 64 < p.N) residual_fetch(n_abs + 64, nb1);
+            }
+          }
+  #pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            if (jj >= nb) continue;
+            const int j = 8 * i + jj;              // n8 block of the accumulator fragment
+            const int cl = 64 * i + 8 * jj + 2 * lm;  // my column pair inside the tile
+            const int col = n0 + cl;
+            const bool in0 = col < p.N, in1 = col + 1 < p.N;
+            const float2 bias2 = *reinterpret_cast<const float2*>(bias_s + cl);
+            float2 cs2 = make_float2(0.0f, 0.0f);
+            if (LNM == LNM_CONSUMER) cs2 = *reinterpret_cast<const float2*>(colsum_s + cl);
+            float glu_out[2];
+  #pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float x = acc[4 * j + 2 * h], y = acc[4 * j + 2 * h + 1];
+              if (LNM == LNM_CONSUMER) {
+                x = __fmaf_rn(x, ln_rstd[h], __fmul_rn(ln_shift[h], cs2.x));
+                y = __fmaf_rn(y, ln_rstd[h], __fmul_rn(ln_shift[h], cs2.y));
+              }
+              if (p.bias) x += bias2.x, y += bias2.y;
+              if (radd_on) {
+                const float2 a = load_pair(p.row_add + g[h] * p.ld_row + col, staged, in0, in1);
+                x += a.x, y += a.y;
+              }
+              if (glu_on) {  // value / gate are adjacent columns
+                glu_out[h] = x * act_eval(y, ac);
+                if (!staged && valid[h] && in1) {
+                  if (fp32_on) reinterpret_cast<float*>(p.C)[c_off[h] + (col >> 1)] = glu_out[h];
+                  else reinterpret_cast<__nv_bfloat16*>(p.C)[c_off[h] + (col >> 1)] = __float2bfloat16(glu_out[h]);
+                }
+                continue;
+              }
+              if (act_on) x = act_eval(x, ac), y = act_eval(y, ac);
+              if (gate_on) {
+                const float2 a = load_pair(p.row_gate + g[h] * p.ld_row + col, staged, in0, in1);
+                x *= a.x, y *= a.y;
+              }
+              uint32_t* word = reinterpret_cast<uint32_t*>(stage + stage_addr(l4 + 8 * h, jj) + 4 * lm);
+              if (res_on) {
+                if (staged) {
+                  const uint32_t r2 = *word;
+                  x += bf16_lo(r2), y += bf16_hi(r2);
+                } else if (valid[h]) {
+                  const __nv_bfloat16* rs = p.residual + r_off[h] + col;
+                  if (in0) x += __bfloat162float(rs[0]);
+                  if (in1) y += __bfloat162float(rs[1]);
+                }
+              }
+              if (scale_on) x *= p.out_scale, y *= p.out_scale;
+              if (staged) {
+                const uint32_t o2 = pack_bf16x2(x, y);
+                *word = o2;  // the word this thread read its residual from
+                if (LNM == LNM_PRODUCER && in0) {  // row statistics of the ROUNDED values (what the consumer of this tensor reads)
+                  const float rx = bf16_lo(o2), ry = bf16_hi(o2);
+                  st_sum[h] += rx + ry;
+                  st_sq[h] = fmaf(ry, ry, fmaf(rx, rx, st_sq[h]));
+                }
+              } else if (valid[h]) {
+                if (fp32_on) {
+                  float* dst = reinterpret_cast<float*>(p.C) + c_off[h] + col;
+                  if (in0) dst[0] = x;
+                  if (in1) dst[1] = y;
+                } else {
+                  __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.C) + c_off[h] + col;
+                  if (in0) dst[0] = __float2bfloat16(x);
+                  if (in1) dst[1] = __float2bfloat16(y);
+                }
+              }
+            }
+            if (glu_on && staged) {
+              // the output column of this pair is cl / 2: lanes lm and lm ^ 1 hold adjacent output columns of both rows.
+              // Even lanes collect row l4, odd lanes row l4 + 8, so every lane stores one bf16 pair.
+              const float got = __shfl_xor_sync(0xffffffffu, (lm & 1) ? glu_out[0] : glu_out[1], 1);
+              const uint32_t o2 = (lm & 1) ? pack_bf16x2(got, glu_out[1]) : pack_bf16x2(glu_out[0], got);
+              *reinterpret_cast<uint32_t*>(stage + stage_addr(l4 + 8 * (lm & 1), jj >> 1) + (jj & 1) * 8 + (lm >> 1) * 4) = o2;
+            }
+          }
+          if (staged) {
+            // staging buffer -> global memory, a row's contiguous bytes by adjacent lanes
+            __syncwarp();
+            const int npieces = glu_on ? nb >> 1 : nb;
+            const int col_out = glu_on ? n_abs >> 1 : n_abs;
+            uint4* cbase = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.C) + col_out) + spiece;
+  #pragma unroll
+            for (int s = 0; s < 4; ++s) {
+              const uint32_t c16 = rows_s[4 * s + srow].x;
+              const uint4 o4 = *reinterpret_cast<const uint4*>(stage + stage_addr(4 * s + srow, spiece));
+              if (c16 != ROW_ABSENT && spiece < npieces && col_out + 8 * spiece < n_end) cbase[c16] = o4;
+            }
+            __syncwarp();
+          }
+        }
+      };
+      if (!tile_staged) epilogue(std::integral_constant<int, EPI_DIRECT>{});
+      else if (p.glu) epilogue(std::integral_constant<int, EPI_GLU>{});
+      else if (p.act != B200MIX_ACT_NONE || p.row_add || p.row_gate || p.out_scale != 1.0f)
+        epilogue(std::integral_constant<int, EPI_GENERAL>{});
+      else epilogue(std::integral_constant<int, EPI_PLAIN>{});
+      if (LNM == LNM_PRODUCER) {
+        // quad reduction in a fixed order, then 2^24 fixed point: integer adds commute, so the row totals are the same
+        // bits whatever order the tiles finish in
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float s = st_sum[h], q = st_sq[h];
+          s += __shfl_xor_sync(0xffffffffu, s, 1), q += __shfl_xor_sync(0xffffffffu, q, 1);
+          s += __shfl_xor_sync(0xffffffffu, s, 2), q += __shfl_xor_sync(0xffffffffu, q, 2);
+          if (lm == 0 && valid[h]) {
+            unsigned long long* dst = reinterpret_cast<unsigned long long*>(p.stats_out + 2 * gm[h]);
+            atomicAdd(dst, static_cast<unsigned long long>(__float2ll_rn(s * 16777216.0f)));
+            atomicAdd(dst + 1, static_cast<unsigned long long>(__float2ll_rn(q * 16777216.0f)));
+          }
         }
       }
     }
@@ -994,10 +866,10 @@ static int g_streamk = [] {
 // A split tile sends its 256 KB of fp32 partials through L2 twice; a tile's own operand traffic is 32 KB per k-block, so
 // only deep reductions (>= 64 k-blocks: the 3x3 convs and FF2 of the SDXL step) are split.
 constexpr int SK_MIN_KBLOCKS = 64;
-constexpr int SK_MAX_CLUSTERS = 74;
+constexpr int SK_MAX_CLUSTERS = 66;  // 132 SMs
 static int sk_min_kblocks() { return g_streamk >= 2 ? 8 : SK_MIN_KBLOCKS; }  // 2 = tests: split shallow reductions too
 
-// Stream-K workspaces: SK_POOL slots per device (19 MB of partial accumulators + 148 flags each, sized for up to 74 clusters of 2 CTAs), allocated together on
+// Stream-K workspaces: SK_POOL slots per device (17 MB of partial accumulators + 132 flags each: 66 clusters of 2 CTAs), allocated together on
 // the first eager GEMM call (never inside a stream capture). A slot belongs to ONE stream: launches on a stream are
 // ordered (a kernel's first global access follows griddepcontrol.wait = completion of its predecessor), so they can
 // share it; kernels captured into a CUDA graph keep the slot of their capture stream. Streams beyond the pool, and
@@ -1144,26 +1016,26 @@ static int dispatch_igemm(const CUtensorMap& tmA, const void* W, long long ldw, 
     int rc = encode_tmap_bf16_sw128(&tmB, W, 2, dims, strides, box);
     if (rc) return rc;
   }
-  // stage counts: as many as fit next to the epilogue buffers (IGemmCfg::EXTRA_BYTES) in 227 KB
+  // stage counts: as many (up to 8) as fit next to the epilogue buffers (IGemmCfg::EXTRA_BYTES) in 227 KB
   if (g_gemm_pair) {
     switch (bn) {
-      case 256: return launch_igemm<256, 3, true>(tmA, tmB, p, stream);
-      case 224: return launch_igemm<224, 3, true>(tmA, tmB, p, stream);
-      case 192: return launch_igemm<192, 4, true>(tmA, tmB, p, stream);
-      case 160: return launch_igemm<160, 4, true>(tmA, tmB, p, stream);
-      case 128: return launch_igemm<128, 5, true>(tmA, tmB, p, stream);
-      case 64: return launch_igemm<64, 6, true>(tmA, tmB, p, stream);
+      case 256: return launch_igemm<256, 4, true>(tmA, tmB, p, stream);
+      case 224: return launch_igemm<224, 4, true>(tmA, tmB, p, stream);
+      case 192: return launch_igemm<192, 5, true>(tmA, tmB, p, stream);
+      case 160: return launch_igemm<160, 5, true>(tmA, tmB, p, stream);
+      case 128: return launch_igemm<128, 6, true>(tmA, tmB, p, stream);
+      case 64: return launch_igemm<64, 8, true>(tmA, tmB, p, stream);
       case 32: return launch_igemm<32, 8, true>(tmA, tmB, p, stream);
       default: set_error("unsupported BN %d", bn); return B200MIX_ERR_INVALID;
     }
   }
   switch (bn) {
-    case 256: return launch_igemm<256, 3, false>(tmA, tmB, p, stream);
-    case 224: return launch_igemm<224, 3, false>(tmA, tmB, p, stream);
-    case 192: return launch_igemm<192, 4, false>(tmA, tmB, p, stream);
-    case 160: return launch_igemm<160, 4, false>(tmA, tmB, p, stream);
-    case 128: return launch_igemm<128, 5, false>(tmA, tmB, p, stream);
-    case 64: return launch_igemm<64, 6, false>(tmA, tmB, p, stream);
+    case 256: return launch_igemm<256, 4, false>(tmA, tmB, p, stream);
+    case 224: return launch_igemm<224, 4, false>(tmA, tmB, p, stream);
+    case 192: return launch_igemm<192, 5, false>(tmA, tmB, p, stream);
+    case 160: return launch_igemm<160, 5, false>(tmA, tmB, p, stream);
+    case 128: return launch_igemm<128, 6, false>(tmA, tmB, p, stream);
+    case 64: return launch_igemm<64, 8, false>(tmA, tmB, p, stream);
     case 32: return launch_igemm<32, 8, false>(tmA, tmB, p, stream);
     default: set_error("unsupported BN %d", bn); return B200MIX_ERR_INVALID;
   }
@@ -1202,11 +1074,11 @@ static int fill_epilogue(IGemmParams& p, const b200mix_epilogue* e, void* C, lon
   bool vec = (reinterpret_cast<uintptr_t>(C) % 16 == 0) && ((ldc * out_elem) % 16 == 0);
   if (p.residual) vec = vec && (reinterpret_cast<uintptr_t>(p.residual) % 16 == 0) && ((p.ldr * 2) % 16 == 0);
   if (p.bias) vec = vec && (reinterpret_cast<uintptr_t>(p.bias) % 16 == 0);
-  // the coalesced epilogue reads the per-group vectors as float4 at (group * ld_row + 32-column chunk)
+  // the row-wise epilogue reads the per-group vectors as float2 at (group * ld_row + even column)
   if (p.row_add) vec = vec && (reinterpret_cast<uintptr_t>(p.row_add) % 16 == 0) && (p.ld_row % 4 == 0);
   if (p.row_gate) vec = vec && (reinterpret_cast<uintptr_t>(p.row_gate) % 16 == 0) && (p.ld_row % 4 == 0);
   p.vec_ok = vec ? 1 : 0;
-  // the statistics are taken in the coalesced bf16 epilogue: whole 32-column chunks, 16-byte aligned rows
+  // the statistics are taken in the row-wise bf16 epilogue: whole 16-byte pieces, 16-byte aligned rows
   B200_CHECK_ARG(!p.stats_out || (vec && !p.glu && !p.out_fp32 && p.N % 32 == 0),
                  "stats_out needs a bf16 output with N %% 32 == 0 and 16-byte aligned rows, no GLU");
   return 0;

@@ -298,6 +298,17 @@ __device__ __forceinline__ bool elect_one_sync() {
   return pred != 0;
 }
 
+// Warpgroup register reallocation: every warp of a warpgroup executes it, as the first statement of its role branch.
+// dec gives registers back to the CTA's pool, inc blocks until the requested count is available.
+template <int REGS>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS));
+}
+template <int REGS>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS));
+}
+
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
