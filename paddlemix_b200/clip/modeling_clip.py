@@ -13,7 +13,8 @@ from typing import Any, Dict, Optional, Union
 
 import torch
 
-from ..ppdiffusers.unet_2d_condition import FrozenDict, _to_t
+from ..modeling import (FrozenDict, bind, device_linear, device_vector, linear_bias, linear_weight,
+                        synthetic_state_dict, to_f32)
 
 bf16 = torch.bfloat16
 _ACTS = {"quick_gelu": 4, "gelu": 2}  # B200MIX_ACT_QUICK_GELU, B200MIX_ACT_GELU_ERF
@@ -48,23 +49,18 @@ class _CLIPBase:
 
     def _load_layers(self, P, dev):
         c = self.config
-
-        def W(n):  # Paddle Linear [in, out] -> [out, in] bf16
-            return _to_t(P[n + ".weight"]).t().contiguous()
-
-        def V(n):
-            return _to_t(P[n]).to(dev)
-
         self.layers = []
         for i in range(c.num_hidden_layers):
             b = f"{self.prefix}.encoder.layers.{i}"
             a = b + ".self_attn"
-            wqkv = torch.cat([W(a + ".q_proj"), W(a + ".k_proj"), W(a + ".v_proj")], 0)
-            bqkv = torch.cat([_to_t(P[a + f".{n}.bias"]) for n in ("q_proj", "k_proj", "v_proj")], 0)
+            qkv = [f"{a}.{n}" for n in ("q_proj", "k_proj", "v_proj")]
             self.layers.append(dict(
-                ln1=(V(b + ".layer_norm1.weight"), V(b + ".layer_norm1.bias")), ln2=(V(b + ".layer_norm2.weight"), V(b + ".layer_norm2.bias")),
-                qkv=(wqkv.to(dev, bf16).contiguous(), bqkv.to(dev)), o=(W(a + ".out_proj").to(dev, bf16), V(a + ".out_proj.bias")),
-                fc1=(W(b + ".mlp.fc1").to(dev, bf16), V(b + ".mlp.fc1.bias")), fc2=(W(b + ".mlp.fc2").to(dev, bf16), V(b + ".mlp.fc2.bias"))))
+                ln1=(device_vector(P, b + ".layer_norm1.weight", dev), device_vector(P, b + ".layer_norm1.bias", dev)),
+                ln2=(device_vector(P, b + ".layer_norm2.weight", dev), device_vector(P, b + ".layer_norm2.bias", dev)),
+                qkv=(torch.cat([linear_weight(P, n) for n in qkv], 0).to(dev, bf16),
+                     torch.cat([linear_bias(P, n) for n in qkv], 0).to(dev)),
+                o=device_linear(P, a + ".out_proj", dev), fc1=device_linear(P, b + ".mlp.fc1", dev),
+                fc2=device_linear(P, b + ".mlp.fc2", dev)))
 
     def _encoder(self, x, causal, mask):
         """CLIPEncoder.forward (:644-723): x bf16 [B,S,D] -> (last, [input of every layer..., last])."""
@@ -86,21 +82,9 @@ class _CLIPBase:
         return x, hidden
 
     def init_synthetic_weights(self, seed: int = 1, device: Union[int, str] = 0):
-        dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
-        g = torch.Generator(device=dev).manual_seed(seed)
-        P = {}
-        for name, shp in sorted(self.state_dict_shapes().items()):
-            if name.endswith(".weight") and len(shp) >= 2 and "embedding" not in name:
-                fan_in = shp[0] if len(shp) == 2 else shp[1] * shp[2] * shp[3]
-                t = (torch.rand(shp, generator=g, device=dev) * 2 - 1) / fan_in ** 0.5
-            elif "embedding" in name:
-                t = 0.3 * torch.randn(shp, generator=g, device=dev)
-            elif name.endswith(".weight"):
-                t = 1.0 + 0.1 * torch.randn(shp, generator=g, device=dev)
-            else:
-                t = 0.05 * torch.randn(shp, generator=g, device=dev)
-            P[name] = t.to(bf16)
-        return self.load_state_dict(P, device=device)
+        def special(name, shp, randn):  # token / position / class embeddings and the patch filter
+            return 0.3 * randn(shp) if "embedding" in name else None
+        return self.load_state_dict(synthetic_state_dict(self.state_dict_shapes(), seed, device, special), device)
 
 
 class CLIPTextModel(_CLIPBase):
@@ -131,20 +115,15 @@ class CLIPTextModel(_CLIPBase):
     EMBEDDING_KEYS = ("token_embedding.weight", "position_embedding.weight")
 
     def load_state_dict(self, P: Dict[str, Any], device: Union[int, str] = 0):
-        from .. import ops
-        dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
-        ops.init(dev.index or 0)
-        self.device = dev
-        missing = [k for k in self.state_dict_shapes() if k not in P]
-        if missing:
-            raise KeyError(f"state dict is missing {len(missing)} parameters, e.g. {missing[:3]}")
-        self.tok = _to_t(P["text_model.embeddings.token_embedding.weight"]).to(dev, bf16).contiguous()
-        self.pos = _to_t(P["text_model.embeddings.position_embedding.weight"]).to(dev, bf16).contiguous()
-        self.final_ln = (_to_t(P["text_model.final_layer_norm.weight"]).to(dev), _to_t(P["text_model.final_layer_norm.bias"]).to(dev))
+        dev = bind(self, P, device)
+        self.tok = to_f32(P["text_model.embeddings.token_embedding.weight"]).to(dev, bf16).contiguous()
+        self.pos = to_f32(P["text_model.embeddings.position_embedding.weight"]).to(dev, bf16).contiguous()
+        self.final_ln = (device_vector(P, "text_model.final_layer_norm.weight", dev),
+                         device_vector(P, "text_model.final_layer_norm.bias", dev))
         self._load_layers(P, dev)
         self.proj = None
         if self.with_projection:
-            self.proj = _to_t(P["text_projection.weight"]).t().contiguous().to(dev, bf16)
+            self.proj = linear_weight(P, "text_projection").to(dev, bf16)
         return self
 
     def forward(self, input_ids=None, attention_mask=None, position_ids=None, output_attentions=None,
@@ -220,25 +199,21 @@ class CLIPVisionModel(_CLIPBase):
     EMBEDDING_KEYS = ("position_embedding.weight",)
 
     def load_state_dict(self, P: Dict[str, Any], device: Union[int, str] = 0):
-        from .. import ops
-        dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
-        ops.init(dev.index or 0)
-        self.device = dev
-        missing = [k for k in self.state_dict_shapes() if k not in P]
-        if missing:
-            raise KeyError(f"state dict is missing {len(missing)} parameters, e.g. {missing[:3]}")
+        dev = bind(self, P, device)
         c = self.config
         D = c.hidden_size
-        w = _to_t(P["vision_model.embeddings.patch_embedding.weight"]).reshape(D, -1)  # [D, C*p*p], columns (c, ph, pw)
+        w = to_f32(P["vision_model.embeddings.patch_embedding.weight"]).reshape(D, -1)  # [D, C*p*p], columns (c, ph, pw)
         self.k_patch = w.shape[1]
         self.k_pad = (self.k_patch + 7) // 8 * 8  # TMA rows are 16-byte multiples: 3*14*14 = 588 -> 592 (zero columns)
         wp = torch.zeros(D, self.k_pad)
         wp[:, : self.k_patch] = w
         self.w_patch = wp.to(dev, bf16).contiguous()
-        self.cls = _to_t(P["vision_model.embeddings.class_embedding"]).to(dev, bf16)
-        self.pos = _to_t(P["vision_model.embeddings.position_embedding.weight"]).to(dev, bf16).contiguous()
-        self.pre_ln = (_to_t(P["vision_model.pre_layrnorm.weight"]).to(dev), _to_t(P["vision_model.pre_layrnorm.bias"]).to(dev))
-        self.post_ln = (_to_t(P["vision_model.post_layernorm.weight"]).to(dev), _to_t(P["vision_model.post_layernorm.bias"]).to(dev))
+        self.cls = to_f32(P["vision_model.embeddings.class_embedding"]).to(dev, bf16)
+        self.pos = to_f32(P["vision_model.embeddings.position_embedding.weight"]).to(dev, bf16).contiguous()
+        self.pre_ln = (device_vector(P, "vision_model.pre_layrnorm.weight", dev),
+                       device_vector(P, "vision_model.pre_layrnorm.bias", dev))
+        self.post_ln = (device_vector(P, "vision_model.post_layernorm.weight", dev),
+                        device_vector(P, "vision_model.post_layernorm.bias", dev))
         self._load_layers(P, dev)
         return self
 

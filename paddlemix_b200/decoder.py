@@ -10,7 +10,7 @@ from typing import Dict
 
 import torch
 
-from .ppdiffusers.unet_2d_condition import _to_t
+from .modeling import device_vector, linear_bias, linear_weight, to_f32
 
 bf16 = torch.bfloat16
 
@@ -54,27 +54,22 @@ class CausalDecoder:
 
     def load_state_dict(self, P: Dict[str, object], dev: torch.device):
         c, p = self.config, self.prefix
-
-        def W(name):  # Paddle [in, out] -> [out, in] fp32
-            return _to_t(P[name + ".weight"]).t().contiguous()
-
-        def vec(name):
-            return _to_t(P[name]).contiguous().to(dev)
-
-        self.embed = _to_t(P[f"{p}.embed_tokens.weight"]).contiguous().to(dev, bf16)
+        self.embed = to_f32(P[f"{p}.embed_tokens.weight"]).contiguous().to(dev, bf16)
         self.layers = []
         for i in range(c.num_hidden_layers):
             b = f"{p}.layers.{i}"
             qkv = [f"{b}.self_attn.{n}_proj" for n in "qkv"]
-            gate, up = W(b + ".mlp.gate_proj"), W(b + ".mlp.up_proj")  # [I, H] each
+            gate, up = linear_weight(P, b + ".mlp.gate_proj"), linear_weight(P, b + ".mlp.up_proj")  # [I, H] each
             gu = torch.stack([up, gate], 1).reshape(2 * up.shape[0], -1)  # interleave: 2j = up (value), 2j+1 = gate
             self.layers.append(dict(
-                ln1=vec(b + ".input_layernorm.weight"), ln2=vec(b + ".post_attention_layernorm.weight"),
-                qkv=torch.cat([W(n) for n in qkv], 0).to(dev, bf16),
-                qkv_bias=torch.cat([_to_t(P[n + ".bias"]) for n in qkv], 0).to(dev) if self.qkv_bias else None,
-                o=W(b + ".self_attn.o_proj").to(dev, bf16), gu=gu.to(dev, bf16), down=W(b + ".mlp.down_proj").to(dev, bf16)))
-        self.norm_w = vec(f"{p}.norm.weight")
-        self.lm_head = W("lm_head").to(dev, bf16)
+                ln1=device_vector(P, b + ".input_layernorm.weight", dev),
+                ln2=device_vector(P, b + ".post_attention_layernorm.weight", dev),
+                qkv=torch.cat([linear_weight(P, n) for n in qkv], 0).to(dev, bf16),
+                qkv_bias=torch.cat([linear_bias(P, n) for n in qkv], 0).to(dev) if self.qkv_bias else None,
+                o=linear_weight(P, b + ".self_attn.o_proj").to(dev, bf16), gu=gu.to(dev, bf16),
+                down=linear_weight(P, b + ".mlp.down_proj").to(dev, bf16)))
+        self.norm_w = device_vector(P, f"{p}.norm.weight", dev)
+        self.lm_head = linear_weight(P, "lm_head").to(dev, bf16)
         return self
 
     def _layers(self, x, attention):

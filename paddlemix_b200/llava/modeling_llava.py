@@ -16,7 +16,7 @@ import torch
 
 from ..clip import CLIPVisionModel
 from ..decoder import CausalDecoder, rope_cos_sin
-from ..ppdiffusers.unet_2d_condition import FrozenDict, _to_t
+from ..modeling import FrozenDict, bind, device_linear
 
 bf16 = torch.bfloat16
 IMAGE_TOKEN_INDEX = -200  # paddlemix/models/llava/constants.py
@@ -48,14 +48,7 @@ class LlamaForCausalLM:
         return self.decoder.state_dict_shapes()
 
     def load_state_dict(self, P: Dict[str, Any], device: Union[int, str] = 0):
-        from .. import ops
-        dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
-        ops.init(dev.index or 0)
-        self.device = dev
-        missing = [k for k in self.state_dict_shapes() if k not in P]
-        if missing:
-            raise KeyError(f"state dict is missing {len(missing)} parameters, e.g. {missing[:3]}")
-        self.decoder.load_state_dict(P, dev)
+        self.decoder.load_state_dict(P, bind(self, P, device))
         return self
 
     def _rope_tables(self, S):
@@ -113,14 +106,10 @@ class LlavaLlamaForCausalLM(LlamaForCausalLM):
         return S
 
     def load_state_dict(self, P, device=0):
-        missing = [k for k in self.state_dict_shapes() if k not in P]
-        if missing:
-            raise KeyError(f"state dict is missing {len(missing)} parameters, e.g. {missing[:3]}")
-        super().load_state_dict(P, device)
+        super().load_state_dict(P, device)  # binds and checks every key of this class's shapes, the vision tower's too
         self.vision_tower.load_state_dict({k[len(self.VT):]: v for k, v in P.items() if k.startswith(self.VT)}, device)
-        dev = self.device
-        self.proj0 = (_to_t(P["llama.mm_projector.0.weight"]).t().contiguous().to(dev, bf16), _to_t(P["llama.mm_projector.0.bias"]).to(dev))
-        self.proj2 = (_to_t(P["llama.mm_projector.2.weight"]).t().contiguous().to(dev, bf16), _to_t(P["llama.mm_projector.2.bias"]).to(dev))
+        self.proj0 = device_linear(P, "llama.mm_projector.0", self.device)
+        self.proj2 = device_linear(P, "llama.mm_projector.2", self.device)
         return self
 
     def encode_images(self, images):

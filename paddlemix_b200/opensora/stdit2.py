@@ -11,12 +11,12 @@ Device graph per block (tokens are [B, T*S, D] with row = (b*T + t)*S + s, never
   The 28 x (6+3) modulation vectors come from two GEMMs and one table-broadcast kernel per forward; all 28 cross-attn
   k|v projections of the text are one GEMM per forward.
 """
-import math
 from typing import Any, Dict, Union
 
 import torch
 
-from ..ppdiffusers.unet_2d_condition import FrozenDict, _to_t
+from ..modeling import (FrozenDict, bind, device_linear, device_vector, linear_bias, linear_weight, pad_head_cols,
+                        pad_head_rows, pad_head_vec, pad_head_width, synthetic_state_dict, to_f32)
 
 bf16 = torch.bfloat16
 
@@ -40,9 +40,9 @@ class STDiT2:
         if c.patch_size[0] != 1 or c.patch_size[1] != c.patch_size[2]:
             raise NotImplementedError("STDiT2(b200): patch_size must be (1, p, p)")
         self.head_dim = c.hidden_size // c.num_heads
-        self.head_pad = 64 if self.head_dim <= 64 else 128
-        if self.head_dim > 128 or self.head_dim % 8:
+        if self.head_dim > 128 or self.head_dim % 8:  # the temporal path runs unpadded heads of at most 128
             raise NotImplementedError("STDiT2(b200): head_dim must be a multiple of 8 and <= 128")
+        self.head_pad = pad_head_width(self.head_dim)
         self.out_channels = c.in_channels * 2 if c.pred_sigma else c.in_channels
         self.dtype = bf16
         self.device = None
@@ -77,97 +77,51 @@ class STDiT2:
         return S
 
     def init_synthetic_weights(self, seed: int = 1, device: Union[int, str] = 0):
-        dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
-        g = torch.Generator(device=dev).manual_seed(seed)
-        P = {}
         D = self.config.hidden_size
-        for name, shp in sorted(self.state_dict_shapes().items()):
-            if "scale_shift_table" in name:
-                t = torch.randn(shp, generator=g, device=dev) / D ** 0.5
-            elif name.endswith(".weight") and len(shp) >= 2:
-                fan_in = shp[0] if len(shp) == 2 else math.prod(shp[1:])
-                t = (torch.rand(shp, generator=g, device=dev) * 2 - 1) / fan_in ** 0.5
-            elif name.endswith(".weight"):
-                t = 1.0 + 0.1 * torch.randn(shp, generator=g, device=dev)
-            else:
-                t = 0.05 * torch.randn(shp, generator=g, device=dev)
-            P[name] = t.to(bf16)
-        return self.load_state_dict(P, device=device)
+
+        def special(name, shp, randn):
+            return randn(shp) / D ** 0.5 if "scale_shift_table" in name else None
+        return self.load_state_dict(synthetic_state_dict(self.state_dict_shapes(), seed, device, special), device)
 
     # ------------------------------------------------------------------------------------------------------------
-    def _pad_heads_rows(self, w):  # [H*d, in] -> [H*dp, in]
-        H, d, dp = self.config.num_heads, self.head_dim, self.head_pad
-        if d == dp:
-            return w
-        out = torch.zeros(H, dp, w.shape[-1], device=w.device)
-        out[:, :d] = w.reshape(H, d, -1)
-        return out.reshape(H * dp, -1)
-
-    def _pad_heads_vec(self, b):
-        H, d, dp = self.config.num_heads, self.head_dim, self.head_pad
-        if d == dp:
-            return b
-        out = torch.zeros(H, dp, device=b.device)
-        out[:, :d] = b.reshape(H, d)
-        return out.reshape(-1)
-
-    def _pad_heads_cols(self, w):  # [out, H*d] -> [out, H*dp]
-        H, d, dp = self.config.num_heads, self.head_dim, self.head_pad
-        if d == dp:
-            return w
-        out = torch.zeros(w.shape[0], H, dp, device=w.device)
-        out[:, :, :d] = w.reshape(w.shape[0], H, d)
-        return out.reshape(w.shape[0], H * dp)
-
     def load_state_dict(self, P: Dict[str, Any], device: Union[int, str] = 0):
-        from .. import ops
-        dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
-        ops.init(dev.index or 0)
-        self.device = dev
-        missing = [k for k in self.state_dict_shapes() if k not in P]
-        if missing:
-            raise KeyError(f"state dict is missing {len(missing)} parameters, e.g. {missing[:3]}")
+        dev = bind(self, P, device)
         c, D = self.config, self.config.hidden_size
+        H, d, dp = c.num_heads, self.head_dim, self.head_pad
 
-        def W(name):
-            return _to_t(P[name + ".weight"]).t().contiguous()
-
-        def Bv(name):
-            return _to_t(P[name + ".bias"])
-
-        def lin(name):
-            return (W(name).to(dev, bf16).contiguous(), Bv(name).to(dev).contiguous())
-
-        self.w_patch = (_to_t(P["x_embedder.proj.weight"]).reshape(D, -1).contiguous().to(dev, bf16), Bv("x_embedder.proj").to(dev))
-        self.t_emb = (lin("t_embedder.mlp.0"), lin("t_embedder.mlp.2"))
-        self.size_emb = {n: (lin(n + ".mlp.0"), lin(n + ".mlp.2")) for n in ("csize_embedder", "ar_embedder", "fl_embedder", "fps_embedder")}
-        self.t_block, self.t_block_temp = lin("t_block.1"), lin("t_block_temp.1")
-        self.y_fc1, self.y_fc2 = lin("y_embedder.y_proj.fc1"), lin("y_embedder.y_proj.fc2")
-        self.tab_spc = torch.cat([_to_t(P[f"blocks.{i}.scale_shift_table"]).reshape(1, 6 * D) for i in range(c.depth)], 0).to(dev).contiguous()
-        self.tab_tmp = torch.cat([_to_t(P[f"blocks.{i}.scale_shift_table_temporal"]).reshape(1, 3 * D) for i in range(c.depth)], 0).to(dev).contiguous()
-        self.tab_final = _to_t(P["final_layer.scale_shift_table"]).reshape(1, 2 * D).to(dev).contiguous()
-        self.final = lin("final_layer.linear")
+        self.w_patch = (to_f32(P["x_embedder.proj.weight"]).reshape(D, -1).contiguous().to(dev, bf16),
+                        device_vector(P, "x_embedder.proj.bias", dev))
+        self.t_emb = tuple(device_linear(P, n, dev) for n in ("t_embedder.mlp.0", "t_embedder.mlp.2"))
+        self.size_emb = {n: (device_linear(P, n + ".mlp.0", dev), device_linear(P, n + ".mlp.2", dev))
+                         for n in ("csize_embedder", "ar_embedder", "fl_embedder", "fps_embedder")}
+        self.t_block, self.t_block_temp = device_linear(P, "t_block.1", dev), device_linear(P, "t_block_temp.1", dev)
+        self.y_fc1, self.y_fc2 = device_linear(P, "y_embedder.y_proj.fc1", dev), device_linear(P, "y_embedder.y_proj.fc2", dev)
+        self.tab_spc = torch.cat([to_f32(P[f"blocks.{i}.scale_shift_table"]).reshape(1, 6 * D) for i in range(c.depth)], 0).to(dev).contiguous()
+        self.tab_tmp = torch.cat([to_f32(P[f"blocks.{i}.scale_shift_table_temporal"]).reshape(1, 3 * D) for i in range(c.depth)], 0).to(dev).contiguous()
+        self.tab_final = to_f32(P["final_layer.scale_shift_table"]).reshape(1, 2 * D).to(dev).contiguous()
+        self.final = device_linear(P, "final_layer.linear", dev)
         self.blocks = []
         kv_w, kv_b = [], []
         for i in range(c.depth):
             b = f"blocks.{i}"
             blk = {}
-            wqkv, bqkv = W(b + ".attn.qkv"), Bv(b + ".attn.qkv")  # rows (3, H, d)
-            blk["s_qkv"] = (torch.cat([self._pad_heads_rows(wqkv[j * D:(j + 1) * D]) for j in range(3)], 0).to(dev, bf16).contiguous(),
-                            torch.cat([self._pad_heads_vec(bqkv[j * D:(j + 1) * D]) for j in range(3)], 0).to(dev).contiguous())
-            blk["s_proj"] = (self._pad_heads_cols(W(b + ".attn.proj")).to(dev, bf16).contiguous(), Bv(b + ".attn.proj").to(dev))
-            blk["t_qkv"], blk["t_proj"] = lin(b + ".attn_temp.qkv"), lin(b + ".attn_temp.proj")
+            # q|k|v rows are (3, H, d) and k|v rows (2, H, d): padded as 3H / 2H heads
+            blk["s_qkv"] = (pad_head_rows(linear_weight(P, b + ".attn.qkv"), 3 * H, d, dp).to(dev, bf16).contiguous(),
+                            pad_head_vec(linear_bias(P, b + ".attn.qkv"), 3 * H, d, dp).to(dev).contiguous())
+            blk["s_proj"] = (pad_head_cols(linear_weight(P, b + ".attn.proj"), H, d, dp).to(dev, bf16).contiguous(),
+                             device_vector(P, b + ".attn.proj.bias", dev))
+            blk["t_qkv"], blk["t_proj"] = device_linear(P, b + ".attn_temp.qkv", dev), device_linear(P, b + ".attn_temp.proj", dev)
             if c.qk_norm:
                 for a, key in (("attn", "s"), ("attn_temp", "t")):
-                    blk[key + "_qn"] = _to_t(P[f"{b}.{a}.q_norm.weight"]).to(dev).contiguous()
-                    blk[key + "_kn"] = _to_t(P[f"{b}.{a}.k_norm.weight"]).to(dev).contiguous()
-            blk["c_q"] = (self._pad_heads_rows(W(b + ".cross_attn.q_linear")).to(dev, bf16).contiguous(),
-                          self._pad_heads_vec(Bv(b + ".cross_attn.q_linear")).to(dev).contiguous())
-            wkv, bkv = W(b + ".cross_attn.kv_linear"), Bv(b + ".cross_attn.kv_linear")  # rows (2, H, d)
-            kv_w.append(torch.cat([self._pad_heads_rows(wkv[:D]), self._pad_heads_rows(wkv[D:])], 0))
-            kv_b.append(torch.cat([self._pad_heads_vec(bkv[:D]), self._pad_heads_vec(bkv[D:])], 0))
-            blk["c_proj"] = (self._pad_heads_cols(W(b + ".cross_attn.proj")).to(dev, bf16).contiguous(), Bv(b + ".cross_attn.proj").to(dev))
-            blk["fc1"], blk["fc2"] = lin(b + ".mlp.fc1"), lin(b + ".mlp.fc2")
+                    blk[key + "_qn"] = device_vector(P, f"{b}.{a}.q_norm.weight", dev)
+                    blk[key + "_kn"] = device_vector(P, f"{b}.{a}.k_norm.weight", dev)
+            blk["c_q"] = (pad_head_rows(linear_weight(P, b + ".cross_attn.q_linear"), H, d, dp).to(dev, bf16).contiguous(),
+                          pad_head_vec(linear_bias(P, b + ".cross_attn.q_linear"), H, d, dp).to(dev).contiguous())
+            kv_w.append(pad_head_rows(linear_weight(P, b + ".cross_attn.kv_linear"), 2 * H, d, dp))
+            kv_b.append(pad_head_vec(linear_bias(P, b + ".cross_attn.kv_linear"), 2 * H, d, dp))
+            blk["c_proj"] = (pad_head_cols(linear_weight(P, b + ".cross_attn.proj"), H, d, dp).to(dev, bf16).contiguous(),
+                             device_vector(P, b + ".cross_attn.proj.bias", dev))
+            blk["fc1"], blk["fc2"] = device_linear(P, b + ".mlp.fc1", dev), device_linear(P, b + ".mlp.fc2", dev)
             self.blocks.append(blk)
         self.kv_w = torch.cat(kv_w, 0).to(dev, bf16).contiguous()  # all blocks' cross-attn k|v projections: one GEMM
         self.kv_b = torch.cat(kv_b, 0).to(dev).contiguous()

@@ -15,7 +15,8 @@ from typing import Any, Dict, Tuple, Union
 
 import torch
 
-from .unet_2d_condition import FrozenDict, _Conv3x3, _Linear, _Norm, _to_t
+from ..modeling import FrozenDict, bind, linear_bias, linear_weight, synthetic_state_dict, to_f32
+from .unet_2d_condition import _Conv3x3, _Linear, _Norm
 
 bf16 = torch.bfloat16
 
@@ -102,40 +103,22 @@ class AutoencoderKL:
         return S
 
     def init_synthetic_weights(self, seed: int = 1, device: Union[int, str] = 0):
-        dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
-        g = torch.Generator(device=dev).manual_seed(seed)
-        P = {}
-        for name, shp in sorted(self.state_dict_shapes().items()):
-            if name.endswith(".weight") and len(shp) >= 2:
-                fan_in = shp[0] if len(shp) == 2 else shp[1] * shp[2] * shp[3]
-                t = (torch.rand(shp, generator=g, device=dev) * 2 - 1) / fan_in ** 0.5
-            elif name.endswith(".weight"):
-                t = 1.0 + 0.1 * torch.randn(shp, generator=g, device=dev)
-            else:
-                t = 0.05 * torch.randn(shp, generator=g, device=dev)
-            P[name] = t.to(bf16)
-        return self.load_state_dict(P, device=device)
+        return self.load_state_dict(synthetic_state_dict(self.state_dict_shapes(), seed, device), device)
 
     def load_state_dict(self, P: Dict[str, Any], device: Union[int, str] = 0):
-        from .. import ops
-        dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
-        ops.init(dev.index or 0)
-        self.device = dev
-        missing = [k for k in self.state_dict_shapes() if k not in P]
-        if missing:
-            raise KeyError(f"state dict is missing {len(missing)} parameters, e.g. {missing[:3]}")
+        dev = bind(self, P, device)
         c = self.config
         lc, C = c.latent_channels, c.block_out_channels[-1]
         # post_quant_conv (1x1, lc -> lc) as a 3x3 filter with only the centre tap set, output padded to 8 channels
         # (zeros), so that conv_in reads an 8-channel NHWC tensor: both run on the tiny-Cin conv kernel
         wpq = torch.zeros(8, 3, 3, lc)
-        wpq[:lc, 1, 1, :] = _to_t(P["post_quant_conv.weight"])[:, :, 0, 0].cpu()
+        wpq[:lc, 1, 1, :] = to_f32(P["post_quant_conv.weight"])[:, :, 0, 0].cpu()
         bpq = torch.zeros(8)
-        bpq[:lc] = _to_t(P["post_quant_conv.bias"]).cpu()
+        bpq[:lc] = to_f32(P["post_quant_conv.bias"]).cpu()
         self.pq_w, self.pq_b = wpq.to(dev, bf16).contiguous(), bpq.to(dev)
         win = torch.zeros(C, 3, 3, 8)
-        win[:, :, :, :lc] = _to_t(P["decoder.conv_in.weight"]).permute(0, 2, 3, 1).cpu()
-        self.in_w, self.in_b = win.to(dev, bf16).contiguous(), _to_t(P["decoder.conv_in.bias"]).to(dev)
+        win[:, :, :, :lc] = to_f32(P["decoder.conv_in.weight"]).permute(0, 2, 3, 1).cpu()
+        self.in_w, self.in_b = win.to(dev, bf16).contiguous(), to_f32(P["decoder.conv_in.bias"]).to(dev)
         leaves = [*self.mid_res0.parts(), *self.mid_res1.parts(), self.attn_norm, self.attn_out, self.norm_out, self.conv_out]
         for res, ups in self.up:
             for r in res:
@@ -145,8 +128,8 @@ class AutoencoderKL:
         for m in leaves:
             m.load(P, dev)
         a = "decoder.mid_block.attentions.0"
-        self.qkv_w = torch.cat([_to_t(P[f"{a}.{n}.weight"]).t() for n in ("to_q", "to_k", "to_v")], 0).contiguous().to(dev, bf16)
-        self.qkv_b = torch.cat([_to_t(P[f"{a}.{n}.bias"]) for n in ("to_q", "to_k", "to_v")], 0).to(dev)
+        self.qkv_w = torch.cat([linear_weight(P, f"{a}.{n}") for n in ("to_q", "to_k", "to_v")], 0).to(dev, bf16)
+        self.qkv_b = torch.cat([linear_bias(P, f"{a}.{n}") for n in ("to_q", "to_k", "to_v")], 0).to(dev)
         self._scratch = {}
         return self
 

@@ -16,7 +16,8 @@ from typing import Any, Dict, List, Optional, Sequence, Tuple, Union
 
 import torch
 
-from .unet_2d_condition import FrozenDict, UNet2DConditionModel, _check_reference_defaults, _Conv3x3, _Linear
+from ..modeling import FrozenDict, synthetic_state_dict
+from .unet_2d_condition import UNet2DConditionModel, _check_reference_defaults, _Conv3x3, _Linear
 
 bf16 = torch.bfloat16
 
@@ -188,7 +189,7 @@ class ControlNetModel(UNet2DConditionModel):
                  conditioning_embedding_out_channels=conditioning_embedding_out_channels,
                  conditioning_channels=conditioning_channels)
         shapes = cn.state_dict_shapes()
-        P = _synthetic_state_dict(shapes, seed)
+        P = synthetic_state_dict(shapes, seed, "cpu")
         for k in shapes:
             if k.startswith(("controlnet_down_blocks.", "controlnet_mid_block.", "controlnet_cond_embedding.conv_out.")):
                 P[k] = torch.zeros(shapes[k], dtype=bf16)
@@ -380,19 +381,3 @@ def _to_nhwc(t, nhwc_in, keep_fp32):
         return t
     return ops.cast(t, bf16)
 
-
-def _synthetic_state_dict(shapes: Dict[str, tuple], seed: int) -> Dict[str, torch.Tensor]:
-    """Host bf16 weights with UNet2DConditionModel.init_synthetic_weights' distribution (there are no checkpoints
-    offline): U(-1/sqrt(fan_in), 1/sqrt(fan_in)) matrices, small biases, norm scales around 1."""
-    g = torch.Generator().manual_seed(seed)
-    P = {}
-    for name, shp in sorted(shapes.items()):
-        if name.endswith(".weight") and len(shp) >= 2:
-            fan_in = shp[0] if len(shp) == 2 else shp[1] * shp[2] * shp[3]
-            t = (torch.rand(shp, generator=g) * 2 - 1) / fan_in ** 0.5
-        elif name.endswith(".weight"):
-            t = 1.0 + 0.1 * torch.randn(shp, generator=g)
-        else:
-            t = 0.05 * torch.randn(shp, generator=g)
-        P[name] = t.to(bf16)
-    return P

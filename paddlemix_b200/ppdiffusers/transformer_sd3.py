@@ -17,7 +17,8 @@ from typing import Any, Dict, Optional, Union
 
 import torch
 
-from .unet_2d_condition import FrozenDict, _to_t
+from ..modeling import (FrozenDict, bind, device_linear, device_vector, linear_bias, linear_weight, synthetic_state_dict,
+                        to_f32)
 
 bf16 = torch.bfloat16
 
@@ -91,45 +92,23 @@ class SD3Transformer2DModel:
                 if k not in sd}
 
     def init_synthetic_weights(self, seed: int = 1, device: Union[int, str] = 0):
-        dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
-        g = torch.Generator(device=dev).manual_seed(seed)
-        P = {}
-        for name, shp in sorted(self.state_dict_shapes().items()):
-            if name == "pos_embed.pos_embed":
-                t = 0.5 * torch.randn(shp, generator=g, device=dev)
-            elif name.endswith(".weight"):
-                fan_in = shp[0] if len(shp) == 2 else shp[1] * shp[2] * shp[3]
-                t = (torch.rand(shp, generator=g, device=dev) * 2 - 1) / fan_in ** 0.5
-            else:
-                t = 0.05 * torch.randn(shp, generator=g, device=dev)
-            P[name] = t.to(bf16)
-        return self.load_state_dict(P, device=device)
+        def special(name, shp, randn):
+            return 0.5 * randn(shp) if name == "pos_embed.pos_embed" else None
+        return self.load_state_dict(synthetic_state_dict(self.state_dict_shapes(), seed, device, special), device)
 
     def load_state_dict(self, P: Dict[str, Any], device: Union[int, str] = 0):
-        from .. import ops
-        dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
-        ops.init(dev.index or 0)
-        self.device = dev
-        missing = [k for k in self.state_dict_shapes() if k not in P]
-        if missing:
-            raise KeyError(f"state dict is missing {len(missing)} parameters, e.g. {missing[:3]}")
+        dev = bind(self, P, device)
         c, D = self.config, self.inner_dim
 
-        def W(name):  # Paddle Linear [in, out] -> [out, in] bf16
-            return _to_t(P[name + ".weight"]).t().contiguous().to(dev, bf16)
-
-        def Bv(name):
-            return _to_t(P[name + ".bias"]).to(dev)
-
-        self.w_patch = _to_t(P["pos_embed.proj.weight"]).reshape(D, -1).contiguous().to(dev, bf16)  # [D, C*p*p]
-        self.b_patch = Bv("pos_embed.proj")
-        self.pos_table = _to_t(P["pos_embed.pos_embed"]).reshape(c.pos_embed_max_size, c.pos_embed_max_size, D).to(dev)
+        self.w_patch = to_f32(P["pos_embed.proj.weight"]).reshape(D, -1).contiguous().to(dev, bf16)  # [D, C*p*p]
+        self.b_patch = device_vector(P, "pos_embed.proj.bias", dev)
+        self.pos_table = to_f32(P["pos_embed.pos_embed"]).reshape(c.pos_embed_max_size, c.pos_embed_max_size, D).to(dev)
         self._pos_cache = {}
-        self.t1, self.t2 = (W("time_text_embed.timestep_embedder.linear_1"), Bv("time_text_embed.timestep_embedder.linear_1")), \
-                           (W("time_text_embed.timestep_embedder.linear_2"), Bv("time_text_embed.timestep_embedder.linear_2"))
-        self.p1, self.p2 = (W("time_text_embed.text_embedder.linear_1"), Bv("time_text_embed.text_embedder.linear_1")), \
-                           (W("time_text_embed.text_embedder.linear_2"), Bv("time_text_embed.text_embedder.linear_2"))
-        self.ctx_emb = (W("context_embedder"), Bv("context_embedder"))
+        self.t1 = device_linear(P, "time_text_embed.timestep_embedder.linear_1", dev)
+        self.t2 = device_linear(P, "time_text_embed.timestep_embedder.linear_2", dev)
+        self.p1 = device_linear(P, "time_text_embed.text_embedder.linear_1", dev)
+        self.p2 = device_linear(P, "time_text_embed.text_embedder.linear_2", dev)
+        self.ctx_emb = device_linear(P, "context_embedder", dev)
         # one GEMM for every AdaLN projection: rows = [blk0.norm1 (6D) | blk0.norm1_context (6D|2D) | ... | norm_out (2D)]
         ws, bs, self.mod_off = [], [], []
         off = 0
@@ -139,31 +118,30 @@ class SD3Transformer2DModel:
             last = i == c.num_layers - 1
             blk = dict(last=last)
             for key in ("norm1", "norm1_context"):
-                w, bias = _to_t(P[f"{b}.{key}.linear.weight"]).t().contiguous(), _to_t(P[f"{b}.{key}.linear.bias"])
+                w, bias = linear_weight(P, f"{b}.{key}.linear"), linear_bias(P, f"{b}.{key}.linear")
                 blk[key + "_off"] = off
                 off += w.shape[0]
                 ws.append(w), bs.append(bias)
-            blk["w_qkv"] = torch.cat([W(f"{b}.attn.to_q"), W(f"{b}.attn.to_k"), W(f"{b}.attn.to_v")], 0).contiguous()
-            blk["b_qkv"] = torch.cat([Bv(f"{b}.attn.to_q"), Bv(f"{b}.attn.to_k"), Bv(f"{b}.attn.to_v")], 0).contiguous()
-            blk["w_cqkv"] = torch.cat([W(f"{b}.attn.add_q_proj"), W(f"{b}.attn.add_k_proj"), W(f"{b}.attn.add_v_proj")], 0).contiguous()
-            blk["b_cqkv"] = torch.cat([Bv(f"{b}.attn.add_q_proj"), Bv(f"{b}.attn.add_k_proj"), Bv(f"{b}.attn.add_v_proj")], 0).contiguous()
-            blk["w_o"], blk["b_o"] = W(f"{b}.attn.to_out.0"), Bv(f"{b}.attn.to_out.0")
-            blk["ff1"], blk["ff2"] = (W(f"{b}.ff.net.0.proj"), Bv(f"{b}.ff.net.0.proj")), (W(f"{b}.ff.net.2"), Bv(f"{b}.ff.net.2"))
+            for key, names in (("qkv", ("to_q", "to_k", "to_v")), ("cqkv", ("add_q_proj", "add_k_proj", "add_v_proj"))):
+                blk["w_" + key] = torch.cat([linear_weight(P, f"{b}.attn.{n}") for n in names], 0).to(dev, bf16)
+                blk["b_" + key] = torch.cat([linear_bias(P, f"{b}.attn.{n}") for n in names], 0).to(dev)
+            blk["w_o"], blk["b_o"] = device_linear(P, f"{b}.attn.to_out.0", dev)
+            blk["ff1"], blk["ff2"] = device_linear(P, f"{b}.ff.net.0.proj", dev), device_linear(P, f"{b}.ff.net.2", dev)
             if last:
-                blk["ctx_ln_bias"] = _to_t(P[f"{b}.norm1_context.norm.bias"]).to(dev)
+                blk["ctx_ln_bias"] = device_vector(P, f"{b}.norm1_context.norm.bias", dev)
             else:
-                blk["w_co"], blk["b_co"] = W(f"{b}.attn.to_add_out"), Bv(f"{b}.attn.to_add_out")
-                blk["cff1"] = (W(f"{b}.ff_context.net.0.proj"), Bv(f"{b}.ff_context.net.0.proj"))
-                blk["cff2"] = (W(f"{b}.ff_context.net.2"), Bv(f"{b}.ff_context.net.2"))
+                blk["w_co"], blk["b_co"] = device_linear(P, f"{b}.attn.to_add_out", dev)
+                blk["cff1"] = device_linear(P, f"{b}.ff_context.net.0.proj", dev)
+                blk["cff2"] = device_linear(P, f"{b}.ff_context.net.2", dev)
             self.blocks.append(blk)
-        w, bias = _to_t(P["norm_out.linear.weight"]).t().contiguous(), _to_t(P["norm_out.linear.bias"])
+        w, bias = linear_weight(P, "norm_out.linear"), linear_bias(P, "norm_out.linear")
         self.norm_out_off = off
         off += w.shape[0]
         ws.append(w), bs.append(bias)
         self.mod_w = torch.cat(ws, 0).to(dev, bf16).contiguous()
         self.mod_b = torch.cat(bs, 0).to(dev).contiguous()
-        self.norm_out_bias = _to_t(P["norm_out.norm.bias"]).to(dev)
-        self.proj_out = (W("proj_out"), Bv("proj_out"))
+        self.norm_out_bias = device_vector(P, "norm_out.norm.bias", dev)
+        self.proj_out = device_linear(P, "proj_out", dev)
         return self
 
     # ------------------------------------------------------------------------------------------------------------

@@ -18,8 +18,10 @@ from types import SimpleNamespace
 from typing import Any, Dict, Optional, Tuple, Union
 
 import os
-import numpy as np
 import torch
+
+from ..modeling import (FrozenDict, bind, linear_bias, linear_weight, pad_head_cols, pad_head_rows, pad_head_width,
+                        synthetic_state_dict, to_f32)
 
 bf16 = torch.bfloat16
 
@@ -28,19 +30,6 @@ bf16 = torch.bfloat16
 class UNet2DConditionOutput:
     """ppdiffusers.models.unet_2d_condition.UNet2DConditionOutput (:55-65)."""
     sample: torch.Tensor = None
-
-
-class FrozenDict(dict):
-    """Attribute-style read-only config, like ppdiffusers.configuration_utils.FrozenDict (:58)."""
-
-    def __getattr__(self, k):
-        try:
-            return self[k]
-        except KeyError as e:
-            raise AttributeError(k) from e
-
-    def __setattr__(self, k, v):
-        raise Exception(f"You cannot use ``__setattr__`` on a {self.__class__.__name__} instance.")
 
 
 # reference defaults of the UNet2DConditionModel constructor arguments this mirror does not implement
@@ -74,20 +63,6 @@ def _tup(v, n):
     return tuple(v) if isinstance(v, (tuple, list)) else (v,) * n
 
 
-def _pad_head(d):
-    for p in (64, 128, 192):
-        if d <= p:
-            return p
-    raise ValueError(f"attention head size {d} > 192 is not supported by the sm_90a attention kernel")
-
-
-def _to_t(x):
-    """fp32 view of a parameter on whatever device it already lives on (host numpy / torch, or CUDA)."""
-    if isinstance(x, np.ndarray):
-        x = torch.from_numpy(x)
-    return x.detach().to(torch.float32)
-
-
 class AttnProcessorB200:
     """Default attention processor: fused qkv projection + flash SDPA + out-projection kernels.
     Follows the reference processor protocol (attention_processor.py:352-385, 673-735):
@@ -103,7 +78,7 @@ class Attention:
     def __init__(self, name, heads, dim, ctx_dim, is_cross):
         self.name, self.heads, self.dim, self.ctx_dim, self.is_cross = name, heads, dim, ctx_dim, is_cross
         self.head_dim = dim // heads
-        self.head_pad = _pad_head(self.head_dim)
+        self.head_pad = pad_head_width(self.head_dim)
         self.scale = self.head_dim ** -0.5
         self.inner = heads * self.head_pad
         self.processor = AttnProcessorB200()
@@ -118,30 +93,14 @@ class Attention:
                 n + ".to_out.0.weight": (c, c), n + ".to_out.0.bias": (c,)}
 
     # -- weight preparation ------------------------------------------------------------------------------------
-    def _pad_rows(self, w_out_in):  # [H*d, in] -> [H*dp, in]
-        H, d, dp = self.heads, self.head_dim, self.head_pad
-        if d == dp:
-            return w_out_in
-        w = w_out_in.reshape(H, d, -1)
-        out = torch.zeros(H, dp, w.shape[-1], device=w.device)
-        out[:, :d] = w
-        return out.reshape(H * dp, -1)
-
     def load(self, P, dev, norm=None):
         """norm: the LayerNorm in front of this layer (BasicTransformerBlock.norm1 / norm2); its affine is folded into a
         second copy of the query-side projection so that the block can run without the LayerNorm kernel (see
         _BasicTransformerBlock.__call__); the plain weights stay for custom processors."""
         from .. import ops
-        n = self.name
-        wq = self._pad_rows(_to_t(P[n + ".to_q.weight"]).t().contiguous())
-        wk = self._pad_rows(_to_t(P[n + ".to_k.weight"]).t().contiguous())
-        wv = self._pad_rows(_to_t(P[n + ".to_v.weight"]).t().contiguous())
-        wo = _to_t(P[n + ".to_out.0.weight"]).t().contiguous()  # [C, H*d]
-        H, d, dp = self.heads, self.head_dim, self.head_pad
-        if d != dp:
-            wo3 = torch.zeros(wo.shape[0], H, dp, device=wo.device)
-            wo3[:, :, :d] = wo.reshape(wo.shape[0], H, d)
-            wo = wo3.reshape(wo.shape[0], H * dp)
+        n, H, d, dp = self.name, self.heads, self.head_dim, self.head_pad
+        wq, wk, wv = (pad_head_rows(linear_weight(P, f"{n}.{p}"), H, d, dp) for p in ("to_q", "to_k", "to_v"))
+        wo = pad_head_cols(linear_weight(P, n + ".to_out.0"), H, d, dp)  # [C, H*dp]
         if self.is_cross:
             self.w_q = wq.to(dev, bf16).contiguous()
             self.w_kv_host = torch.cat([wk, wv], 0)  # batched across blocks by the model
@@ -153,7 +112,7 @@ class Attention:
         if norm is not None:
             self.ln_fold = ops.fold_layernorm_into_linear(w_in.to(dev, torch.float32), norm.w, norm.b)
         self.w_o = wo.to(dev, bf16).contiguous()
-        self.b_o = _to_t(P[n + ".to_out.0.bias"]).to(dev)
+        self.b_o = linear_bias(P, n + ".to_out.0").to(dev)
 
     # -- reference-style sub-layers for custom processors --------------------------------------------------------
     def to_q(self, x):
@@ -216,8 +175,8 @@ class _Norm:
         return {self.name + ".weight": (self.c,), self.name + ".bias": (self.c,)}
 
     def load(self, P, dev):
-        self.w = _to_t(P[self.name + ".weight"]).to(dev)
-        self.b = _to_t(P[self.name + ".bias"]).to(dev)
+        self.w = to_f32(P[self.name + ".weight"]).to(dev)
+        self.b = to_f32(P[self.name + ".bias"]).to(dev)
 
 
 class _Linear:
@@ -229,14 +188,14 @@ class _Linear:
         return {self.name + ".weight": w, self.name + ".bias": (self.cout,)}
 
     def load(self, P, dev):
-        w = _to_t(P[self.name + ".weight"])
+        w = to_f32(P[self.name + ".weight"])
         if w.ndim == 4:  # 1x1 conv [out, in, 1, 1]
             w = w[:, :, 0, 0]
         else:  # Paddle Linear [in, out]
             w = w.t()
         self.w = w.contiguous().to(dev, bf16)
         b = P.get(self.name + ".bias")
-        self.b = None if b is None else _to_t(b).to(dev)
+        self.b = None if b is None else to_f32(b).to(dev)
 
 
 class _Conv3x3:
@@ -249,9 +208,9 @@ class _Conv3x3:
         return {self.name + ".weight": (self.cout, self.cin, 3, 3), self.name + ".bias": (self.cout,)}
 
     def load(self, P, dev):
-        w = _to_t(P[self.name + ".weight"])  # [O, I, 3, 3] -> [O, 3, 3, I]
+        w = to_f32(P[self.name + ".weight"])  # [O, I, 3, 3] -> [O, 3, 3, I]
         self.w = w.permute(0, 2, 3, 1).contiguous().to(dev, bf16)
-        self.b = _to_t(P[self.name + ".bias"]).to(dev)
+        self.b = to_f32(P[self.name + ".bias"]).to(dev)
         if self.upsample:
             from .. import ops
             self.w4 = ops.fold_upsample_conv_weight(w.permute(0, 2, 3, 1).to(dev, torch.float32))
@@ -287,8 +246,8 @@ class _Resnet:
             m.load(P, dev)
         if self.shortcut is not None:
             self.shortcut.load(P, dev)
-        self.temb_w = _to_t(P[self.name + ".time_emb_proj.weight"]).t().contiguous()  # [cout, ted], batched later
-        self.temb_b = _to_t(P[self.name + ".time_emb_proj.bias"])
+        self.temb_w = linear_weight(P, self.name + ".time_emb_proj")  # [cout, ted], batched later
+        self.temb_b = linear_bias(P, self.name + ".time_emb_proj")
 
     def __call__(self, x, temb_all, skip=None):
         from .. import ops
@@ -338,8 +297,8 @@ class _BasicTransformerBlock:
         self.attn2.load(P, dev, norm=self.norm2)
         self.attn1.ln_eps = self.attn2.ln_eps = self.LN_EPS
         # GEGLU: proj(x).chunk(2) = (value, gate) -> interleave rows so both land in the same accumulator tile
-        w = _to_t(P[self.name + ".ff.net.0.proj.weight"]).t().contiguous()  # [8C, C]
-        b = _to_t(P[self.name + ".ff.net.0.proj.bias"])
+        w = linear_weight(P, self.name + ".ff.net.0.proj")  # [8C, C]
+        b = linear_bias(P, self.name + ".ff.net.0.proj")
         half = w.shape[0] // 2
         w_il = torch.stack([w[:half], w[half:]], 1).reshape(2 * half, -1).contiguous()
         b_il = torch.stack([b[:half], b[half:]], 1).reshape(2 * half).contiguous()
@@ -582,20 +541,8 @@ class UNet2DConditionModel:
 
     def init_synthetic_weights(self, seed: int = 1, device: Union[int, str] = 0):
         """Random-init weights of this architecture generated directly on the device (there are no checkpoints
-        offline): U(-1/sqrt(fan_in), 1/sqrt(fan_in)) matrices, small biases, norm scales around 1."""
-        dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
-        g = torch.Generator(device=dev).manual_seed(seed)
-        P = {}
-        for name, shp in sorted(self.state_dict_shapes().items()):
-            if name.endswith(".weight") and len(shp) >= 2:
-                fan_in = shp[0] if len(shp) == 2 else shp[1] * shp[2] * shp[3]
-                t = (torch.rand(shp, generator=g, device=dev) * 2 - 1) / fan_in ** 0.5
-            elif name.endswith(".weight"):
-                t = 1.0 + 0.1 * torch.randn(shp, generator=g, device=dev)
-            else:
-                t = 0.05 * torch.randn(shp, generator=g, device=dev)
-            P[name] = t.to(bf16)
-        return self.load_state_dict(P, device=device)
+        offline, see modeling.synthetic_state_dict)."""
+        return self.load_state_dict(synthetic_state_dict(self.state_dict_shapes(), seed, device), device)
 
     # ------------------------------------------------------------------------------------------------------------
     @property
@@ -628,14 +575,8 @@ class UNet2DConditionModel:
     def load_state_dict(self, state_dict: Dict[str, Any], device: Union[int, str] = 0):
         """Reference-named parameters (ppdiffusers state-dict keys, Paddle layouts). Every Linear is transposed once,
         convs go to [O,kh,kw,I], q/k/v (and cross k/v, time_emb_proj) are concatenated for batched GEMMs."""
-        from .. import ops
-        dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
-        ops.init(dev.index or 0)
-        self.device = dev
         P = state_dict
-        missing = [k for k in self.state_dict_shapes() if k not in P]
-        if missing:
-            raise KeyError(f"state dict is missing {len(missing)} parameters, e.g. {missing[:3]}")
+        dev = bind(self, P, device)
         for m in self._leaves():
             m.load(P, dev)
         # batched time_emb_proj: one GEMM [B, ted] x [sum(cout), ted]^T per forward

@@ -14,14 +14,14 @@ Device graph (one process per GPU, every arithmetic op is a libb200mix kernel):
 Host side (pure index math, no arithmetic on activations): get_rope_index (:1217-1360), rot_pos_emb (:940-971),
 the cos/sin tables of both rotary embeddings.
 """
-import math
 from dataclasses import dataclass
 from typing import Any, Dict, List, Optional, Union
 
 import torch
 
 from ..decoder import CausalDecoder, rope_cos_sin
-from ..ppdiffusers.unet_2d_condition import FrozenDict, _to_t
+from ..modeling import (FrozenDict, bind, device_linear, device_vector, linear_bias, linear_weight, pad_head_cols,
+                        pad_head_rows, pad_head_vec, pad_head_width, synthetic_state_dict, to_f32)
 
 bf16 = torch.bfloat16
 
@@ -145,22 +145,6 @@ class GraphedDecodeStep:
         return self.logits
 
 
-def _pad_rows(w, heads, d, dp):  # [heads*d, in] -> [heads*dp, in]
-    if d == dp:
-        return w
-    out = torch.zeros(heads, dp, w.shape[-1], device=w.device)
-    out[:, :d] = w.reshape(heads, d, -1)
-    return out.reshape(heads * dp, -1)
-
-
-def _pad_vec(b, heads, d, dp):
-    if d == dp:
-        return b
-    out = torch.zeros(heads, dp, device=b.device)
-    out[:, :d] = b.reshape(heads, d)
-    return out.reshape(-1)
-
-
 class Qwen2VLForConditionalGeneration:
     def __init__(self, config: Union[Qwen2VLConfig, Dict[str, Any]]):
         self.config = config if isinstance(config, Qwen2VLConfig) else Qwen2VLConfig(**config)
@@ -172,7 +156,7 @@ class Qwen2VLForConditionalGeneration:
         if self.head_dim not in (64, 128):
             raise NotImplementedError("Qwen2VL(b200): LLM head_dim must be 64 or 128")
         self.v_head = c.vision["embed_dim"] // c.vision["num_heads"]
-        self.v_pad = 64 if self.v_head <= 64 else 128
+        self.v_pad = pad_head_width(self.v_head)
         self.decoder = CausalDecoder(c, "model", qkv_bias=True)
         self.dtype = bf16
         self.device = None
@@ -209,62 +193,33 @@ class Qwen2VLForConditionalGeneration:
         return {}
 
     def init_synthetic_weights(self, seed: int = 1, device: Union[int, str] = 0):
-        dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
-        g = torch.Generator(device=dev).manual_seed(seed)
-        P = {}
-        for name, shp in sorted(self.state_dict_shapes().items()):
-            if name == "model.embed_tokens.weight":
-                t = 0.5 * torch.randn(shp, generator=g, device=dev)
-            elif name.endswith(".weight") and len(shp) >= 2:
-                fan_in = shp[0] if len(shp) == 2 else math.prod(shp[1:])
-                t = (torch.rand(shp, generator=g, device=dev) * 2 - 1) / fan_in ** 0.5
-            elif name.endswith(".weight"):
-                t = 1.0 + 0.1 * torch.randn(shp, generator=g, device=dev)
-            else:
-                t = 0.05 * torch.randn(shp, generator=g, device=dev)
-            P[name] = t.to(bf16)
-        return self.load_state_dict(P, device=device)
+        def special(name, shp, randn):
+            return 0.5 * randn(shp) if name == "model.embed_tokens.weight" else None
+        return self.load_state_dict(synthetic_state_dict(self.state_dict_shapes(), seed, device, special), device)
 
     def load_state_dict(self, P: Dict[str, Any], device: Union[int, str] = 0):
-        from .. import ops
-        dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
-        ops.init(dev.index or 0)
-        self.device = dev
-        missing = [k for k in self.state_dict_shapes() if k not in P]
-        if missing:
-            raise KeyError(f"state dict is missing {len(missing)} parameters, e.g. {missing[:3]}")
+        dev = bind(self, P, device)
         v = self.config.vision
         E, nh = v["embed_dim"], v["num_heads"]
         d, dp = self.v_head, self.v_pad
 
-        def W(name):
-            return _to_t(P[name + ".weight"]).t().contiguous()
-
-        def Bv(name):
-            return _to_t(P[name + ".bias"])
-
-        def dv(t, dtype=None):
-            return t.contiguous().to(dev, dtype) if dtype is not None else t.contiguous().to(dev)
-
-        self.w_patch = dv(_to_t(P["visual.patch_embed.proj.weight"]).reshape(E, -1), bf16)
+        self.w_patch = to_f32(P["visual.patch_embed.proj.weight"]).reshape(E, -1).contiguous().to(dev, bf16)
         self.vblocks = []
         for i in range(v["depth"]):
             b = f"visual.blocks.{i}"
-            wqkv, bqkv = W(b + ".attn.qkv"), Bv(b + ".attn.qkv")  # [3E, E] rows ordered (3, heads, d)
-            wq = torch.cat([_pad_rows(wqkv[j * E:(j + 1) * E], nh, d, dp) for j in range(3)], 0)
-            bq = torch.cat([_pad_vec(bqkv[j * E:(j + 1) * E], nh, d, dp) for j in range(3)], 0)
-            wp = W(b + ".attn.proj")  # [E, heads*d] -> [E, heads*dp]
-            if d != dp:
-                wp3 = torch.zeros(E, nh, dp, device=wp.device)
-                wp3[:, :, :d] = wp.reshape(E, nh, d)
-                wp = wp3.reshape(E, nh * dp)
+            # q|k|v rows are (3, heads, d): padded as 3 * heads heads
+            wqkv = pad_head_rows(linear_weight(P, b + ".attn.qkv"), 3 * nh, d, dp)
+            bqkv = pad_head_vec(linear_bias(P, b + ".attn.qkv"), 3 * nh, d, dp)
+            wp = pad_head_cols(linear_weight(P, b + ".attn.proj"), nh, d, dp)  # [E, heads*dp]
             self.vblocks.append(dict(
-                n1=(dv(_to_t(P[b + ".norm1.weight"])), dv(Bv(b + ".norm1"))), n2=(dv(_to_t(P[b + ".norm2.weight"])), dv(Bv(b + ".norm2"))),
-                qkv=(dv(wq, bf16), dv(bq)), proj=(dv(wp, bf16), dv(Bv(b + ".attn.proj"))),
-                fc1=(dv(W(b + ".mlp.fc1"), bf16), dv(Bv(b + ".mlp.fc1"))), fc2=(dv(W(b + ".mlp.fc2"), bf16), dv(Bv(b + ".mlp.fc2")))))
-        self.merger = dict(ln=(dv(_to_t(P["visual.merger.ln_q.weight"])), dv(Bv("visual.merger.ln_q"))),
-                           m0=(dv(W("visual.merger.mlp.0"), bf16), dv(Bv("visual.merger.mlp.0"))),
-                           m2=(dv(W("visual.merger.mlp.2"), bf16), dv(Bv("visual.merger.mlp.2"))))
+                n1=(device_vector(P, b + ".norm1.weight", dev), device_vector(P, b + ".norm1.bias", dev)),
+                n2=(device_vector(P, b + ".norm2.weight", dev), device_vector(P, b + ".norm2.bias", dev)),
+                qkv=(wqkv.to(dev, bf16), bqkv.to(dev)),
+                proj=(wp.to(dev, bf16), device_vector(P, b + ".attn.proj.bias", dev)),
+                fc1=device_linear(P, b + ".mlp.fc1", dev), fc2=device_linear(P, b + ".mlp.fc2", dev)))
+        self.merger = dict(ln=(device_vector(P, "visual.merger.ln_q.weight", dev),
+                               device_vector(P, "visual.merger.ln_q.bias", dev)),
+                           m0=device_linear(P, "visual.merger.mlp.0", dev), m2=device_linear(P, "visual.merger.mlp.2", dev))
         self.decoder.load_state_dict(P, dev)
         return self
 
