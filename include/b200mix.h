@@ -119,6 +119,30 @@ int b200mix_linear_batched(const void* A, int64_t lda, int64_t a_bstride, const 
                            int64_t ldc, int64_t c_bstride, int64_t rows, int64_t nbatch, int64_t N, int64_t K,
                            const b200mix_epilogue* epi, int64_t r_bstride, void* stream);
 
+/* ---- weight-only int8 Linear (PaddleNLP quant_type="weight_only_int8": paddle.nn.quant.weight_quantize +
+ * weight_only_linear; PaddleMIX triton_ops.py:363-563 weight_only_int8) ----------------------------------------------
+ * b200mix_quantize_w8: W fp32 (w_is_fp32 = 1) or bf16 [N, K] row-major -> q int8 (N * K bytes, 16-byte aligned) and
+ * scale fp32 [N]. Per row n: scale[n] = max_k |W[n,k]| / 127.0f and q[n,k] = clip(roundf(W[n,k] / scale[n]), -127, 127),
+ * both IEEE fp32 divisions, roundf rounding half away from zero (paddle.round). A row that is all zero gets scale 0 and
+ * q 0 (deliberately not 0 / 0 = NaN). Requires N % 16 == 0 and K % 64 == 0.
+ * q is written in the device layout the GEMM reads, and this function is its only producer:
+ *   q = [N / 16][K / 32][32 lanes][16 bytes]; byte 8 s + 2 r + e of lane l = 4 g + t holds element
+ *   (row 16 tile + g + 8 (r & 1), k 32 blk + 16 s + 2 t + 8 (r >> 1) + e), s, e in {0, 1}, r in 0..3
+ * (the A-operand fragments of two mma.m16n8k16 steps: one coalesced 512-byte load per warp and 16 x 32 block).
+ *
+ * b200mix_linear_w8: C[M, N(/2 if glu)] = epilogue(scale[n] * sum_k A[m,k] * q[n,k]); the scale multiplies the fp32
+ * accumulator before the bias. A bf16 (16-byte aligned, lda % 8 == 0), q / scale from b200mix_quantize_w8.
+ * Epilogue fields: bias, act, glu (interleaved rows as b200mix_linear), residual, out_fp32; any other field set returns
+ * B200MIX_ERR_UNSUPPORTED. Requires N % 16 == 0 and K % 64 == 0 (B200MIX_ERR_INVALID otherwise).
+ * Small M (decode) streams q through tensor cores; larger M expands bf16(q * scale) into `workspace` and runs
+ * b200mix_linear. The workspace (16-byte aligned) must hold b200mix_linear_w8_workspace_size bytes; it is 0 for small M,
+ * where workspace may be NULL. No allocation and no host synchronisation: CUDA-graph capturable. */
+int b200mix_quantize_w8(const void* W, int32_t w_is_fp32, void* q, float* scale, int64_t N, int64_t K, void* stream);
+int b200mix_linear_w8_workspace_size(int64_t M, int64_t N, int64_t K, int64_t* bytes);
+int b200mix_linear_w8(const void* A, int64_t lda, const void* q, const float* scale, void* C, int64_t ldc, int64_t M,
+                      int64_t N, int64_t K, const b200mix_epilogue* epi, void* workspace, int64_t workspace_bytes,
+                      void* stream);
+
 /* y[B,Ho,Wo,Cout] = epilogue(conv3x3(x[B,H,W,Cin], w[Cout,3,3,Cin], padding 1, stride 1|2)). Implicit GEMM without
  * im2col: each of the 9 taps is a shifted TMA box load with hardware zero fill at the borders.
  * Replaces F.conv2d in ResnetBlock2D / Downsample2D / Upsample2D / conv_out (resnet.py:271-294,169-218,728-808).

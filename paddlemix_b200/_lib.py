@@ -63,6 +63,10 @@ SIGNATURES = {
     "b200mix_comm_destroy": [c_void_p],
     "b200mix_linear": [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_int64,
                        POINTER(Epilogue), c_void_p],
+    "b200mix_quantize_w8": [c_void_p, c_int32, c_void_p, c_void_p, c_int64, c_int64, c_void_p],
+    "b200mix_linear_w8_workspace_size": [c_int64, c_int64, c_int64, POINTER(c_int64)],
+    "b200mix_linear_w8": [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64,
+                          POINTER(Epilogue), c_void_p, c_int64, c_void_p],
     "b200mix_linear_batched": [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_int64,
                                c_int64, c_int64, POINTER(Epilogue), c_int64, c_void_p],
     "b200mix_patchify": [c_void_p, c_int32, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int32, c_void_p],

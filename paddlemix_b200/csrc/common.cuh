@@ -13,6 +13,10 @@ namespace b200 {
 void set_error(const char* fmt, ...);
 int ensure_device();  // 0 if an sm_90 device is current, else negative status (with message)
 int num_sms();
+// K split of the weight-streaming GEMMs (gemm.cu skinny_linear_kernel, linear_w8.cu): ctas_n CTAs along N, kcap = the K
+// elements one CTA stages in one pass, slots = CTAs resident on the machine. Returns the cluster size (<= 8) and the K
+// elements per cluster rank (a multiple of 256). b200mix_debug_skinny_splits forces the split of both.
+void skinny_split(int ctas_n, int K, int kcap, int slots, int* splits, int* kpart);
 
 #define B200_CHECK_ARG(cond, ...)                 \
   do {                                            \

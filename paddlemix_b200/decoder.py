@@ -5,6 +5,10 @@ Per layer: RMSNorm -> fused q|k|v GEMM (+bias) -> attention -> o_proj GEMM (+res
 SwiGLU epilogue (interleaved rows) -> down GEMM (+residual); then the final RMSNorm and the lm_head GEMM with fp32
 output. Only the attention differs between prefill() (RoPE in place, optional KV-cache fill, causal or masked flash
 attention) and decode() (one token per sequence, every position on the device: CUDA-graph capturable).
+
+config.quant_type = "weight_only_int8" (PaddleNLP's inference models, qwen/modeling.py:73-85,194-235) quantizes the four
+projection matrices of every layer to int8 with one scale per output row at load time; ops.linear takes them in place
+of the bf16 weights, so the layer loop is the same. The embedding, lm_head, norms and biases stay as they are.
 """
 from typing import Dict
 
@@ -27,11 +31,17 @@ def rope_cos_sin(theta: float, head_dim: int, n_positions: int):
 class CausalDecoder:
     """Embedding table, decoder layers, final norm and lm_head. Parameters are `{prefix}.embed_tokens`,
     `{prefix}.layers.{i}.*`, `{prefix}.norm` and `lm_head` in the Paddle Linear layout ([in, out]); on the device q|k|v
-    rows are fused, up / gate rows interleaved, GEMM weights bf16 [N, K], norm weights and biases fp32."""
+    rows are fused, up / gate rows interleaved, GEMM weights bf16 [N, K] (the layers' four matrices ops.Int8Weight with
+    config.quant_type = "weight_only_int8"), norm weights and biases fp32."""
+
+    QUANT_TYPES = (None, "weight_only_int8")
 
     def __init__(self, config, prefix: str, qkv_bias: bool):
         self.config, self.prefix, self.qkv_bias = config, prefix, qkv_bias
         self.head_dim = config.hidden_size // config.num_attention_heads
+        self.quant_type = config.get("quant_type")
+        if self.quant_type not in self.QUANT_TYPES:
+            raise ValueError(f"quant_type must be one of {self.QUANT_TYPES}, got {self.quant_type!r}")
 
     def state_dict_shapes(self) -> Dict[str, tuple]:
         c, p = self.config, self.prefix
@@ -53,8 +63,17 @@ class CausalDecoder:
         return S
 
     def load_state_dict(self, P: Dict[str, object], dev: torch.device):
+        from . import ops
         c, p = self.config, self.prefix
         self.embed = to_f32(P[f"{p}.embed_tokens.weight"]).contiguous().to(dev, bf16)
+        if self.quant_type == "weight_only_int8":
+            # quantized after fusing (the scales are per output row) from the fp32 values; one bf16 workspace, as large
+            # as the largest of the four matrices, serves every layer's GEMMs above the weight-streaming range
+            H, I, kv = c.hidden_size, c.intermediate_size, c.num_key_value_heads * self.head_dim
+            ws = torch.empty(max((H + 2 * kv) * H, H * H, 2 * I * H, H * I), device=dev, dtype=bf16)
+            weight = lambda w: ops.quantize_w8(w.to(dev), ws)  # noqa: E731
+        else:
+            weight = lambda w: w.to(dev, bf16)  # noqa: E731
         self.layers = []
         for i in range(c.num_hidden_layers):
             b = f"{p}.layers.{i}"
@@ -64,10 +83,10 @@ class CausalDecoder:
             self.layers.append(dict(
                 ln1=device_vector(P, b + ".input_layernorm.weight", dev),
                 ln2=device_vector(P, b + ".post_attention_layernorm.weight", dev),
-                qkv=torch.cat([linear_weight(P, n) for n in qkv], 0).to(dev, bf16),
+                qkv=weight(torch.cat([linear_weight(P, n) for n in qkv], 0)),
                 qkv_bias=torch.cat([linear_bias(P, n) for n in qkv], 0).to(dev) if self.qkv_bias else None,
-                o=linear_weight(P, b + ".self_attn.o_proj").to(dev, bf16), gu=gu.to(dev, bf16),
-                down=linear_weight(P, b + ".mlp.down_proj").to(dev, bf16)))
+                o=weight(linear_weight(P, b + ".self_attn.o_proj")), gu=weight(gu),
+                down=weight(linear_weight(P, b + ".mlp.down_proj"))))
         self.norm_w = device_vector(P, f"{p}.norm.weight", dev)
         self.lm_head = linear_weight(P, "lm_head").to(dev, bf16)
         return self

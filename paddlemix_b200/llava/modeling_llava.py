@@ -28,7 +28,7 @@ class LlamaForCausalLM:
 
     def __init__(self, config: Union[Dict[str, Any], Any] = None, **kw):
         cfg = dict(vocab_size=32000, hidden_size=4096, intermediate_size=11008, num_hidden_layers=32, num_attention_heads=32,
-                   num_key_value_heads=32, rms_norm_eps=1e-5, rope_theta=10000.0)
+                   num_key_value_heads=32, rms_norm_eps=1e-5, rope_theta=10000.0, quant_type=None)
         cfg.update(dict(config or {}))
         cfg.update(kw)
         self.config = FrozenDict(cfg)

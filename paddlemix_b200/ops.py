@@ -160,13 +160,79 @@ def _epi_tag(e) -> str:
     return (" " + "+".join(parts)) if parts else ""
 
 
-def linear(a: torch.Tensor, w: torch.Tensor, bias=None, *, act=ACT_NONE, glu=GLU_NONE, residual=None, row_add=None,
+class Int8Weight:
+    """A Linear weight [N, K] quantized to int8 with one fp32 scale per output row (quantize_w8). q holds the N * K
+    bytes in the device layout of b200mix_quantize_w8 (only the kernels read it); workspace is the bf16 buffer linear()
+    expands the weight into when M is above the weight-streaming range, shared by every weight of a model (None: such
+    calls are refused)."""
+    __slots__ = ("q", "scale", "N", "K", "workspace")
+
+    def __init__(self, q: torch.Tensor, scale: torch.Tensor, N: int, K: int, workspace: Optional[torch.Tensor]):
+        self.q, self.scale, self.N, self.K, self.workspace = q, scale, N, K, workspace
+
+
+def quantize_w8(w: torch.Tensor, workspace: Optional[torch.Tensor]) -> Int8Weight:
+    """Weight-only int8 of w fp32 or bf16 [N, K] on the device (N % 16 == 0, K % 64 == 0): per row scale = absmax / 127,
+    q = clip(round(w / scale), -127, 127), rounding half away from zero; an all-zero row gets scale 0. workspace: bf16
+    with at least N * K elements, or None."""
+    if w.dtype not in (torch.float32, bf16):
+        raise TypeError(f"quantize_w8 takes an fp32 or bf16 weight, got {w.dtype}")
+    _req(w, w.dtype, "w")
+    if w.dim() != 2:
+        raise ValueError(f"quantize_w8 takes a [N, K] weight, got {tuple(w.shape)}")
+    N, K = w.shape
+    if workspace is not None and (_req(workspace, bf16, "workspace").numel() < N * K):
+        raise ValueError(f"the workspace holds {workspace.numel()} bf16 elements, a [{N}, {K}] weight needs {N * K}")
+    w = w.contiguous()
+    q = torch.empty(N * K, device=w.device, dtype=torch.int8)
+    scale = torch.empty(N, device=w.device, dtype=torch.float32)
+    check(lib.b200mix_quantize_w8(_p(w), 1 if w.dtype == torch.float32 else 0, _p(q), _p(scale), N, K, _stream()),
+          "b200mix_quantize_w8")
+    _count()
+    return Int8Weight(q, scale, N, K, workspace)
+
+
+def _linear_w8(a, w: Int8Weight, bias, act, glu, residual, out_fp32, out):
+    _req(a, bf16, "a")
+    K = a.shape[-1]
+    if K != w.K:
+        raise ValueError(f"input has {K} features, the weight takes {w.K}")
+    a2 = a.reshape(-1, K)
+    if a2.stride(-1) != 1 or a2.data_ptr() % 16 or a2.stride(0) % 8:
+        a2 = a2.contiguous()
+    M, N = a2.shape[0], w.N
+    n_out = N // 2 if glu else N
+    if out is None:
+        out = torch.empty(*a.shape[:-1], n_out, device=a.device, dtype=torch.float32 if out_fp32 else bf16)
+    res2 = None if residual is None else residual.reshape(-1, residual.shape[-1])
+    e = make_epilogue(bias=bias, residual=res2, ldr=0 if res2 is None else res2.stride(0), act=act, glu=glu,
+                      out_fp32=out_fp32)
+    out2 = out.reshape(-1, n_out)
+    ws = w.workspace
+    with _Timed("w8gemm", 2.0 * M * N * K, "flop", lambda: f"w8 {M}x{N}x{K}" + _epi_tag(e)):
+        check(lib.b200mix_linear_w8(_p(a2), a2.stride(0), _p(w.q), _p(w.scale), _p(out2), out2.stride(0), M, N, K,
+                                    ctypes.byref(e), _p(ws), 0 if ws is None else 2 * ws.numel(), _stream()),
+              "b200mix_linear_w8")
+    _count()
+    return out
+
+
+def linear(a: torch.Tensor, w, bias=None, *, act=ACT_NONE, glu=GLU_NONE, residual=None, row_add=None,
            row_gate=None, rows_per_group=0, out_fp32=False, out=None, out_scale=1.0, residual_row_mod=0, stats=False,
            ln=None):
-    """out[M, N(/2)] = epilogue(a[M, K] @ w[N, K]^T). a: bf16 [..., K] (last dim contiguous), w: bf16 [N, K].
+    """out[M, N(/2)] = epilogue(a[M, K] @ w[N, K]^T). a: bf16 [..., K] (last dim contiguous), w: bf16 [N, K] or an
+    Int8Weight (then only bias / act / glu / residual / out_fp32 / out apply).
     stats=True or a ZEROED int64 [M, 2] tensor (RowStats.arena): also returns the RowStats of the output rows
     (-> (out, RowStats)); ln=(RowStats of a's rows, colsum, eps[, rms]): a is the UN-normalised tensor and w / bias carry
     the folded affine (fold_layernorm_into_linear)."""
+    if isinstance(w, Int8Weight):
+        unsupported = [n for n, on in (("row_add", row_add is not None), ("row_gate", row_gate is not None),
+                                       ("rows_per_group", rows_per_group), ("out_scale", out_scale != 1.0),
+                                       ("residual_row_mod", residual_row_mod), ("stats", stats is not None and stats is not False),
+                                       ("ln", ln is not None)) if on]
+        if unsupported:
+            raise ValueError(f"an Int8Weight linear does not support {', '.join(unsupported)}")
+        return _linear_w8(a, w, bias, act, glu, residual, out_fp32, out)
     _req(a, bf16, "a"), _req(w, bf16, "w")
     K = a.shape[-1]
     a2 = a.reshape(-1, K)

@@ -33,7 +33,7 @@ class Qwen2VLConfig(FrozenDict):
                  num_key_value_heads=4, vocab_size=152064, rms_norm_eps=1e-6, rope_theta=1000000.0,
                  mrope_section=(16, 24, 24), image_token_id=151655, video_token_id=151656,
                  vision_start_token_id=151652, vision_end_token_id=151653, vision=None, tie_word_embeddings=False,
-                 **kw):
+                 quant_type=None, **kw):
         vision = dict(depth=32, embed_dim=1280, num_heads=16, mlp_ratio=4, in_channels=3, patch_size=14,
                       temporal_patch_size=2, spatial_merge_size=2, hidden_act="quick_gelu") if vision is None else dict(vision)
         super().__init__(hidden_size=hidden_size, intermediate_size=intermediate_size,
@@ -42,7 +42,7 @@ class Qwen2VLConfig(FrozenDict):
                          rope_theta=rope_theta, mrope_section=tuple(mrope_section), image_token_id=image_token_id,
                          video_token_id=video_token_id, vision_start_token_id=vision_start_token_id,
                          vision_end_token_id=vision_end_token_id, vision=FrozenDict(vision),
-                         tie_word_embeddings=bool(tie_word_embeddings))
+                         tie_word_embeddings=bool(tie_word_embeddings), quant_type=quant_type)
 
 
 @dataclass
