@@ -153,6 +153,19 @@ struct IGemmCfg {
 constexpr int IG_THREADS = 384;
 constexpr int IG_PRODUCER_REGS = 40, IG_CONSUMER_REGS = 232;
 
+// Cycle-accounting build (compiled with -DIGEMM_CYCLES, off in the shipped library; tools/igemm_cycles.py builds and
+// reads it): per CTA and consumer warpgroup, clock64() totals of the wait on full_bar, the k-loop (those waits included)
+// and the epilogue (the stream-K exchange included), plus the pieces and k-blocks run, summed over launches until read
+// with b200mix_debug_igemm_cycles.
+#ifdef IGEMM_CYCLES
+#define IG_CYC(...) __VA_ARGS__
+enum { CYC_WAIT = 0, CYC_KLOOP = 1, CYC_EPI = 2, CYC_PIECES = 3, CYC_KBLOCKS = 4, CYC_FIELDS = 5 };
+constexpr int CYC_SLOTS = 1024;  // CTA * 2 + consumer warpgroup
+__device__ unsigned long long g_igemm_cycles[CYC_SLOTS][CYC_FIELDS];
+#else
+#define IG_CYC(...)
+#endif
+
 // Epilogue families (see the dispatch in the kernel): bias / residual / statistics only, GLU, everything else on the
 // row-wise path, and the element-wise path (fp32 output, rows that are not whole 16-byte pieces).
 enum { EPI_PLAIN = 0, EPI_GLU = 1, EPI_GENERAL = 2, EPI_DIRECT = 3 };
@@ -221,9 +234,9 @@ __global__ void __launch_bounds__(IG_THREADS, 1)
         for (int kb = seg.kb0; kb < seg.kb1; ++kb) {
           const int tg = tap_base + tap;
           const int dc = p.tap_dc[tg], dx = p.tap_dx[tg], pp = p.tap_p[tg], dy = p.tap_dy[tg];
-          // MCAST: the peer CTA's consumers release this stage too (remote arrivals)
-          if (MCAST) mbar_wait_cluster(&empty_bar[stage], phase ^ 1);
-          else mbar_wait(&empty_bar[stage], phase ^ 1);
+          // MCAST: the peer CTA's consumers release this stage too (remote arrivals). A plain wait: the TMA writes that
+          // follow need no acquire (see mbar_arrive_remote_stage)
+          mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
           uint8_t* sB = sA + Cfg::A_BYTES;
           if (elect_one_sync()) {
@@ -270,15 +283,21 @@ __global__ void __launch_bounds__(IG_THREADS, 1)
     auto release = [&](int s) {  // this warp's wgmma reads of stage s are complete
       if (lane == 0) {
         mbar_arrive(&empty_bar[s]);
-        if (MCAST) mbar_arrive_cluster(peer_empty + 8u * s);
+        if (MCAST) mbar_arrive_remote_stage(peer_empty + 8u * s);
       }
     };
+    IG_CYC(unsigned long long cyc[CYC_FIELDS] = {}; long long cyc_epi0 = -1;)
     for (SegIter seg(p.sk_tiles, total_super, kblocks, cluster_id, num_clusters); seg.next();) {
+      // the previous piece's epilogue ends where this piece's k-loop starts (the stream-K tail piece skips the epilogue)
+      IG_CYC(const long long cyc_k0 = clock64(); if (cyc_epi0 >= 0) cyc[CYC_EPI] += cyc_k0 - cyc_epi0;
+             cyc[CYC_PIECES] += 1, cyc[CYC_KBLOCKS] += seg.kb1 - seg.kb0;)
       float acc[BN / 2];
       {
         int prev = -1;
         for (int kb = seg.kb0; kb < seg.kb1; ++kb) {
+          IG_CYC(const long long cyc_w0 = clock64();)
           mbar_wait(&full_bar[kstage], kphase);
+          IG_CYC(cyc[CYC_WAIT] += clock64() - cyc_w0;)
           const uint32_t a_addr = smem_u32(smem + kstage * Cfg::STAGE_BYTES) + grp * 64 * 128;
           const uint32_t b_addr = smem_u32(smem + kstage * Cfg::STAGE_BYTES + Cfg::A_BYTES);
           wgmma_fence();
@@ -297,6 +316,7 @@ __global__ void __launch_bounds__(IG_THREADS, 1)
         wgmma_fence_operands(acc);
         release(prev);
       }
+      IG_CYC(cyc_epi0 = clock64(); cyc[CYC_KLOOP] += cyc_epi0 - cyc_k0;)
 
       const int st = seg.st;
       const int seg_mode = seg.mode();
@@ -566,6 +586,10 @@ __global__ void __launch_bounds__(IG_THREADS, 1)
         }
       }
     }
+    IG_CYC(if (cyc_epi0 >= 0) cyc[CYC_EPI] += clock64() - cyc_epi0;
+           if ((ctid & 127) == 0 && blockIdx.x * 2 + grp < CYC_SLOTS) {
+             for (int f = 0; f < CYC_FIELDS; ++f) atomicAdd(&g_igemm_cycles[blockIdx.x * 2 + grp][f], cyc[f]);
+           })
   }
 
   __syncthreads();
@@ -1035,6 +1059,19 @@ extern "C" void b200mix_debug_max_clusters(int n) { b200::g_max_clusters = n; }
 extern "C" void b200mix_debug_skinny(int on) { b200::g_skinny = on; }
 extern "C" void b200mix_debug_streamk(int on) { b200::g_streamk = on; }
 extern "C" void b200mix_debug_skinny_splits(int splits) { b200::g_skinny_splits = splits; }
+#ifdef IGEMM_CYCLES
+// Cycle-accounting build only: copies the [1024][5] counters (see g_igemm_cycles) to `out`, then zeroes them if `reset`.
+extern "C" int b200mix_debug_igemm_cycles(unsigned long long* out, int reset) {
+  if (int rc = ensure_device()) return rc;
+  B200_CUDA(cudaDeviceSynchronize());
+  if (out) B200_CUDA(cudaMemcpyFromSymbol(out, b200::g_igemm_cycles, sizeof(b200::g_igemm_cycles)));
+  if (reset) {
+    static const unsigned long long zeros[b200::CYC_SLOTS][b200::CYC_FIELDS] = {};
+    B200_CUDA(cudaMemcpyToSymbol(b200::g_igemm_cycles, zeros, sizeof(zeros)));
+  }
+  return 0;
+}
+#endif
 
 extern "C" int b200mix_linear(const void* A, int64_t lda, const void* W, int64_t ldw, void* C, int64_t ldc, int64_t M,
                               int64_t N, int64_t K, const b200mix_epilogue* epi, void* stream) {

@@ -115,22 +115,13 @@ __device__ __forceinline__ uint32_t mapa_smem(const void* ptr, uint32_t rank) {
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(ptr)), "r"(rank));
   return r;
 }
-// arrive on an mbarrier that may live in another CTA of the cluster (address from mapa_smem)
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// wait with cluster-scope acquire: pairs with mbar_arrive_cluster from the peer CTA
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t ok = 0;
-  while (!ok) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-  }
+// Release a TMA ring stage on an mbarrier that may live in another CTA of the cluster (address from mapa_smem), with no
+// memory ordering beyond the arrive itself: the stage is written only by TMA and read only by wgmma, both async-proxy
+// accesses, and wgmma.wait_group has already completed this thread's reads of it. The .release.cluster form would make
+// ptxas put a GPU-scope MEMBAR (which also waits for every outstanding global store) in front of each arrive, on the
+// k-loop's critical path; the producer's plain mbar_wait is the matching side. Not for data written by generic stores.
+__device__ __forceinline__ void mbar_arrive_remote_stage(uint32_t cluster_addr) {
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
 
 // ----------------------------------------------------------------------------------------------

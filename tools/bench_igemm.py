@@ -11,10 +11,14 @@
     name, power limit and max SM clock read in the same run;
   * --other-lib PATH loads a second build of libb200mix.so and alternates the two per problem in the same process over
     --rounds rounds: median and min-max of each, which is how a kernel change is compared against its parent;
-  * --force-bn 128,64 also times the --top heaviest problems with the tile width forced (b200mix_debug_force_bn).
+  * --force-bn 128,64 also times the --top heaviest problems with the tile width forced (b200mix_debug_force_bn);
+  * --gemm-pair 0 runs every build without 2-CTA clusters (b200mix_debug_gemm_pair: each CTA loads its whole B tile,
+    no multicast and no cross-CTA release of ring stages), except the folded-LayerNorm problems, which exist only
+    clustered; the default 1 is the shipped schedule.
 Writes nothing to the tree unless --json PATH is given.
 
-    python tools/bench_igemm.py [--other-lib /path/to/libb200mix.so] [--rounds 3] [--force-bn 128,64] [--json out.json]
+    python tools/bench_igemm.py [--other-lib /path/to/libb200mix.so] [--rounds 3] [--force-bn 128,64] [--gemm-pair 0]
+                                [--json out.json]
 """
 import argparse
 import json
@@ -106,6 +110,8 @@ class Problem:
         self.M, self.N, self.K = int(m.group(2)), int(m.group(3)), int(m.group(4))
         self.flags = set((m.group(5) or "").split("+")) - {""}
         self.batch = batch
+        # the folded-LayerNorm epilogues exist only in the clustered (multicast) kernel
+        self.pair_only = bool(self.flags & {"ln", "stats"})
         self.act = next((ACTS[f] for f in self.flags if f in ACTS), 0)
         self.glu = next((int(f[3:]) for f in self.flags if f.startswith("glu")), 0)
         self.taps = {"lin": 1, "conv1": 9, "conv2": 9, "convup": 4}[self.kind]
@@ -173,13 +179,14 @@ class Problem:
                         residual=d["res"], act=self.act, out=d["out"])
 
 
-def time_us(prob, lib, min_seconds, force_bn=0):
+def time_us(prob, lib, min_seconds, force_bn=0, gemm_pair=1):
     """Mean us per launch of `prob` through build `lib`, over enough launches to fill min_seconds."""
     import torch
 
     from paddlemix_b200 import ops
     saved, ops.lib = ops.lib, lib
     lib.b200mix_debug_force_bn(force_bn)
+    lib.b200mix_debug_gemm_pair(1 if prob.pair_only else gemm_pair)
     try:
         def run(n):
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -193,6 +200,7 @@ def time_us(prob, lib, min_seconds, force_bn=0):
         return run(max(2 * len(prob.sets), math.ceil(min_seconds / per))) * 1e6
     finally:
         lib.b200mix_debug_force_bn(0)
+        lib.b200mix_debug_gemm_pair(1)
         ops.lib = saved
 
 
@@ -209,6 +217,8 @@ def main():
     ap.add_argument("--other-lib", default=None, help="a second build of libb200mix.so to alternate with the tree's")
     ap.add_argument("--force-bn", default="", help="comma-separated tile widths to force on the --top heaviest problems")
     ap.add_argument("--top", type=int, default=5)
+    ap.add_argument("--gemm-pair", type=int, default=1, choices=[0, 1],
+                    help="1: 2-CTA clusters sharing the B tile through multicast (default); 0: independent CTAs")
     ap.add_argument("--json", default=None, help="also write the result as JSON to this path")
     args = ap.parse_args()
 
@@ -222,7 +232,8 @@ def main():
         builds["other"] = load_lib(args.other_lib)
     sms = ops.lib.b200mix_num_sms()
     info = gpu_info()
-    print(json.dumps({"gpu": info, "sms": sms, "builds": {"tree": ops._lib.LIB_PATH, "other": args.other_lib}}), flush=True)
+    print(json.dumps({"gpu": info, "sms": sms, "gemm_pair": args.gemm_pair,
+                      "builds": {"tree": ops._lib.LIB_PATH, "other": args.other_lib}}), flush=True)
 
     rec = record_problems(args.batch, args.height)
     order = sorted(rec, key=lambda t: -rec[t]["flop"] * rec[t]["calls"])
@@ -238,7 +249,7 @@ def main():
         t = {name: [] for name in builds}
         for _ in range(args.rounds):
             for name, lib in builds.items():
-                t[name].append(time_us(prob, lib, args.min_seconds))
+                t[name].append(time_us(prob, lib, args.min_seconds, gemm_pair=args.gemm_pair))
         row = {"problem": tag, "calls": rec[tag]["calls"], "flop": prob.flop, "bn": bn, "tiles": tiles,
                "rounds": round(rounds, 2), "us": {n: spread(v) for n, v in t.items()}, "forced": {}}
         line = f"{tag:44s} {row['calls']:5d} {bn:4d} {tiles:6d} {rounds:6.2f}"
@@ -250,7 +261,7 @@ def main():
             for fbn in forced:
                 fb, ftiles, frounds = tile_schedule(prob.m_tiles, prob.N, prob.kblocks, sms, fbn)
                 for name, lib in builds.items():
-                    v = [time_us(prob, lib, args.min_seconds, fbn) for _ in range(args.rounds)]
+                    v = [time_us(prob, lib, args.min_seconds, fbn, args.gemm_pair) for _ in range(args.rounds)]
                     row["forced"].setdefault(str(fbn), {})[name] = spread(v)
                     s = spread(v)
                     print(f"    forced BN {fb:3d} ({name}): tiles {ftiles}, rounds {frounds:.2f}, {s['median']:.1f} us "
@@ -265,7 +276,7 @@ def main():
         ms = {k: sum(r["us"][name][k] * r["calls"] for r in rows) * 1e-3 for k in ("median", "min", "max")}
         totals[name] = {"igemm_ms_per_step": {k: round(v, 2) for k, v in ms.items()},
                         "tflops": round(total_flop / ms["median"] / 1e9, 1)}
-    out = {"gpu": info, "sms": sms, "batch": args.batch, "height": args.height, "rounds": args.rounds,
+    out = {"gpu": info, "sms": sms, "gemm_pair": args.gemm_pair, "batch": args.batch, "height": args.height, "rounds": args.rounds,
            "igemm_tflop_per_step": round(total_flop / 1e12, 3), "totals": totals, "problems": rows}
     print(json.dumps({k: out[k] for k in ("gpu", "igemm_tflop_per_step", "totals")}), flush=True)
     if args.json:
