@@ -28,6 +28,25 @@ def rope_cos_sin(theta: float, head_dim: int, n_positions: int):
     return emb.cos(), emb.sin()
 
 
+def decode_attention(qkv, cache_k, cache_v, heads: int, kv_heads: int, head_dim: int, kv_lens, key_bias=None, out=None):
+    """Attention of one token per sequence over its KV cache: qkv bf16 [B, (heads + 2 * kv_heads) * head_dim] row view
+    (q heads after RoPE), cache_k / cache_v bf16 [B, max_len, kv_heads, head_dim], kv_lens int32 [B] (keys [0, kv_len)
+    are read), key_bias fp32 [B, max_len] additive key mask or None. The G = heads / kv_heads query heads that share a
+    KV head are presented to the attention kernel as G query rows of ONE head (Sq = G, Hq = kv_heads): one K / V stream
+    per KV head instead of one per query head. Returns bf16 [B, heads * head_dim], written into `out` (a row view with a
+    contiguous last axis) when it is given."""
+    from . import ops
+    B, G, qd = qkv.shape[0], heads // kv_heads, heads * head_dim
+    kb = None if key_bias is None else key_bias[:, None, None, :]
+    if out is not None and (tuple(out.shape) != (B, qd) or out.stride(1) != 1):
+        raise ValueError(f"out must be a [{B}, {qd}] view with a contiguous last axis, got {tuple(out.shape)}")
+    a = torch.empty(B, qd, device=qkv.device, dtype=bf16) if out is None else out
+    qg = qkv.as_strided((B, G, kv_heads, head_dim), (qkv.stride(0), head_dim, G * head_dim, 1), qkv.storage_offset())
+    ag = a.as_strided((B, G, kv_heads, head_dim), (a.stride(0), head_dim, G * head_dim, 1), a.storage_offset())
+    ops.sdpa(qg, cache_k, cache_v, scale=head_dim ** -0.5, kv_lens=kv_lens, attn_mask=kb, out=ag)
+    return a
+
+
 class CausalDecoder:
     """Embedding table, decoder layers, final norm and lm_head. Parameters are `{prefix}.embed_tokens`,
     `{prefix}.layers.{i}.*`, `{prefix}.norm` and `lm_head` in the Paddle Linear layout ([in, out]); on the device q|k|v
@@ -136,21 +155,14 @@ class CausalDecoder:
     def decode(self, ids, cos, sin, cache, rows, kv_lens):
         """One token per sequence against `cache`: ids int64 [B], cos / sin fp32 [B, head_dim] for its position, rows
         int64 [B] = b * max_len + position (the flattened cache row its K / V go to), kv_lens int32 [B] = position + 1,
-        all on the device. The G = heads / kv_heads query heads that share a KV head are presented to the attention
-        kernel as G query rows of ONE head (Sq = G, Hq = Hkv): one K / V stream per KV head instead of one per query
-        head. Returns fp32 logits [B, vocab]; advancing cache.length is the caller's job."""
+        all on the device. Attention is decode_attention() over the cache. Returns fp32 logits [B, vocab]; advancing
+        cache.length is the caller's job."""
         from . import ops
         c, hd = self.config, self.head_dim
         nh, nkv = c.num_attention_heads, c.num_key_value_heads
-        G, qd, kvd = nh // nkv, nh * hd, nkv * hd
-        B = ids.shape[0]
-        kb = None if cache.key_bias is None else cache.key_bias[:, None, None, :]
+        kvd = nkv * hd
 
         def attention(li, qkv):
             ops.decode_rope_cache(qkv, nh, nkv, hd, cos, sin, rows, cache.k[li].view(-1, kvd), cache.v[li].view(-1, kvd))
-            a = torch.empty(B, qd, device=qkv.device, dtype=bf16)
-            qg = qkv.as_strided((B, G, nkv, hd), (qkv.stride(0), hd, G * hd, 1), qkv.storage_offset())
-            ag = a.as_strided((B, G, nkv, hd), (qd, hd, G * hd, 1))
-            ops.sdpa(qg, cache.k[li], cache.v[li], scale=hd ** -0.5, kv_lens=kv_lens, attn_mask=kb, out=ag)
-            return a
+            return decode_attention(qkv, cache.k[li], cache.v[li], nh, nkv, hd, kv_lens, cache.key_bias)
         return self._layers(ops.gather_rows(self.embed, ids), attention)
