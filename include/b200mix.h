@@ -337,7 +337,8 @@ int b200mix_head_rmsnorm_inplace(void* x, int64_t rows, int64_t H, int64_t d, in
                                  const float* weight, float eps, void* stream);
 /* Temporal self-attention of STDiT2Block (stdit2.py:160-171; Attention.forward, blocks.py:200-241): sequences of
  * length T <= 32 along the frame axis of the token-major qkv buffer [B, T, S, 3, H, d] (row = (b*T+t)*S+s), with
- * interleaved-pair RoPE (cos/sin fp32 [T, d/2], blocks.py:566-591) and optional q/k RMSNorm, out [B, T, S, H*d]. */
+ * interleaved-pair RoPE (cos/sin fp32 [T, d/2], blocks.py:566-591) and optional q/k RMSNorm, out [B, T, S, H*d].
+ * Even d <= 128; row strides ld_row >= 3*H*d and ld_out >= H*d, both even, on 4-byte aligned buffers. */
 int b200mix_small_attention(const void* qkv, void* out, int64_t B, int64_t T, int64_t S, int64_t H, int64_t d,
                             int64_t ld_row, int64_t ld_out, const float* rope_cos, const float* rope_sin,
                             const float* q_norm_w, const float* k_norm_w, float eps, float scale, void* stream);

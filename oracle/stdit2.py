@@ -179,8 +179,11 @@ def stdit2_block(x, y, t_mlp, t_tmp_mlp, y_lens, P, p, cfg, T, S):
     return x + gate_mlp * x_mlp
 
 
-def stdit2_forward(cfg, P: Params, x, timestep, y, mask=None, num_frames=None, height=None, width=None, ar=None, fps=None):
-    """STDiT2.forward, stdit2.py:334-448. x [B,C,T,H,W]; y [B,1,L,caption]; mask [B,L] or None; returns fp32."""
+def stdit2_conditioning(cfg, P: Params, x, timestep, y, mask=None, num_frames=None, height=None, width=None, ar=None,
+                        fps=None):
+    """STDiT2.forward up to the first block, stdit2.py:338-394: returns dict(h = patch + position embedding [B, T*S, D],
+    t, t_mlp [B, 6D], t_tmp_mlp [B, 3D], ye [B, 1, L, D] (before packing), y_packed [1, sum(y_lens), D], y_lens, T, H,
+    W)."""
     B = x.shape[0]
     D = cfg["hidden_size"]
     pt, ph, pw = cfg["patch_size"]
@@ -202,12 +205,24 @@ def stdit2_forward(cfg, P: Params, x, timestep, y, mask=None, num_frames=None, h
     ye = linear(F.gelu(linear(y, P, "y_embedder.y_proj.fc1"), approximate="tanh"), P, "y_embedder.y_proj.fc2")
     if mask is not None:
         y_lens = mask.sum(dim=1).tolist()
-        ye = ye.squeeze(1)[mask != 0].reshape(1, -1, D)
+        y_packed = ye.squeeze(1)[mask != 0].reshape(1, -1, D)
     else:
         y_lens = [ye.shape[2]] * B
-        ye = ye.squeeze(1).reshape(1, -1, D)
+        y_packed = ye.squeeze(1).reshape(1, -1, D)
+    return dict(h=h, t=t, t_mlp=t_mlp, t_tmp_mlp=t_tmp_mlp, ye=ye, y_packed=y_packed, y_lens=y_lens, T=T, H=H, W=W)
+
+
+def stdit2_forward(cfg, P: Params, x, timestep, y, mask=None, num_frames=None, height=None, width=None, ar=None, fps=None):
+    """STDiT2.forward, stdit2.py:334-448. x [B,C,T,H,W]; y [B,1,L,caption]; mask [B,L] or None; returns fp32."""
+    B = x.shape[0]
+    D = cfg["hidden_size"]
+    pt, ph, pw = cfg["patch_size"]
+    _, _, Tx, Hx, Wx = x.shape
+    c = stdit2_conditioning(cfg, P, x, timestep, y, mask, num_frames, height, width, ar, fps)
+    T, H, W, t, h = c["T"], c["H"], c["W"], c["t"], c["h"]
+    y, y_lens = c["y_packed"], c["y_lens"]
     for i in range(cfg["depth"]):
-        h = stdit2_block(h, ye, t_mlp, t_tmp_mlp, y_lens, P, f"blocks.{i}", cfg, T, S)
+        h = stdit2_block(h, y, c["t_mlp"], c["t_tmp_mlp"], y_lens, P, f"blocks.{i}", cfg, T, H * W)
     shift, scale = (P["final_layer.scale_shift_table"][None] + t[:, None]).chunk(2, dim=1)  # T2IFinalLayer :376-385
     h = linear(F.layer_norm(h, (D,), None, None, 1e-6) * (1 + scale) + shift, P, "final_layer.linear")
     oc = cfg["in_channels"] * (2 if cfg["pred_sigma"] else 1)

@@ -1029,9 +1029,20 @@ extern "C" int b200mix_small_attention(const void* qkv, void* out, int64_t B, in
   B200_CHECK_ARG(T > 0 && T <= 32 && d > 0 && d <= 128 && d % 2 == 0, "small_attention: T <= 32, even d <= 128");
   B200_CHECK_ARG((rope_cos == nullptr) == (rope_sin == nullptr) && (q_norm_w == nullptr) == (k_norm_w == nullptr),
                  "small_attention: rope / norm tables come in pairs");
+  // the kernel reads and writes (even column) bf16 pairs
+  B200_CHECK_ARG(ld_row % 2 == 0 && ld_out % 2 == 0 && ld_row >= 3 * H * d && ld_out >= H * d &&
+                     reinterpret_cast<uintptr_t>(qkv) % 4 == 0 && reinterpret_cast<uintptr_t>(out) % 4 == 0,
+                 "small_attention: rows must be 4-byte aligned, ld_row >= 3*H*d, ld_out >= H*d");
   const size_t smem = (size_t)(3 * T * d + T * T) * sizeof(float);
   const long long ctas = B * S * H;
   B200_CHECK_ARG(ctas < (1ll << 31), "small_attention: too many sequences");
+  // T = 32, d = 128 needs 52 KB, above the 48 KB available without opting in
+  constexpr int kMaxSmem = (3 * 32 * 128 + 32 * 32) * sizeof(float);
+  static bool configured = false;
+  if (!configured) {
+    B200_CUDA(cudaFuncSetAttribute(small_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
+    configured = true;
+  }
   small_attention_kernel<<<(unsigned)ctas, 128, smem, ST(stream)>>>(
       reinterpret_cast<const __nv_bfloat16*>(qkv), reinterpret_cast<__nv_bfloat16*>(out), (int)T, (int)S, (int)H, (int)d,
       ld_row, ld_out, rope_cos, rope_sin, q_norm_w, k_norm_w, eps, scale);

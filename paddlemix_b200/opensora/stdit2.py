@@ -11,7 +11,7 @@ Device graph per block (tokens are [B, T*S, D] with row = (b*T + t)*S + s, never
   The 28 x (6+3) modulation vectors come from two GEMMs and one table-broadcast kernel per forward; all 28 cross-attn
   k|v projections of the text are one GEMM per forward.
 """
-from typing import Any, Dict, Union
+from typing import Any, Dict, NamedTuple, Optional, Union
 
 import torch
 
@@ -19,6 +19,26 @@ from ..modeling import (FrozenDict, bind, device_linear, device_vector, linear_b
                         pad_head_rows, pad_head_vec, pad_head_width, synthetic_state_dict, to_f32)
 
 bf16 = torch.bfloat16
+
+
+class _Conditioning(NamedTuple):
+    """What STDiT2._conditioning hands to every block: h bf16 [B, T*H*W, D] (patch + position embedding), mod_s /
+    mod_t fp32 [B, depth, 6D / 3D] and mod_f fp32 [B, 2D] (modulation table + timestep terms), ye bf16 [B, L, D]
+    (caption embedding), kv_all bf16 [B, L, depth*2*H*dp] (every block's cross-attention k|v), kv_lens int32 [B] or
+    None (valid caption tokens), rope_cos / rope_sin fp32 [T, head_dim/2]; B, T and the patch grid H x W."""
+    h: torch.Tensor
+    mod_s: torch.Tensor
+    mod_t: torch.Tensor
+    mod_f: torch.Tensor
+    ye: torch.Tensor
+    kv_all: torch.Tensor
+    kv_lens: Optional[torch.Tensor]
+    rope_cos: torch.Tensor
+    rope_sin: torch.Tensor
+    B: int
+    T: int
+    H: int
+    W: int
 
 
 class STDiT2Config(FrozenDict):
@@ -157,16 +177,15 @@ class STDiT2:
             self._pos_cache[key] = t
         return t
 
-    def forward(self, x, timestep, y, mask=None, x_mask=None, num_frames=None, height=None, width=None, ar=None, fps=None):
-        """Same signature as the reference (stdit2.py:334-336). x [B,C,T,H,W]; y [B,1,L,caption]; returns fp32."""
+    def _conditioning(self, x, timestep, y, mask=None, num_frames=None, height=None, width=None, ar=None, fps=None):
+        """Everything the blocks read (stdit2.py:338-394): the patch + position embedding h, the per-sample modulation
+        tables, the caption embedding and all blocks' cross-attention K/V, and the temporal RoPE tables."""
         from .. import ops
         from .._lib import ACT_GELU_TANH, ACT_SILU
         if self.device is None:
             raise RuntimeError("load_state_dict() must be called before forward()")
-        if x_mask is not None:
-            raise NotImplementedError("x_mask (frame masking) is outside the hot path")
         c, dev, D = self.config, self.device, self.config.hidden_size
-        Hh, hd, dp = c.num_heads, self.head_dim, self.head_pad
+        hd = self.head_dim
         ps = c.patch_size[1]
         x = x.to(dev)
         if x.dtype not in (torch.float32, bf16):
@@ -176,7 +195,6 @@ class STDiT2:
             raise NotImplementedError("STDiT2(b200): H and W must be multiples of the patch size")
         T, H, W = Tx, Hx // ps, Wx // ps
         S = H * W
-        N = T * S
         f32 = lambda v: v.to(device=dev, dtype=torch.float32)
         height, width, ar, fps, num_frames = f32(height), f32(width), f32(ar), f32(fps), f32(num_frames)
         rs = (float(height[0]) * float(width[0])) ** 0.5
@@ -215,43 +233,65 @@ class STDiT2:
         freqs = 1.0 / 10000.0 ** (torch.arange(0, hd, 2)[: hd // 2].float() / hd)
         ang = torch.outer(torch.arange(T, dtype=torch.float32), freqs)
         rcos, rsin = ang.cos().contiguous().to(dev), ang.sin().contiguous().to(dev)
+        return _Conditioning(h=h, mod_s=mod_s, mod_t=mod_t, mod_f=mod_f, ye=ye, kv_all=kv_all, kv_lens=kv_lens,
+                             rope_cos=rcos, rope_sin=rsin, B=B, T=T, H=H, W=W)
+
+    def _block(self, i, h, cond):
+        """STDiT2Block i (stdit2.py:119-191) on the bf16 residual stream h [B, T*S, D]; returns the new h."""
+        from .. import ops
+        from .._lib import ACT_GELU_TANH
+        c, D = self.config, self.config.hidden_size
+        Hh, hd, dp = c.num_heads, self.head_dim, self.head_pad
+        B, T, S = cond.B, cond.T, cond.H * cond.W
+        N = T * S
         inner = Hh * dp
-        ldm_s, ldm_t = mod_s.stride(0), mod_t.stride(0)
-        for i, blk in enumerate(self.blocks):
-            ms, mt = mod_s[:, i], mod_t[:, i]  # [B, 6D] / [B, 3D] views with batch stride depth*6D
-            # spatial branch: shift_msa, scale_msa, gate_msa = chunks 0, 1, 2
-            xm = ops.layernorm(h, eps=1e-6, scale=ms[:, D:], shift=ms[:, 0:], rows_per_group=N)
-            qkv = ops.linear(xm, *blk["s_qkv"])  # [B, N, 3*H*dp]
-            q = qkv[:, :, :inner].reshape(B * T, S, Hh, dp) if False else qkv.view(B * T, S, 3 * inner)[:, :, :inner].unflatten(-1, (Hh, dp))
-            k = qkv.view(B * T, S, 3 * inner)[:, :, inner:2 * inner].unflatten(-1, (Hh, dp))
-            v = qkv.view(B * T, S, 3 * inner)[:, :, 2 * inner:].unflatten(-1, (Hh, dp))
-            if c.qk_norm:
-                rows = qkv.view(B * N, 3 * inner)
-                ops.head_rmsnorm_inplace(rows[:, :inner].unflatten(-1, (Hh, dp)), blk["s_qn"], hd)
-                ops.head_rmsnorm_inplace(rows[:, inner:2 * inner].unflatten(-1, (Hh, dp)), blk["s_kn"], hd)
-            a = ops.sdpa(q, k, v, scale=hd ** -0.5)  # [B*T, S, H, dp]
-            h = ops.linear(a.reshape(B, N, inner), *blk["s_proj"], row_gate=ms[:, 2 * D:], rows_per_group=N, residual=h)
-            # temporal branch (shift_tmp, scale_tmp, gate_tmp)
-            xm = ops.layernorm(h, eps=1e-6, scale=mt[:, D:], shift=mt[:, 0:], rows_per_group=N)
-            tqkv = ops.linear(xm, *blk["t_qkv"]).reshape(B * N, 3 * D)
-            ta = ops.small_attention(tqkv, B, T, S, Hh, hd, scale=hd ** -0.5, rope_cos=rcos, rope_sin=rsin,
-                                     q_norm_w=blk.get("t_qn"), k_norm_w=blk.get("t_kn"))
-            h = ops.linear(ta.reshape(B, N, D), *blk["t_proj"], row_gate=mt[:, 2 * D:], rows_per_group=N, residual=h)
-            # cross attention (no modulation, no gate) :173-174
-            cq = ops.linear(h, *blk["c_q"]).unflatten(-1, (Hh, dp))  # [B, N, H, dp]
-            off = i * 2 * inner
-            ck = kv_all[:, :, off:off + inner].unflatten(-1, (Hh, dp))
-            cv = kv_all[:, :, off + inner:off + 2 * inner].unflatten(-1, (Hh, dp))
-            ca = ops.sdpa(cq, ck, cv, scale=hd ** -0.5, kv_lens=kv_lens)
-            h = ops.linear(ca.reshape(B, N, inner), *blk["c_proj"], residual=h)
-            # MLP (shift_mlp, scale_mlp, gate_mlp = chunks 3, 4, 5)
-            xm = ops.layernorm(h, eps=1e-6, scale=ms[:, 4 * D:], shift=ms[:, 3 * D:], rows_per_group=N)
-            f = ops.linear(xm, *blk["fc1"], act=ACT_GELU_TANH)
-            h = ops.linear(f, *blk["fc2"], row_gate=ms[:, 5 * D:], rows_per_group=N, residual=h)
+        blk = self.blocks[i]
+        ms, mt = cond.mod_s[:, i], cond.mod_t[:, i]  # [B, 6D] / [B, 3D] views with batch stride depth*6D / depth*3D
+        # spatial branch: shift_msa, scale_msa, gate_msa = chunks 0, 1, 2
+        xm = ops.layernorm(h, eps=1e-6, scale=ms[:, D:], shift=ms[:, 0:], rows_per_group=N)
+        qkv = ops.linear(xm, *blk["s_qkv"])  # [B, N, 3*H*dp]
+        q = qkv.view(B * T, S, 3 * inner)[:, :, :inner].unflatten(-1, (Hh, dp))
+        k = qkv.view(B * T, S, 3 * inner)[:, :, inner:2 * inner].unflatten(-1, (Hh, dp))
+        v = qkv.view(B * T, S, 3 * inner)[:, :, 2 * inner:].unflatten(-1, (Hh, dp))
+        if c.qk_norm:
+            rows = qkv.view(B * N, 3 * inner)
+            ops.head_rmsnorm_inplace(rows[:, :inner].unflatten(-1, (Hh, dp)), blk["s_qn"], hd)
+            ops.head_rmsnorm_inplace(rows[:, inner:2 * inner].unflatten(-1, (Hh, dp)), blk["s_kn"], hd)
+        a = ops.sdpa(q, k, v, scale=hd ** -0.5)  # [B*T, S, H, dp]
+        h = ops.linear(a.reshape(B, N, inner), *blk["s_proj"], row_gate=ms[:, 2 * D:], rows_per_group=N, residual=h)
+        # temporal branch (shift_tmp, scale_tmp, gate_tmp)
+        xm = ops.layernorm(h, eps=1e-6, scale=mt[:, D:], shift=mt[:, 0:], rows_per_group=N)
+        tqkv = ops.linear(xm, *blk["t_qkv"]).reshape(B * N, 3 * D)
+        ta = ops.small_attention(tqkv, B, T, S, Hh, hd, scale=hd ** -0.5, rope_cos=cond.rope_cos,
+                                 rope_sin=cond.rope_sin, q_norm_w=blk.get("t_qn"), k_norm_w=blk.get("t_kn"))
+        h = ops.linear(ta.reshape(B, N, D), *blk["t_proj"], row_gate=mt[:, 2 * D:], rows_per_group=N, residual=h)
+        # cross attention (no modulation, no gate) :173-174
+        cq = ops.linear(h, *blk["c_q"]).unflatten(-1, (Hh, dp))  # [B, N, H, dp]
+        off = i * 2 * inner
+        ck = cond.kv_all[:, :, off:off + inner].unflatten(-1, (Hh, dp))
+        cv = cond.kv_all[:, :, off + inner:off + 2 * inner].unflatten(-1, (Hh, dp))
+        ca = ops.sdpa(cq, ck, cv, scale=hd ** -0.5, kv_lens=cond.kv_lens)
+        h = ops.linear(ca.reshape(B, N, inner), *blk["c_proj"], residual=h)
+        # MLP (shift_mlp, scale_mlp, gate_mlp = chunks 3, 4, 5)
+        xm = ops.layernorm(h, eps=1e-6, scale=ms[:, 4 * D:], shift=ms[:, 3 * D:], rows_per_group=N)
+        f = ops.linear(xm, *blk["fc1"], act=ACT_GELU_TANH)
+        return ops.linear(f, *blk["fc2"], row_gate=ms[:, 5 * D:], rows_per_group=N, residual=h)
+
+    def forward(self, x, timestep, y, mask=None, x_mask=None, num_frames=None, height=None, width=None, ar=None, fps=None):
+        """Same signature as the reference (stdit2.py:334-336). x [B,C,T,H,W]; y [B,1,L,caption]; returns fp32."""
+        from .. import ops
+        if x_mask is not None:
+            raise NotImplementedError("x_mask (frame masking) is outside the hot path")
+        cond = self._conditioning(x, timestep, y, mask, num_frames, height, width, ar, fps)
+        D, ps = self.config.hidden_size, self.config.patch_size[1]
+        N = cond.T * cond.H * cond.W
+        h = cond.h
+        for i in range(len(self.blocks)):
+            h = self._block(i, h, cond)
         # T2IFinalLayer (blocks.py:376-392): shift, scale = (table + t).chunk(2)
-        hn = ops.layernorm(h, eps=1e-6, scale=mod_f[:, D:], shift=mod_f[:, 0:], rows_per_group=N)
+        hn = ops.layernorm(h, eps=1e-6, scale=cond.mod_f[:, D:], shift=cond.mod_f[:, 0:], rows_per_group=N)
         out = ops.linear(hn, *self.final)  # [B, N, p*p*C_out]
-        return ops.unpatchify3d(out, self.out_channels, T, H, W, ps)
+        return ops.unpatchify3d(out, self.out_channels, cond.T, cond.H, cond.W, ps)
 
     __call__ = forward
 

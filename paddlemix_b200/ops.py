@@ -90,6 +90,22 @@ def init(device: int = 0):
     check(lib.b200mix_init(int(device)), "b200mix_init")
 
 
+def _check_mod_views(op, **mods):
+    """Per-group vectors (AdaLN scale / shift / gate, row_add / row_gate) reach the kernels as (pointer, stride(0)) and
+    are read at group * stride(0) + column: a [groups, width] view is fine, a column stride other than 1 is not, and
+    vectors passed together must share stride(0) (one stride reaches the kernel)."""
+    given = {k: v for k, v in mods.items() if v is not None}
+    for name, v in given.items():
+        if v.dim() == 0 or (v.dim() > 1 and v.shape[-1] > 1 and v.stride(-1) != 1):
+            raise ValueError(f"{op}: {name} must be a [groups, width] view with a contiguous last dimension, "
+                             f"got shape {tuple(v.shape)} strides {v.stride()}")
+        if v.dim() == 1 and v.shape[0] > 1 and v.stride(0) != 1:
+            raise ValueError(f"{op}: {name} must be contiguous, got stride {v.stride(0)}")
+    lds = {v.stride(0) for v in given.values() if v.dim() > 1 and v.shape[0] > 1}
+    if len(lds) > 1:
+        raise ValueError(f"{op}: {', '.join(given)} must share one row stride, got {sorted(lds)}")
+
+
 def make_epilogue(bias=None, row_add=None, row_gate=None, ld_row=0, rows_per_group=0, residual=None, ldr=0,
                   act=ACT_NONE, glu=GLU_NONE, out_fp32=False, out_scale=1.0, residual_row_mod=0, stats_out=None,
                   ln=None) -> Epilogue:
@@ -246,6 +262,8 @@ def linear(a: torch.Tensor, w, bias=None, *, act=ACT_NONE, glu=GLU_NONE, residua
     if residual is not None:
         res2 = residual.reshape(-1, residual.shape[-1])
     mod = row_add if row_add is not None else row_gate
+    if mod is not None:
+        _check_mod_views("linear", row_add=row_add, row_gate=row_gate)
     rs = None
     want_stats = stats is not None and stats is not False
     if want_stats:
@@ -276,6 +294,8 @@ def linear_batched(a: torch.Tensor, w: torch.Tensor, bias=None, *, out: torch.Te
     N = w.shape[0]
     assert a.stride(-1) == 1 and out.stride(-1) == 1 and out.shape[0] == B and out.shape[1] == rows
     mod = row_add if row_add is not None else row_gate
+    if mod is not None:
+        _check_mod_views("linear_batched", row_add=row_add, row_gate=row_gate)
     e = make_epilogue(bias=bias, row_add=row_add, row_gate=row_gate, ld_row=0 if mod is None else mod.stride(0),
                       rows_per_group=rows, residual=residual, ldr=0 if residual is None else residual.stride(1),
                       act=act, glu=glu, out_fp32=(out.dtype == torch.float32))
@@ -318,6 +338,8 @@ def conv3x3(x: torch.Tensor, w: torch.Tensor, bias=None, *, stride=1, row_add=No
     Ho, Wo = H // stride, W // stride
     if out is None:
         out = torch.empty(B, Ho, Wo, Cout, device=x.device, dtype=bf16)
+    if row_add is not None:
+        _check_mod_views("conv3x3", row_add=row_add)
     e = make_epilogue(bias=bias, row_add=row_add, ld_row=0 if row_add is None else row_add.stride(0),
                       rows_per_group=Ho * Wo, residual=residual, ldr=Cout, act=act, out_scale=out_scale)
     with _Timed("igemm", 2.0 * B * Ho * Wo * Cout * 9 * Cin, "flop",
@@ -354,6 +376,8 @@ def conv3x3_up2x(x: torch.Tensor, w4: torch.Tensor, bias=None, *, row_add=None, 
     assert x.is_contiguous() and w4.is_contiguous() and tuple(w4.shape[1:]) == (16, Cin)
     if out is None:
         out = torch.empty(B, 2 * H, 2 * W, Cout, device=x.device, dtype=bf16)
+    if row_add is not None:
+        _check_mod_views("conv3x3_up2x", row_add=row_add)
     e = make_epilogue(bias=bias, row_add=row_add, ld_row=0 if row_add is None else row_add.stride(0),
                       rows_per_group=4 * H * W, residual=residual, ldr=Cout, act=act, out_scale=out_scale)
     with _Timed("igemm", 2.0 * B * 4 * H * W * Cout * 4 * Cin, "flop",
@@ -472,6 +496,8 @@ def layernorm(x: torch.Tensor, weight=None, bias=None, *, eps=1e-5, rms=False, d
         out = torch.empty_like(x)
     resid = torch.empty_like(x) if (want_resid and delta is not None) else None
     mod = gate if gate is not None else (scale if scale is not None else shift)
+    if mod is not None:
+        _check_mod_views("layernorm", gate=gate, scale=scale, shift=shift)
     ld_mod = 0 if mod is None else mod.stride(0)
     nbytes = 2.0 * M * N * (2 + (1 if delta is not None else 0) + (1 if resid is not None else 0))
     with _Timed("layernorm", nbytes, "byte", lambda: f"ln {M}x{N}" + (" +delta" if delta is not None else "")):
@@ -844,10 +870,15 @@ def head_rmsnorm_inplace(x: torch.Tensor, weight: torch.Tensor, d: int, eps: flo
 
 
 def small_attention(qkv: torch.Tensor, B: int, T: int, S: int, H: int, d: int, *, scale: float, rope_cos=None,
-                    rope_sin=None, q_norm_w=None, k_norm_w=None, eps: float = 1e-6) -> torch.Tensor:
-    """qkv bf16 [B*T*S, 3*H*d] (row = (b*T+t)*S+s) -> bf16 [B*T*S, H*d]; attention along the T axis."""
+                    rope_sin=None, q_norm_w=None, k_norm_w=None, eps: float = 1e-6, out=None) -> torch.Tensor:
+    """qkv bf16 [B*T*S, 3*H*d] (row = (b*T+t)*S+s) -> bf16 [B*T*S, H*d]; attention along the T axis. qkv and out may
+    be row-strided views (last dim contiguous)."""
     _req(qkv, bf16, "qkv")
-    out = torch.empty(qkv.shape[0], H * d, device=qkv.device, dtype=bf16)
+    if out is None:
+        out = torch.empty(qkv.shape[0], H * d, device=qkv.device, dtype=bf16)
+    _req(out, bf16, "out")
+    if qkv.stride(-1) != 1 or out.stride(-1) != 1:
+        raise ValueError("small_attention: qkv and out need a contiguous last dimension")
     with _Timed("small_attention", 2.0 * 2 * qkv.shape[0] * 4 * H * d, "byte"):
         check(lib.b200mix_small_attention(_p(qkv), _p(out), B, T, S, H, d, qkv.stride(0), out.stride(0), _p(rope_cos),
                                           _p(rope_sin), _p(q_norm_w), _p(k_norm_w), float(eps), float(scale), _stream()),
