@@ -280,6 +280,30 @@ int b200mix_lcm_step(const void* m_u, const void* m_c, int32_t m_fp32, float gui
                      float c_out, float sqrt_alpha_prev, float sqrt_beta_prev, int32_t prediction_type,
                      float clip_sample_range, void* stream);
 
+/* Open-Sora IDDPM sampling step with learned-range variance and the reference's CFG (ppdiffusers/examples/Open-Sora:
+ * schedulers/iddpm/__init__.py:97-114 forward_with_cfg, gaussian_diffusion.py:278-372 p_mean_variance, :409-485
+ * p_sample; epsilon prediction, clip_denoised = False), one launch, fp32 state x [B, C, N] (N = T*H*W):
+ *   model_out [2B, 2C, N] fp32 | bf16 (m_fp32), conditional rows [0, B) first; channel k < cfg_channel is guided,
+ *     g = uncond + cfg_scale * (cond - uncond), every other channel comes from the conditional rows;
+ *   eps = channels [0, C), v = channels [C, 2C);
+ *   frac = (v + 1) / 2;  logvar = frac * max_log + (1 - frac) * min_log
+ *   x0 = sqrt_recip_ac * x - sqrt_recipm1_ac * eps;  mean = coef1 * x0 + coef2 * x
+ *   x_prev = mean + exp(0.5 * logvar) * noise  (add_noise != 0),  x_prev = mean  (add_noise == 0: respaced index 0)
+ * The six scalars are the scheduler's fp64 tables rounded to fp32 (max_log = log(beta_t), min_log =
+ * posterior_log_variance_clipped[t]). Every operation is rounded on its own in this order; exp is the fp64 exp rounded
+ * to fp32. noise [B, C, N] fp32, or NULL: standard normals from Philox4x32-10 keyed by `seed`, four per element group
+ * g (elements 4g .. 4g+3 of x):
+ *   (r0..r3) = philox4x32_10(counter = (step, g mod 2^32, g div 2^32, 0), key = (seed mod 2^32, seed div 2^32)),
+ *   u_k = (r_k + 0.5) 2^-32,  z_{2p} = fp32(sqrt(-2 ln u_{2p}) cos(2 pi u_{2p+1})),
+ *   z_{2p+1} = fp32(sqrt(-2 ln u_{2p}) sin(2 pi u_{2p+1}))  (fp64 Box-Muller, p = 0, 1).
+ * x_prev may alias x. x_dup (may be NULL) receives a second copy of x_prev: the unconditional half of the next step's
+ * [2B, C, N] model input. */
+int b200mix_iddpm_step(const void* model_out, int32_t m_fp32, const float* x, const float* noise, float* x_prev,
+                       float* x_dup, int64_t B, int64_t C, int64_t n_per_channel, float cfg_scale, int32_t cfg_channel,
+                       float sqrt_recip_alphas_cumprod, float sqrt_recipm1_alphas_cumprod, float posterior_mean_coef1,
+                       float posterior_mean_coef2, float max_log, float min_log, int32_t add_noise, uint64_t seed,
+                       int64_t step, void* stream);
+
 /* rescale_noise_cfg (pipeline_stable_diffusion.py:69-80; pipeline_stable_diffusion_xl.py:1061-1067) in two launches:
  *   ratio[b] = std(eps_c[b]) / std(noise_cfg[b]),  noise_cfg = eps_u + g*(eps_c - eps_u)   (unbiased std over C,H,W)
  *   out = noise_cfg;  ratio != NULL: out = guidance_rescale * (noise_cfg*ratio[b]) + (1 - guidance_rescale) * noise_cfg

@@ -101,6 +101,9 @@ SIGNATURES = {
                              c_float, c_float, c_int32, c_float, c_void_p],
     "b200mix_lcm_step": [c_void_p, c_void_p, c_int32, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_float,
                          c_float, c_float, c_float, c_float, c_float, c_int32, c_float, c_void_p],
+    "b200mix_iddpm_step": [c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_float,
+                           c_int32, c_float, c_float, c_float, c_float, c_float, c_float, c_int32, c_uint64, c_int64,
+                           c_void_p],
     "b200mix_cfg_rescale_ratio": [c_void_p, c_void_p, c_int32, c_float, c_void_p, c_int64, c_int64, c_void_p],
     "b200mix_cfg_combine": [c_void_p, c_void_p, c_int32, c_float, c_void_p, c_float, c_int64, c_void_p, c_int64, c_void_p],
     "b200mix_euler_step": [c_void_p, c_void_p, c_int32, c_float, c_void_p, c_void_p, c_int64, c_float, c_float,

@@ -1,7 +1,8 @@
 // Small HBM-/latency-bound kernels around the denoiser: timestep embedding, activation, nearest upsample, channel
-// concat, NCHW<->NHWC, conv_in (tiny C_in), fused CFG + DDIM / flow-match Euler step, casts, rotary embedding.
+// concat, NCHW<->NHWC, conv_in (tiny C_in), fused CFG + DDIM / flow-match Euler / IDDPM step, casts, rotary embedding.
 // Reference call sites are cited per function in include/b200mix.h.
 #include "common.cuh"
+#include "philox.cuh"
 #include "ptx.cuh"
 
 namespace b200 {
@@ -325,6 +326,66 @@ __global__ void lcm_step_kernel(const void* __restrict__ m_u, const void* __rest
     const float den = __fadd_rn(__fmul_rn(c_out, x0), __fmul_rn(c_skip, xi));
     if (denoised_out) denoised_out[i] = den;
     x_prev[i] = noise ? __fadd_rn(__fmul_rn(sa_p, den), __fmul_rn(sb_p, noise[i])) : den;
+  }
+}
+
+// Open-Sora IDDPM p_sample with learned-range variance (gaussian_diffusion.py:278-372, 409-485) behind forward_with_cfg
+// (schedulers/iddpm/__init__.py:97-114). One thread per group of 4 consecutive state elements, which is one Philox
+// call (philox_normal4). Output channel k of the 2C model channels is guided when k < cfg_channel; the rest are read
+// from the conditional rows [0, B). Every operation is rounded on its own, in the reference's order; exp is the fp32
+// rounding of the fp64 exp.
+struct IddpmArgs {
+  const void* m;           // [2B, 2C, N], conditional rows first
+  const float* x;          // [B, C, N]; may alias x_prev
+  const float* noise;      // [B, C, N] or NULL (Philox)
+  float* x_prev;           // [B, C, N]
+  float* x_dup;            // optional second copy of x_prev (the unconditional half of the model input)
+  long long B, C, N;
+  int m_fp32, cfg_channel, add_noise;
+  float cfg_scale, sqrt_recip, sqrt_recipm1, coef1, coef2, max_log, min_log;
+  unsigned long long seed;
+  uint32_t step;
+};
+
+__global__ void __launch_bounds__(256) iddpm_step_kernel(IddpmArgs a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const long long n = a.B * a.C * a.N, CN = a.C * a.N;
+  const long long groups = (n + 3) >> 2;
+  for (long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x; g < groups; g += (long long)gridDim.x * blockDim.x) {
+    float z[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+    if (a.add_noise && !a.noise) philox_normal4(a.seed, a.step, (unsigned long long)g, z);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const long long i = 4 * g + k;
+      if (i >= n) break;
+      const long long b = i / CN, r = i - b * CN;
+      const long long c = r / a.N, j = r - c * a.N;
+      const long long ec = (b * 2 * a.C + c) * a.N + j;          // eps channel c, conditional row b
+      const long long vc = ec + CN;                                // variance channel C + c
+      const long long off_u = a.B * 2 * CN;                        // unconditional row B + b
+      float e = load_any(a.m, ec, a.m_fp32);
+      if (c < a.cfg_channel) {
+        const float u = load_any(a.m, ec + off_u, a.m_fp32);
+        e = __fadd_rn(u, __fmul_rn(a.cfg_scale, __fsub_rn(e, u)));
+      }
+      float v = load_any(a.m, vc, a.m_fp32);
+      if (a.C + c < a.cfg_channel) {
+        const float u = load_any(a.m, vc + off_u, a.m_fp32);
+        v = __fadd_rn(u, __fmul_rn(a.cfg_scale, __fsub_rn(v, u)));
+      }
+      const float xi = a.x[i];
+      const float frac = __fdiv_rn(__fadd_rn(v, 1.0f), 2.0f);
+      const float logvar = __fadd_rn(__fmul_rn(frac, a.max_log), __fmul_rn(__fsub_rn(1.0f, frac), a.min_log));
+      const float x0 = __fsub_rn(__fmul_rn(a.sqrt_recip, xi), __fmul_rn(a.sqrt_recipm1, e));
+      float out = __fadd_rn(__fmul_rn(a.coef1, x0), __fmul_rn(a.coef2, xi));
+      if (a.add_noise) {
+        const float sd = (float)exp((double)__fmul_rn(0.5f, logvar));
+        out = __fadd_rn(out, __fmul_rn(sd, a.noise ? a.noise[i] : z[k]));
+      }
+      a.x_prev[i] = out;
+      if (a.x_dup) a.x_dup[i] = out;
+    }
   }
 }
 
@@ -672,6 +733,27 @@ extern "C" int b200mix_lcm_step(const void* m_u, const void* m_c, int32_t m_fp32
                                                           sqrt_alpha_t, sqrt_beta_t, c_skip, c_out, sqrt_alpha_prev,
                                                           sqrt_beta_prev, prediction_type, clip_sample_range);
   B200_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int b200mix_iddpm_step(const void* model_out, int32_t m_fp32, const float* x, const float* noise, float* x_prev,
+                                  float* x_dup, int64_t B, int64_t C, int64_t n_per_channel, float cfg_scale,
+                                  int32_t cfg_channel, float sqrt_recip_alphas_cumprod, float sqrt_recipm1_alphas_cumprod,
+                                  float posterior_mean_coef1, float posterior_mean_coef2, float max_log, float min_log,
+                                  int32_t add_noise, uint64_t seed, int64_t step, void* stream) {
+  if (int rc = ensure_device()) return rc;
+  B200_CHECK_ARG(model_out && x && x_prev && B > 0 && C > 0 && n_per_channel > 0, "iddpm_step: bad arguments");
+  B200_CHECK_ARG(cfg_channel >= 0 && cfg_channel <= 2 * C, "iddpm_step: cfg_channel must lie in [0, 2C]");
+  B200_CHECK_ARG(step >= 0 && step <= 0xFFFFFFFFll, "iddpm_step: step must fit 32 bits");
+  IddpmArgs a;
+  a.m = model_out, a.x = x, a.noise = noise, a.x_prev = x_prev, a.x_dup = x_dup;
+  a.B = B, a.C = C, a.N = n_per_channel;
+  a.m_fp32 = m_fp32, a.cfg_channel = cfg_channel, a.add_noise = add_noise ? 1 : 0;
+  a.cfg_scale = cfg_scale, a.sqrt_recip = sqrt_recip_alphas_cumprod, a.sqrt_recipm1 = sqrt_recipm1_alphas_cumprod;
+  a.coef1 = posterior_mean_coef1, a.coef2 = posterior_mean_coef2, a.max_log = max_log, a.min_log = min_log;
+  a.seed = seed, a.step = (uint32_t)step;
+  const long long groups = (B * C * n_per_channel + 3) / 4;
+  B200_CUDA(launch_pdl(iddpm_step_kernel, dim3(ew_grid(groups, 256)), dim3(256), 0, ST(stream), 1, a));
   return 0;
 }
 

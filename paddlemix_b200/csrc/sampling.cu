@@ -24,6 +24,7 @@
 #include <float.h>
 
 #include "common.cuh"
+#include "philox.cuh"
 #include "ptx.cuh"
 
 namespace b200 {
@@ -52,20 +53,6 @@ struct SampleArgs {
   float temperature, top_p, penalty;
   unsigned long long seed;
 };
-
-__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    if (r) {
-      k.x += 0x9E3779B9u;
-      k.y += 0xBB67AE85u;
-    }
-    const uint32_t lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
-    const uint32_t lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
-    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
-  }
-  return c;
-}
 
 struct Row {
   const float* x;

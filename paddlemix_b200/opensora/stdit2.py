@@ -66,6 +66,7 @@ class STDiT2:
         self.out_channels = c.in_channels * 2 if c.pred_sigma else c.in_channels
         self.dtype = bf16
         self.device = None
+        self.y_embedding = None
 
     def state_dict_shapes(self) -> Dict[str, tuple]:
         c = self.config
@@ -145,8 +146,23 @@ class STDiT2:
             self.blocks.append(blk)
         self.kv_w = torch.cat(kv_w, 0).to(dev, bf16).contiguous()  # all blocks' cross-attn k|v projections: one GEMM
         self.kv_b = torch.cat(kv_b, 0).to(dev).contiguous()
+        # the null caption of classifier-free guidance (CaptionEmbedder.y_embedding, blocks.py:452-458): kept when the
+        # state dict has it, outside state_dict_shapes() so that synthetic weights do not change
+        self.y_embedding = None
+        if "y_embedder.y_embedding" in P:
+            ye = to_f32(P["y_embedder.y_embedding"])
+            if ye.ndim != 2 or ye.shape[1] != c.caption_channels:
+                raise ValueError(f"y_embedder.y_embedding {tuple(ye.shape)} must be [model_max_length, {c.caption_channels}]")
+            self.y_embedding = ye.to(dev, bf16).contiguous()
         self._pos_cache = {}
         return self
+
+    def null_caption(self, n: int) -> Optional[torch.Tensor]:
+        """The null caption tiled to n samples, bf16 [n, 1, L, caption] (T5Encoder.null, t5.py:124-126), or None when
+        the loaded weights did not hold y_embedder.y_embedding."""
+        if self.y_embedding is None:
+            return None
+        return self.y_embedding[None, None].repeat(n, 1, 1, 1)
 
     # ------------------------------------------------------------------------------------------------------------
     def _embed_scalar(self, pair, s, residual=None):

@@ -646,6 +646,36 @@ def lcm_step(m_u, m_c, guidance, x, noise, sa_t, sb_t, c_skip, c_out, sa_p, sb_p
     return out
 
 
+def iddpm_step(model_out, x, cfg_scale, cfg_channel, scalars, add_noise, seed=0, step=0, noise=None, out=None, out_dup=None):
+    """Open-Sora IDDPM p_sample behind forward_with_cfg (b200mix_iddpm_step). model_out [2B, 2C, ...] fp32 | bf16 with
+    the conditional rows first; x fp32 [B, C, ...]; scalars = (sqrt_recip_ac, sqrt_recipm1_ac, coef1, coef2, max_log,
+    min_log) as fp32 values; noise fp32 like x, or None for Philox noise keyed by (seed, step). out may be x itself;
+    out_dup receives a second copy of the result. Returns out."""
+    _req(x, torch.float32, "x")
+    B, C = x.shape[:2]
+    if model_out.dtype not in (torch.float32, bf16) or not model_out.is_contiguous():
+        raise ValueError("model_out must be contiguous fp32 or bf16")
+    if tuple(model_out.shape) != (2 * B, 2 * C, *x.shape[2:]):
+        raise ValueError(f"model_out {tuple(model_out.shape)} must be [2B, 2C, ...] for x {tuple(x.shape)}")
+    if noise is not None:
+        _req(noise, torch.float32, "noise")
+        assert noise.shape == x.shape
+    if out is None:
+        out = torch.empty_like(x)
+    for t in (out, out_dup):
+        if t is not None:
+            _req(t, torch.float32, "out")
+            assert t.shape == x.shape
+    if not all(t is None or t.is_contiguous() for t in (x, noise, out, out_dup)):
+        raise ValueError("iddpm_step: x, noise and the outputs must be contiguous")
+    check(lib.b200mix_iddpm_step(_p(model_out), 1 if model_out.dtype == torch.float32 else 0, _p(x), _p(noise), _p(out),
+                                 _p(out_dup), B, C, x.numel() // (B * C), float(cfg_scale), int(cfg_channel),
+                                 *(float(v) for v in scalars), 1 if add_noise else 0, int(seed), int(step), _stream()),
+          "b200mix_iddpm_step")
+    _count()
+    return out
+
+
 def cfg_combine(eps_u, eps_c, guidance, guidance_rescale=0.0, out=None):
     """noise_pred_uncond + g * (noise_pred_text - noise_pred_uncond), then rescale_noise_cfg when guidance_rescale > 0
     (pipeline_stable_diffusion.py:69-80, :882-888). eps_*: [B, ...] bf16 / fp32 contiguous. Returns fp32."""
