@@ -254,19 +254,15 @@ int b200mix_nhwc_to_nchw(const void* x, void* y, int32_t y_fp32, int64_t B, int6
 int b200mix_add_residual_nhwc(const void* a, const void* r, int32_t r_fp32, int32_t r_nchw, void* y, int64_t B, int64_t C,
                               int64_t H, int64_t W, void* stream);
 
-/* Fused classifier-free-guidance combine + DDIM step (eta = 0, epsilon prediction), fp32 state:
- *   eps = eps_u + g*(eps_c - eps_u)  (pipeline_stable_diffusion.py:882-884; eps_c NULL => eps = eps_u)
- *   x0 = (x - sqrt_beta_t*eps) / sqrt_alpha_t ; x_prev = sqrt_alpha_prev*x0 + sqrt_beta_prev*eps
- * The four scalars are computed on the host by the scheduler, bit-exactly as scheduling_ddim.py:410-457 does, and
- * applied here with the same operation order in fp32. eps inputs bf16 or fp32 (eps_fp32). */
-int b200mix_ddim_step(const void* eps_u, const void* eps_c, int32_t eps_fp32, float guidance, const float* x,
-                      float* x_prev, int64_t n, float sqrt_alpha_t, float sqrt_beta_t, float sqrt_alpha_prev,
-                      float sqrt_beta_prev, void* stream);
-
-/* DDIM step for every prediction_type (0 = epsilon, 1 = sample, 2 = v_prediction; scheduling_ddim.py:424-443) with
- * optional clip_sample (clip_sample_range > 0 clips the predicted x0, :446-452; <= 0: off), eta = 0, fused CFG combine:
+/* Fused classifier-free-guidance combine + DDIM step (scheduling_ddim.py:410-457), eta = 0, fp32 state, for every
+ * prediction_type (0 = epsilon, 1 = sample, 2 = v_prediction; :424-443) with optional clip_sample (clip_sample_range > 0
+ * clips the predicted x0, :446-452; <= 0: off):
+ *   m = m_u + g*(m_c - m_u)  (pipeline_stable_diffusion.py:882-884; m_c NULL => m = m_u); m_u, m_c bf16 or fp32 (m_fp32)
  *   epsilon: x0 = (x - sb_t*m)/sa_t, eps = m;  sample: x0 = m, eps = (x - sa_t*x0)/sb_t;
- *   v_prediction: x0 = sa_t*x - sb_t*m, eps = sa_t*m + sb_t*x;   x_prev = sa_p*clip(x0) + sb_p*eps. */
+ *   v_prediction: x0 = sa_t*x - sb_t*m, eps = sa_t*m + sb_t*x;   x_prev = sa_p*clip(x0) + sb_p*eps.
+ * The four scalars sa_t = sqrt(alpha_prod_t), sb_t = sqrt(1 - alpha_prod_t) and sa_p, sb_p (the same for the previous
+ * timestep) are computed on the host by the scheduler, bit-exactly as scheduling_ddim.py:410-457 does, and applied here
+ * with the same operation order in fp32. */
 int b200mix_ddim_step_ex(const void* m_u, const void* m_c, int32_t m_fp32, float guidance, const float* x, float* x_prev,
                          int64_t n, float sqrt_alpha_t, float sqrt_beta_t, float sqrt_alpha_prev, float sqrt_beta_prev,
                          int32_t prediction_type, float clip_sample_range, void* stream);

@@ -95,8 +95,6 @@ SIGNATURES = {
     "b200mix_nhwc_to_nchw": [c_void_p, c_void_p, c_int32, c_int64, c_int64, c_int64, c_int64, c_void_p],
     "b200mix_add_residual_nhwc": [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int64, c_int64, c_int64, c_int64,
                                   c_void_p],
-    "b200mix_ddim_step": [c_void_p, c_void_p, c_int32, c_float, c_void_p, c_void_p, c_int64, c_float, c_float,
-                          c_float, c_float, c_void_p],
     "b200mix_ddim_step_ex": [c_void_p, c_void_p, c_int32, c_float, c_void_p, c_void_p, c_int64, c_float, c_float,
                              c_float, c_float, c_int32, c_float, c_void_p],
     "b200mix_lcm_step": [c_void_p, c_void_p, c_int32, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_float,

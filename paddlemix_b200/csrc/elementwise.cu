@@ -24,6 +24,18 @@ __device__ __forceinline__ float load_any(const void* p, long long i, int fp32) 
   return fp32 ? reinterpret_cast<const float*>(p)[i] : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p)[i]);
 }
 
+// Classifier-free guidance, u + g*(c - u) (pipeline_stable_diffusion.py:882-884), every operation rounded on its own
+// so that every sampler step matches the fp32 CPU evaluation of the same expression bit for bit.
+__device__ __forceinline__ float cfg_mix(float u, float c, float g) {
+  return __fadd_rn(u, __fmul_rn(g, __fsub_rn(c, u)));
+}
+
+// Element i of the model output, guided: m_c == NULL means no guidance (the output is m_u itself).
+__device__ __forceinline__ float load_guided(const void* m_u, const void* m_c, long long i, int fp32, float g) {
+  const float u = load_any(m_u, i, fp32);
+  return m_c ? cfg_mix(u, load_any(m_c, i, fp32), g) : u;
+}
+
 // embeddings.py:26-64 — exponent = -ln(max_period) * i / (half - shift); emb = scale * t * exp(exponent);
 // [sin | cos], swapped to [cos | sin] when flip_sin_to_cos.
 __global__ void timestep_embedding_kernel(const float* __restrict__ t, void* __restrict__ out, int out_fp32, int B,
@@ -256,55 +268,39 @@ __global__ void conv3x3_small_cin_kernel(const void* __restrict__ x, int x_fp32,
 }
 
 
-// scheduling_ddim.py:410-457 with eta = 0, epsilon prediction, no clipping; every operation individually rounded
-// (no FMA contraction) so the result is bit-identical to the fp32 CPU evaluation of the same expression.
-__global__ void ddim_step_kernel(const void* __restrict__ eps_u, const void* __restrict__ eps_c, int eps_fp32,
-                                 float guidance, const float* __restrict__ x, float* __restrict__ x_prev, long long n,
-                                 float sa_t, float sb_t, float sa_p, float sb_p) {
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    float e = load_any(eps_u, i, eps_fp32);
-    if (eps_c) {
-      const float ec = load_any(eps_c, i, eps_fp32);
-      e = __fadd_rn(e, __fmul_rn(guidance, __fsub_rn(ec, e)));
-    }
-    const float x0 = __fdiv_rn(__fsub_rn(x[i], __fmul_rn(sb_t, e)), sa_t);
-    x_prev[i] = __fadd_rn(__fmul_rn(sa_p, x0), __fmul_rn(sb_p, e));
-  }
-}
-
-// DDIM step for every prediction type (scheduling_ddim.py:424-443) with optional clipping of the predicted x0
-// (:446-452), eta = 0; same operation order as the reference, every operation rounded individually.
+// x0 and eps from the model output m for each prediction_type (scheduling_ddim.py:424-443, scheduling_lcm.py:530-535),
+// in the reference's operation order:
 //   epsilon      x0 = (x - sb_t*m) / sa_t            eps = m
 //   sample       x0 = m                               eps = (x - sa_t*x0) / sb_t
 //   v_prediction x0 = sa_t*x - sb_t*m                 eps = sa_t*m + sb_t*x
+__device__ __forceinline__ void predict_x0_eps(int pred_type, float m, float x, float sa_t, float sb_t, float& x0,
+                                               float& eps) {
+  if (pred_type == 0) {
+    x0 = __fdiv_rn(__fsub_rn(x, __fmul_rn(sb_t, m)), sa_t);
+    eps = m;
+  } else if (pred_type == 1) {
+    x0 = m;
+    eps = __fdiv_rn(__fsub_rn(x, __fmul_rn(sa_t, x0)), sb_t);
+  } else {
+    x0 = __fsub_rn(__fmul_rn(sa_t, x), __fmul_rn(sb_t, m));
+    eps = __fadd_rn(__fmul_rn(sa_t, m), __fmul_rn(sb_t, x));
+  }
+}
+
+// DDIM step (scheduling_ddim.py:410-457), eta = 0, with optional clipping of the predicted x0 (:446-452):
 //   x_prev = sa_p * clip(x0) + sb_p * eps            (use_clipped_model_output = False: eps is NOT re-derived)
 __global__ void ddim_step_ex_kernel(const void* __restrict__ m_u, const void* __restrict__ m_c, int m_fp32, float guidance,
                                     const float* __restrict__ x, float* __restrict__ x_prev, long long n, float sa_t,
                                     float sb_t, float sa_p, float sb_p, int pred_type, float clip) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    float m = load_any(m_u, i, m_fp32);
-    if (m_c) {
-      const float mc = load_any(m_c, i, m_fp32);
-      m = __fadd_rn(m, __fmul_rn(guidance, __fsub_rn(mc, m)));
-    }
-    const float xi = x[i];
     float x0, e;
-    if (pred_type == 0) {
-      x0 = __fdiv_rn(__fsub_rn(xi, __fmul_rn(sb_t, m)), sa_t);
-      e = m;
-    } else if (pred_type == 1) {
-      x0 = m;
-      e = __fdiv_rn(__fsub_rn(xi, __fmul_rn(sa_t, x0)), sb_t);
-    } else {
-      x0 = __fsub_rn(__fmul_rn(sa_t, xi), __fmul_rn(sb_t, m));
-      e = __fadd_rn(__fmul_rn(sa_t, m), __fmul_rn(sb_t, xi));
-    }
+    predict_x0_eps(pred_type, load_guided(m_u, m_c, i, m_fp32, guidance), x[i], sa_t, sb_t, x0, e);
     if (clip > 0.0f) x0 = fminf(fmaxf(x0, -clip), clip);
     x_prev[i] = __fadd_rn(__fmul_rn(sa_p, x0), __fmul_rn(sb_p, e));
   }
 }
 
-// LCMScheduler.step (scheduling_lcm.py:468-545): x0 from the model output (as above), optional clip,
+// LCMScheduler.step (scheduling_lcm.py:468-545): x0 from the model output (as above; eps unused), optional clip,
 // denoised = c_out*x0 + c_skip*x, then x_prev = sa_p*denoised + sb_p*noise (multi-step; the noise tensor is the
 // caller's randn) or x_prev = denoised on the final step (noise == NULL).
 __global__ void lcm_step_kernel(const void* __restrict__ m_u, const void* __restrict__ m_c, int m_fp32, float guidance,
@@ -312,16 +308,9 @@ __global__ void lcm_step_kernel(const void* __restrict__ m_u, const void* __rest
                                 float* __restrict__ denoised_out, long long n, float sa_t, float sb_t, float c_skip,
                                 float c_out, float sa_p, float sb_p, int pred_type, float clip) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    float m = load_any(m_u, i, m_fp32);
-    if (m_c) {
-      const float mc = load_any(m_c, i, m_fp32);
-      m = __fadd_rn(m, __fmul_rn(guidance, __fsub_rn(mc, m)));
-    }
     const float xi = x[i];
-    float x0;
-    if (pred_type == 0) x0 = __fdiv_rn(__fsub_rn(xi, __fmul_rn(sb_t, m)), sa_t);
-    else if (pred_type == 1) x0 = m;
-    else x0 = __fsub_rn(__fmul_rn(sa_t, xi), __fmul_rn(sb_t, m));
+    float x0, unused;
+    predict_x0_eps(pred_type, load_guided(m_u, m_c, i, m_fp32, guidance), xi, sa_t, sb_t, x0, unused);
     if (clip > 0.0f) x0 = fminf(fmaxf(x0, -clip), clip);
     const float den = __fadd_rn(__fmul_rn(c_out, x0), __fmul_rn(c_skip, xi));
     if (denoised_out) denoised_out[i] = den;
@@ -365,15 +354,9 @@ __global__ void __launch_bounds__(256) iddpm_step_kernel(IddpmArgs a) {
       const long long vc = ec + CN;                                // variance channel C + c
       const long long off_u = a.B * 2 * CN;                        // unconditional row B + b
       float e = load_any(a.m, ec, a.m_fp32);
-      if (c < a.cfg_channel) {
-        const float u = load_any(a.m, ec + off_u, a.m_fp32);
-        e = __fadd_rn(u, __fmul_rn(a.cfg_scale, __fsub_rn(e, u)));
-      }
+      if (c < a.cfg_channel) e = cfg_mix(load_any(a.m, ec + off_u, a.m_fp32), e, a.cfg_scale);
       float v = load_any(a.m, vc, a.m_fp32);
-      if (a.C + c < a.cfg_channel) {
-        const float u = load_any(a.m, vc + off_u, a.m_fp32);
-        v = __fadd_rn(u, __fmul_rn(a.cfg_scale, __fsub_rn(v, u)));
-      }
+      if (a.C + c < a.cfg_channel) v = cfg_mix(load_any(a.m, vc + off_u, a.m_fp32), v, a.cfg_scale);
       const float xi = a.x[i];
       const float frac = __fdiv_rn(__fadd_rn(v, 1.0f), 2.0f);
       const float logvar = __fadd_rn(__fmul_rn(frac, a.max_log), __fmul_rn(__fsub_rn(1.0f, frac), a.min_log));
@@ -400,7 +383,7 @@ __global__ void __launch_bounds__(256) cfg_rescale_ratio_kernel(const void* __re
   double st = 0.0, qt = 0.0, sc = 0.0, qc = 0.0;
   for (long long i = threadIdx.x; i < nps; i += blockDim.x) {
     const float u = load_any(e_u, base + i, fp32), c = load_any(e_c, base + i, fp32);
-    const float cfg = __fadd_rn(u, __fmul_rn(guidance, __fsub_rn(c, u)));
+    const float cfg = cfg_mix(u, c, guidance);
     st += c, qt += (double)c * c, sc += cfg, qc += (double)cfg * cfg;
   }
   sh[0][threadIdx.x] = st, sh[1][threadIdx.x] = qt, sh[2][threadIdx.x] = sc, sh[3][threadIdx.x] = qc;
@@ -425,7 +408,7 @@ __global__ void cfg_combine_kernel(const void* __restrict__ e_u, const void* __r
   const float one_minus = __fsub_rn(1.0f, gr);
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const float u = load_any(e_u, i, fp32), c = load_any(e_c, i, fp32);
-    float cfg = __fadd_rn(u, __fmul_rn(guidance, __fsub_rn(c, u)));
+    float cfg = cfg_mix(u, c, guidance);
     if (ratio) {
       const float resc = __fmul_rn(cfg, __ldg(ratio + i / nps));
       cfg = __fadd_rn(__fmul_rn(gr, resc), __fmul_rn(one_minus, cfg));
@@ -445,11 +428,7 @@ __global__ void euler_step_kernel(const void* __restrict__ v_u, const void* __re
                                   const float* __restrict__ x, float* __restrict__ x_prev, long long n, float sigma,
                                   float dt) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    float v = load_any(v_u, i, v_fp32);
-    if (v_c) {
-      const float vc = load_any(v_c, i, v_fp32);
-      v = __fadd_rn(v, __fmul_rn(guidance, __fsub_rn(vc, v)));
-    }
+    const float v = load_guided(v_u, v_c, i, v_fp32, guidance);
     // scheduling_flow_match_euler_discrete.py:262-270: denoised = x - v*sigma; derivative = (x - denoised)/sigma_hat
     const float xi = x[i];
     const float den = __fsub_rn(xi, __fmul_rn(v, sigma));
@@ -696,17 +675,6 @@ extern "C" int b200mix_conv3x3_small_cin(const void* x, int32_t x_fp32, const vo
   return 0;
 }
 
-extern "C" int b200mix_ddim_step(const void* eps_u, const void* eps_c, int32_t eps_fp32, float guidance, const float* x,
-                                 float* x_prev, int64_t n, float sqrt_alpha_t, float sqrt_beta_t,
-                                 float sqrt_alpha_prev, float sqrt_beta_prev, void* stream) {
-  if (int rc = ensure_device()) return rc;
-  B200_CHECK_ARG(eps_u && x && x_prev && n > 0, "ddim_step: bad arguments");
-  ddim_step_kernel<<<ew_grid(n, 256), 256, 0, ST(stream)>>>(eps_u, eps_c, eps_fp32, guidance, x, x_prev, n,
-                                                           sqrt_alpha_t, sqrt_beta_t, sqrt_alpha_prev, sqrt_beta_prev);
-  B200_LAUNCH_CHECK();
-  return 0;
-}
-
 extern "C" int b200mix_ddim_step_ex(const void* m_u, const void* m_c, int32_t m_fp32, float guidance, const float* x,
                                     float* x_prev, int64_t n, float sqrt_alpha_t, float sqrt_beta_t,
                                     float sqrt_alpha_prev, float sqrt_beta_prev, int32_t prediction_type,
@@ -793,11 +761,7 @@ __global__ void dpmpp_2m_step_kernel(const void* __restrict__ eps_u, const void*
                                      float* __restrict__ x_next, float* __restrict__ m_out, long long n, float sigma_cur,
                                      float alpha_cur, float A, float C, float halfC, float inv_r0) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    float e = load_any(eps_u, i, eps_fp32);
-    if (eps_c) {
-      const float ec = load_any(eps_c, i, eps_fp32);
-      e = __fadd_rn(e, __fmul_rn(guidance, __fsub_rn(ec, e)));
-    }
+    const float e = load_guided(eps_u, eps_c, i, eps_fp32, guidance);
     const float xv = x[i];
     const float m0 = __fdiv_rn(__fsub_rn(xv, __fmul_rn(sigma_cur, e)), alpha_cur);
     float r = __fsub_rn(__fmul_rn(A, xv), __fmul_rn(C, m0));

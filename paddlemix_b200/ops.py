@@ -604,28 +604,41 @@ def add_residual_nhwc(a: torch.Tensor, r: torch.Tensor, *, r_nchw: bool, out=Non
     return out
 
 
-def ddim_step(eps_u, eps_c, guidance, x, sa_t, sb_t, sa_p, sb_p, out=None):
-    _req(x, torch.float32, "x")
+def _step_tensors(op, x, m_u, m_c, out, **fp32_bufs):
+    """Checks the tensors of a sampler step before anything is launched; returns (m_u's dtype flag, out), allocating out
+    like x (like m_u when x is None) if it is None. The kernels read every tensor flat over x's element count (m_u's
+    when x is None) and m_c with m_u's dtype flag, so each given tensor must be contiguous, have that many elements and
+    the dtype below: x, out and fp32_bufs fp32, m_u fp32 or bf16, m_c m_u's dtype."""
+    f32 = (torch.float32,)
+    want = {"x": (x, f32), "model output": (m_u, (torch.float32, bf16)), "model_output_cond": (m_c, (m_u.dtype,)),
+            "out": (out, f32), **{k: (t, f32) for k, t in fp32_bufs.items()}}
+    given = {k: v for k, v in want.items() if v[0] is not None}
+    n = (m_u if x is None else x).numel()
+    for name, (t, dtypes) in given.items():
+        if t.dtype not in dtypes:
+            raise TypeError(f"{op}: {name} must be {' or '.join(map(str, dtypes))}, got {t.dtype}")
+        if t.numel() != n:
+            raise ValueError(f"{op}: {name} has {t.numel()} elements, expected {n}")
+        if not t.is_contiguous():
+            raise ValueError(f"{op}: {name} must be contiguous, got strides {t.stride()} for shape {tuple(t.shape)}")
+    for name, (t, _) in given.items():
+        if not t.is_cuda:
+            raise _lib.B200MixError(f"{op}: {name} must be a CUDA tensor (b200mix has no CPU path)")
     if out is None:
-        out = torch.empty_like(x)
-    check(lib.b200mix_ddim_step(_p(eps_u), _p(eps_c), 1 if eps_u.dtype == torch.float32 else 0, float(guidance), _p(x),
-                                _p(out), x.numel(), float(sa_t), float(sb_t), float(sa_p), float(sb_p), _stream()),
-          "b200mix_ddim_step")
-    _count()
-    return out
+        like = m_u if x is None else x
+        out = torch.empty(like.shape, device=like.device, dtype=torch.float32)
+    return (1 if m_u.dtype == torch.float32 else 0), out
 
 
 PRED_TYPES = {"epsilon": 0, "sample": 1, "v_prediction": 2}
 
 
-def ddim_step_ex(m_u, m_c, guidance, x, sa_t, sb_t, sa_p, sb_p, prediction_type="epsilon", clip_sample_range=0.0, out=None):
+def ddim_step(m_u, m_c, guidance, x, sa_t, sb_t, sa_p, sb_p, prediction_type="epsilon", clip_sample_range=0.0, out=None):
     """DDIM step for any prediction_type, optional x0 clipping (clip_sample_range > 0), fused CFG combine."""
-    _req(x, torch.float32, "x")
-    if out is None:
-        out = torch.empty_like(x)
-    check(lib.b200mix_ddim_step_ex(_p(m_u), _p(m_c), 1 if m_u.dtype == torch.float32 else 0, float(guidance), _p(x), _p(out),
-                                   x.numel(), float(sa_t), float(sb_t), float(sa_p), float(sb_p),
-                                   PRED_TYPES[prediction_type], float(clip_sample_range), _stream()), "b200mix_ddim_step_ex")
+    fp32, out = _step_tensors("ddim_step", x, m_u, m_c, out)
+    check(lib.b200mix_ddim_step_ex(_p(m_u), _p(m_c), fp32, float(guidance), _p(x), _p(out), x.numel(), float(sa_t),
+                                   float(sb_t), float(sa_p), float(sb_p), PRED_TYPES[prediction_type],
+                                   float(clip_sample_range), _stream()), "b200mix_ddim_step_ex")
     _count()
     return out
 
@@ -633,15 +646,10 @@ def ddim_step_ex(m_u, m_c, guidance, x, sa_t, sb_t, sa_p, sb_p, prediction_type=
 def lcm_step(m_u, m_c, guidance, x, noise, sa_t, sb_t, c_skip, c_out, sa_p, sb_p, prediction_type="epsilon",
              clip_sample_range=0.0, out=None, denoised=None):
     """LCMScheduler.step; noise None = final step (x_prev = denoised)."""
-    _req(x, torch.float32, "x")
-    if noise is not None:
-        _req(noise, torch.float32, "noise")
-    if out is None:
-        out = torch.empty_like(x)
-    check(lib.b200mix_lcm_step(_p(m_u), _p(m_c), 1 if m_u.dtype == torch.float32 else 0, float(guidance), _p(x), _p(noise),
-                               _p(out), _p(denoised), x.numel(), float(sa_t), float(sb_t), float(c_skip), float(c_out),
-                               float(sa_p), float(sb_p), PRED_TYPES[prediction_type], float(clip_sample_range), _stream()),
-          "b200mix_lcm_step")
+    fp32, out = _step_tensors("lcm_step", x, m_u, m_c, out, noise=noise, denoised=denoised)
+    check(lib.b200mix_lcm_step(_p(m_u), _p(m_c), fp32, float(guidance), _p(x), _p(noise), _p(out), _p(denoised),
+                               x.numel(), float(sa_t), float(sb_t), float(c_skip), float(c_out), float(sa_p), float(sb_p),
+                               PRED_TYPES[prediction_type], float(clip_sample_range), _stream()), "b200mix_lcm_step")
     _count()
     return out
 
@@ -679,12 +687,11 @@ def iddpm_step(model_out, x, cfg_scale, cfg_channel, scalars, add_noise, seed=0,
 def cfg_combine(eps_u, eps_c, guidance, guidance_rescale=0.0, out=None):
     """noise_pred_uncond + g * (noise_pred_text - noise_pred_uncond), then rescale_noise_cfg when guidance_rescale > 0
     (pipeline_stable_diffusion.py:69-80, :882-888). eps_*: [B, ...] bf16 / fp32 contiguous. Returns fp32."""
-    assert eps_u.shape == eps_c.shape and eps_u.dtype == eps_c.dtype and eps_u.is_contiguous() and eps_c.is_contiguous()
+    fp32, out = _step_tensors("cfg_combine", None, eps_u, eps_c, out)
+    if eps_c is None or eps_c.shape != eps_u.shape:
+        raise ValueError(f"cfg_combine: eps_c must have eps_u's shape {tuple(eps_u.shape)}: samples are along dim 0")
     B = eps_u.shape[0]
     nps = eps_u.numel() // B
-    fp32 = 1 if eps_u.dtype == torch.float32 else 0
-    if out is None:
-        out = torch.empty(eps_u.shape, device=eps_u.device, dtype=torch.float32)
     ratio = None
     if guidance_rescale > 0.0:
         ratio = torch.empty(B, device=eps_u.device, dtype=torch.float32)
@@ -698,23 +705,19 @@ def cfg_combine(eps_u, eps_c, guidance, guidance_rescale=0.0, out=None):
 
 
 def euler_step(v_u, v_c, guidance, x, sigma, dt, out=None):
-    _req(x, torch.float32, "x")
-    if out is None:
-        out = torch.empty_like(x)
-    check(lib.b200mix_euler_step(_p(v_u), _p(v_c), 1 if v_u.dtype == torch.float32 else 0, float(guidance), _p(x),
-                                 _p(out), x.numel(), float(sigma), float(dt), _stream()), "b200mix_euler_step")
+    fp32, out = _step_tensors("euler_step", x, v_u, v_c, out)
+    check(lib.b200mix_euler_step(_p(v_u), _p(v_c), fp32, float(guidance), _p(x), _p(out), x.numel(), float(sigma),
+                                 float(dt), _stream()), "b200mix_euler_step")
     _count()
     return out
 
 
 def dpmpp_2m_step(eps_u, eps_c, guidance, x, m_prev, m_out, sigma_cur, alpha_cur, A, C, halfC, inv_r0, out=None):
     """DPM-Solver++ 2M update (see include/b200mix.h); m_prev None = first-order step; m_out receives x0."""
-    _req(x, torch.float32, "x"), _req(m_out, torch.float32, "m_out")
-    if out is None:
-        out = torch.empty_like(x)
-    check(lib.b200mix_dpmpp_2m_step(_p(eps_u), _p(eps_c), 1 if eps_u.dtype == torch.float32 else 0, float(guidance), _p(x),
-                                    _p(m_prev), _p(out), _p(m_out), x.numel(), float(sigma_cur), float(alpha_cur), float(A),
-                                    float(C), float(halfC), float(inv_r0), _stream()), "b200mix_dpmpp_2m_step")
+    fp32, out = _step_tensors("dpmpp_2m_step", x, eps_u, eps_c, out, m_prev=m_prev, m_out=m_out)
+    check(lib.b200mix_dpmpp_2m_step(_p(eps_u), _p(eps_c), fp32, float(guidance), _p(x), _p(m_prev), _p(out), _p(m_out),
+                                    x.numel(), float(sigma_cur), float(alpha_cur), float(A), float(C), float(halfC),
+                                    float(inv_r0), _stream()), "b200mix_dpmpp_2m_step")
     _count()
     return out
 

@@ -3,7 +3,7 @@
 The index and scalar math runs on the host in numpy float32, operation by operation as the reference does on 0-d
 fp32 tensors (ppdiffusers/schedulers/scheduling_ddim.py:205-238, 305-348, 410-457;
 scheduling_flow_match_euler_discrete.py:64-83, 140-163, 244-275); the elementwise update of the latent runs in one
-fused CUDA kernel (b200mix_ddim_step / b200mix_euler_step) that also folds in the classifier-free-guidance combine.
+fused CUDA kernel (b200mix_ddim_step_ex / b200mix_euler_step) that also folds in the classifier-free-guidance combine.
 tests/test_schedulers.py checks the host scalars bit-for-bit against the oracle.
 """
 import math
@@ -18,6 +18,44 @@ def _betas_for_alpha_bar(n, max_beta=0.999):
     def alpha_bar(t):
         return math.cos((t + 0.008) / 1.008 * math.pi / 2) ** 2
     return np.array([min(1 - alpha_bar((i + 1) / n) / alpha_bar(i / n), max_beta) for i in range(n)], dtype=f32)
+
+
+def _beta_tables(beta_schedule, beta_start, beta_end, n, owner):
+    """betas, alphas = 1 - betas and alphas_cumprod of a training schedule in fp32, as the reference's schedulers build
+    them in __init__ (scheduling_ddim.py:205-238); `owner` is the scheduler class named in the error."""
+    if beta_schedule == "linear":
+        betas = _linspace_f32(beta_start, beta_end, n)
+    elif beta_schedule == "scaled_linear":
+        betas = _linspace_f32(beta_start ** 0.5, beta_end ** 0.5, n) ** 2
+    elif beta_schedule == "squaredcos_cap_v2":
+        betas = _betas_for_alpha_bar(n)
+    else:
+        raise NotImplementedError(f"{beta_schedule} does is not implemented for {owner}")
+    alphas = (f32(1.0) - betas).astype(f32)
+    return betas, alphas, _cumprod_f32(alphas)
+
+
+def _train_sigmas(alphas_cumprod):
+    """((1 - alphas_cumprod) / alphas_cumprod) ** 0.5 in fp32: the sigmas of the training timesteps."""
+    ac = alphas_cumprod
+    return np.sqrt(((f32(1.0) - ac) / ac).astype(f32), dtype=f32)
+
+
+def _karras_sigmas(sigma_min, sigma_max, num_inference_steps, rho=7.0):
+    """Karras et al. (2022) noise levels from sigma_max down to sigma_min, in float64."""
+    ramp = np.linspace(0, 1, num_inference_steps)
+    return (sigma_max ** (1 / rho) + ramp * (sigma_min ** (1 / rho) - sigma_max ** (1 / rho))) ** rho
+
+
+def _sigma_to_t(sigma, log_sigmas):
+    """The (fractional) training timestep of `sigma`, interpolated in log sigma."""
+    log_sigma = np.log(np.maximum(sigma, 1e-10))
+    dists = log_sigma - log_sigmas[:, np.newaxis]
+    low_idx = np.cumsum((dists >= 0), axis=0).argmax(axis=0).clip(max=log_sigmas.shape[0] - 2)
+    high_idx = low_idx + 1
+    low, high = log_sigmas[low_idx], log_sigmas[high_idx]
+    w = np.clip((low - log_sigma) / (low - high), 0, 1)
+    return ((1 - w) * low_idx + w * high_idx).reshape(np.shape(sigma))
 
 
 class DDIMScheduler:
@@ -36,16 +74,8 @@ class DDIMScheduler:
             raise ValueError(f"prediction_type given as {prediction_type} must be one of `epsilon`, `sample`, or"
                              " `v_prediction`")
         self.clip_sample_range = clip_sample_range
-        if beta_schedule == "linear":
-            self.betas = _linspace_f32(beta_start, beta_end, num_train_timesteps)
-        elif beta_schedule == "scaled_linear":
-            self.betas = _linspace_f32(beta_start ** 0.5, beta_end ** 0.5, num_train_timesteps) ** 2
-        elif beta_schedule == "squaredcos_cap_v2":
-            self.betas = _betas_for_alpha_bar(num_train_timesteps)
-        else:
-            raise NotImplementedError(f"{beta_schedule} does is not implemented for {self.__class__}")
-        self.alphas = (f32(1.0) - self.betas).astype(f32)
-        self.alphas_cumprod = _cumprod_f32(self.alphas)
+        self.betas, self.alphas, self.alphas_cumprod = _beta_tables(beta_schedule, beta_start, beta_end,
+                                                                    num_train_timesteps, type(self))
         self.final_alpha_cumprod = f32(1.0) if set_alpha_to_one else self.alphas_cumprod[0]
         self.num_train_timesteps = num_train_timesteps
         self.clip_sample = clip_sample
@@ -103,17 +133,15 @@ class DDIMScheduler:
 
     def step(self, model_output, timestep, sample, eta: float = 0.0, model_output_cond=None, guidance_scale=0.0,
              out=None):
-        """sample, result: fp32 CUDA tensors; model_output: bf16/fp32 CUDA tensor of the same numel (any layout that
-        matches `sample` elementwise). With model_output_cond the CFG combine is fused into the same kernel."""
+        """sample, result: fp32 CUDA tensors; model_output: contiguous bf16/fp32 CUDA tensor with sample's element
+        count, read in sample's element order. With model_output_cond (same dtype) the CFG combine is fused into the same
+        kernel."""
         if eta != 0.0:
             raise NotImplementedError("b200mix DDIM step covers eta = 0 (the deterministic sampler the pipelines use)")
         from .. import ops
         sa_t, sb_t, sa_p, sb_p = self.step_scalars(timestep)
-        if self.prediction_type == "epsilon" and not self.clip_sample:  # the Stable Diffusion configuration
-            return ops.ddim_step(model_output, model_output_cond, guidance_scale, sample, sa_t, sb_t, sa_p, sb_p, out=out)
-        # v_prediction (SD 2.x), sample prediction, clip_sample (scheduling_ddim.py:424-452)
-        return ops.ddim_step_ex(model_output, model_output_cond, guidance_scale, sample, sa_t, sb_t, sa_p, sb_p,
-                                self.prediction_type, self.clip_sample_range if self.clip_sample else 0.0, out=out)
+        return ops.ddim_step(model_output, model_output_cond, guidance_scale, sample, sa_t, sb_t, sa_p, sb_p,
+                             self.prediction_type, self.clip_sample_range if self.clip_sample else 0.0, out=out)
 
 
 class LCMScheduler:
@@ -134,16 +162,8 @@ class LCMScheduler:
         if prediction_type not in ("epsilon", "sample", "v_prediction"):
             raise ValueError(f"prediction_type given as {prediction_type} must be one of `epsilon`, `sample` or"
                              " `v_prediction` for `LCMScheduler`.")
-        if beta_schedule == "linear":
-            self.betas = _linspace_f32(beta_start, beta_end, num_train_timesteps)
-        elif beta_schedule == "scaled_linear":
-            self.betas = _linspace_f32(beta_start ** 0.5, beta_end ** 0.5, num_train_timesteps) ** 2
-        elif beta_schedule == "squaredcos_cap_v2":
-            self.betas = _betas_for_alpha_bar(num_train_timesteps)
-        else:
-            raise NotImplementedError(f"{beta_schedule} does is not implemented for {self.__class__}")
-        self.alphas = (f32(1.0) - self.betas).astype(f32)
-        self.alphas_cumprod = _cumprod_f32(self.alphas)
+        self.betas, self.alphas, self.alphas_cumprod = _beta_tables(beta_schedule, beta_start, beta_end,
+                                                                    num_train_timesteps, type(self))
         self.final_alpha_cumprod = f32(1.0) if set_alpha_to_one else self.alphas_cumprod[0]
         self.num_train_timesteps, self.original_inference_steps = num_train_timesteps, original_inference_steps
         self.clip_sample, self.clip_sample_range = clip_sample, clip_sample_range
@@ -323,33 +343,21 @@ class EulerDiscreteScheduler:
                  beta_schedule: str = "linear", prediction_type: str = "epsilon", interpolation_type: str = "linear",
                  use_karras_sigmas: bool = False, sigma_min: Optional[float] = None, sigma_max: Optional[float] = None,
                  timestep_spacing: str = "linspace", timestep_type: str = "discrete", steps_offset: int = 0):
-        if beta_schedule == "linear":
-            self.betas = _linspace_f32(beta_start, beta_end, num_train_timesteps)
-        elif beta_schedule == "scaled_linear":
-            self.betas = _linspace_f32(beta_start ** 0.5, beta_end ** 0.5, num_train_timesteps) ** 2
-        elif beta_schedule == "squaredcos_cap_v2":
-            self.betas = _betas_for_alpha_bar(num_train_timesteps)
-        else:
-            raise NotImplementedError(f"{beta_schedule} does is not implemented for {self.__class__}")
+        self.betas, self.alphas, self.alphas_cumprod = _beta_tables(beta_schedule, beta_start, beta_end,
+                                                                    num_train_timesteps, type(self))
         if prediction_type != "epsilon":
             raise NotImplementedError("EulerDiscreteScheduler(b200): only prediction_type='epsilon' has a device step")
         if timestep_type != "discrete":
             raise NotImplementedError("EulerDiscreteScheduler(b200): only timestep_type='discrete'")
-        self.alphas = (f32(1.0) - self.betas).astype(f32)
-        self.alphas_cumprod = _cumprod_f32(self.alphas)
         self.num_train_timesteps = num_train_timesteps
         self.interpolation_type, self.use_karras_sigmas = interpolation_type, use_karras_sigmas
         self.sigma_min, self.sigma_max = sigma_min, sigma_max
         self.timestep_spacing, self.steps_offset = timestep_spacing, steps_offset
-        sig = self._train_sigmas()
+        sig = _train_sigmas(self.alphas_cumprod)
         self.timesteps = np.linspace(0, num_train_timesteps - 1, num_train_timesteps, dtype=float)[::-1].astype(f32)
         self.sigmas = np.concatenate([sig[::-1], np.zeros(1, dtype=f32)]).astype(f32)
         self.num_inference_steps: Optional[int] = None
         self._step_index: Optional[int] = None
-
-    def _train_sigmas(self):
-        ac = self.alphas_cumprod
-        return np.sqrt(((f32(1.0) - ac) / ac).astype(f32), dtype=f32)
 
     @property
     def init_noise_sigma(self) -> float:
@@ -374,7 +382,7 @@ class EulerDiscreteScheduler:
         else:
             raise ValueError(f"{self.timestep_spacing} is not supported. Please make sure to choose one of 'linspace', "
                              "'leading' or 'trailing'.")
-        sigmas = self._train_sigmas()
+        sigmas = _train_sigmas(self.alphas_cumprod)
         log_sigmas = np.log(sigmas)
         if self.interpolation_type == "linear":
             sigmas = np.interp(timesteps, np.arange(0, len(sigmas)), sigmas)
@@ -386,23 +394,11 @@ class EulerDiscreteScheduler:
         if self.use_karras_sigmas:
             smin = self.sigma_min if self.sigma_min is not None else sigmas[-1].item()
             smax = self.sigma_max if self.sigma_max is not None else sigmas[0].item()
-            rho = 7.0
-            ramp = np.linspace(0, 1, num_inference_steps)
-            sigmas = (smax ** (1 / rho) + ramp * (smin ** (1 / rho) - smax ** (1 / rho))) ** rho
-            timesteps = np.array([self._sigma_to_t(s, log_sigmas) for s in sigmas])
+            sigmas = _karras_sigmas(smin, smax, num_inference_steps)
+            timesteps = np.array([_sigma_to_t(s, log_sigmas) for s in sigmas])
         self.timesteps = np.asarray(timesteps).astype(f32)
         self.sigmas = np.concatenate([np.asarray(sigmas).astype(f32), np.zeros(1, dtype=f32)])
         self._step_index = None
-
-    @staticmethod
-    def _sigma_to_t(sigma, log_sigmas):
-        log_sigma = np.log(np.maximum(sigma, 1e-10))
-        dists = log_sigma - log_sigmas[:, np.newaxis]
-        low_idx = np.cumsum((dists >= 0), axis=0).argmax(axis=0).clip(max=log_sigmas.shape[0] - 2)
-        high_idx = low_idx + 1
-        low, high = log_sigmas[low_idx], log_sigmas[high_idx]
-        w = np.clip((low - log_sigma) / (low - high), 0, 1)
-        return ((1 - w) * low_idx + w * high_idx).reshape(np.shape(sigma))
 
     def _init_step_index(self, timestep):
         cand = np.nonzero(self.timesteps == f32(timestep))[0]
@@ -461,20 +457,12 @@ class DPMSolverMultistepScheduler:
                  solver_type: str = "midpoint", lower_order_final: bool = True, euler_at_final: bool = False,
                  use_karras_sigmas: bool = False, use_lu_lambdas: bool = False, lambda_min_clipped: float = -float("inf"),
                  variance_type: Optional[str] = None, timestep_spacing: str = "linspace", steps_offset: int = 0):
-        if beta_schedule == "linear":
-            self.betas = _linspace_f32(beta_start, beta_end, num_train_timesteps)
-        elif beta_schedule == "scaled_linear":
-            self.betas = _linspace_f32(beta_start ** 0.5, beta_end ** 0.5, num_train_timesteps) ** 2
-        elif beta_schedule == "squaredcos_cap_v2":
-            self.betas = _betas_for_alpha_bar(num_train_timesteps)
-        else:
-            raise NotImplementedError(f"{beta_schedule} does is not implemented for {self.__class__}")
+        self.betas, self.alphas, self.alphas_cumprod = _beta_tables(beta_schedule, beta_start, beta_end,
+                                                                    num_train_timesteps, type(self))
         if (algorithm_type != "dpmsolver++" or solver_type != "midpoint" or solver_order not in (1, 2) or thresholding or
                 prediction_type != "epsilon" or variance_type):
             raise NotImplementedError("DPMSolverMultistepScheduler(b200): the device step covers dpmsolver++ / midpoint / "
                                       "order 1-2 / epsilon prediction without thresholding")
-        self.alphas = (f32(1.0) - self.betas).astype(f32)
-        self.alphas_cumprod = _cumprod_f32(self.alphas)
         self.num_train_timesteps, self.solver_order = num_train_timesteps, solver_order
         self.lower_order_final, self.euler_at_final = lower_order_final, euler_at_final
         self.use_karras_sigmas, self.use_lu_lambdas = use_karras_sigmas, use_lu_lambdas
@@ -511,21 +499,18 @@ class DPMSolverMultistepScheduler:
         else:
             raise ValueError(f"{self.timestep_spacing} is not supported. Please make sure to choose one of 'linspace', "
                              "'leading' or 'trailing'.")
-        sigmas = np.sqrt(((f32(1.0) - ac) / ac).astype(f32), dtype=f32)
+        sigmas = _train_sigmas(ac)
         log_sigmas = np.log(sigmas)
         if self.use_karras_sigmas:
-            sigmas = np.flip(sigmas).copy()
-            smin, smax, rho = sigmas[-1].item(), sigmas[0].item(), 7.0
-            ramp = np.linspace(0, 1, num_inference_steps)
-            sigmas = (smax ** (1 / rho) + ramp * (smin ** (1 / rho) - smax ** (1 / rho))) ** rho
-            timesteps = np.array([EulerDiscreteScheduler._sigma_to_t(s, log_sigmas) for s in sigmas]).round()
+            sigmas = _karras_sigmas(sigmas[0].item(), sigmas[-1].item(), num_inference_steps)  # training sigmas ascend
+            timesteps = np.array([_sigma_to_t(s, log_sigmas) for s in sigmas]).round()
             sigmas = np.concatenate([sigmas, sigmas[-1:]]).astype(f32)
         elif self.use_lu_lambdas:
             lambdas = np.flip(log_sigmas.copy())
             lmin, lmax = lambdas[-1].item(), lambdas[0].item()
             ramp = np.linspace(0, 1, num_inference_steps)
             sigmas = np.exp(lmax + ramp * (lmin - lmax))
-            timesteps = np.array([EulerDiscreteScheduler._sigma_to_t(s, log_sigmas) for s in sigmas]).round()
+            timesteps = np.array([_sigma_to_t(s, log_sigmas) for s in sigmas]).round()
             sigmas = np.concatenate([sigmas, sigmas[-1:]]).astype(f32)
         else:
             sigmas = np.interp(timesteps, np.arange(0, len(sigmas)), sigmas)
