@@ -147,17 +147,15 @@ def joint_block(x, c, temb, P, p, heads, last):
     return c, x
 
 
-def sd3_forward(cfg, P: Params, hidden_states, encoder_hidden_states, pooled_projections, timestep):
-    """SD3Transformer2DModel.forward, transformer_sd3.py:279-365. hidden_states [B,16,H,W]; timestep [B] float."""
-    ps, heads = cfg["patch_size"], cfg["num_attention_heads"]
+def sd3_embed(cfg, P: Params, hidden_states, encoder_hidden_states, pooled_projections, timestep):
+    """The part of SD3Transformer2DModel.forward before the blocks (transformer_sd3.py:318-324): returns the patch
+    embedding x [B, h*w, D], the context stream c [B, L, D] and temb [B, D]."""
+    ps = cfg["patch_size"]
     B, _, H, W = hidden_states.shape
     # PatchEmbed.forward, embeddings.py:212-247 (conv p x p stride p, flatten, + cropped sincos pos embed)
     x = F.conv2d(hidden_states, P["pos_embed.proj.weight"], P["pos_embed.proj.bias"], stride=ps)
     x = x.flatten(2).transpose(1, 2)
-    h, w, mx = H // ps, W // ps, cfg["pos_embed_max_size"]
-    top, left = (mx - h) // 2, (mx - w) // 2
-    pe = P["pos_embed.pos_embed"].reshape(1, mx, mx, -1)[:, top:top + h, left:left + w, :].reshape(1, h * w, -1)
-    x = x + pe
+    x = x + sd3_pos_embed(cfg, P, H // ps, W // ps)
     # CombinedTimestepTextProjEmbeddings, embeddings.py:530-546
     t = torch.as_tensor(timestep, dtype=torch.float32).reshape(-1).expand(B)
     t_proj = get_timestep_embedding(t, 256, flip_sin_to_cos=True, downscale_freq_shift=0)
@@ -167,15 +165,35 @@ def sd3_forward(cfg, P: Params, hidden_states, encoder_hidden_states, pooled_pro
                    "time_text_embed.text_embedder.linear_2")
     temb = t_emb + p_emb
     c = linear(encoder_hidden_states, P, "context_embedder")
-    for i in range(cfg["num_layers"]):
-        c, x = joint_block(x, c, temb, P, f"transformer_blocks.{i}", heads, i == cfg["num_layers"] - 1)
-    e = linear(F.silu(temb), P, "norm_out.linear")  # AdaLayerNormContinuous (scale, shift)
+    return x, c, temb
+
+
+def sd3_pos_embed(cfg, P: Params, h, w):
+    """PatchEmbed.cropped_pos_embed, embeddings.py:186-210: the centred h x w crop of the max-size table, [1, h*w, D]."""
+    mx = cfg["pos_embed_max_size"]
+    top, left = (mx - h) // 2, (mx - w) // 2
+    return P["pos_embed.pos_embed"].reshape(1, mx, mx, -1)[:, top:top + h, left:left + w, :].reshape(1, h * w, -1)
+
+
+def sd3_final(cfg, P: Params, x, temb, h, w):
+    """norm_out (AdaLayerNormContinuous, (scale, shift)), proj_out and the unpatchify of transformer_sd3.py:345-356."""
+    ps, oc = cfg["patch_size"], cfg["out_channels"]
+    B = x.shape[0]
+    e = linear(F.silu(temb), P, "norm_out.linear")
     scale, shift = e.chunk(2, dim=1)
     x = (_ln(x) + P["norm_out.norm.bias"]) * (1 + scale)[:, None, :] + shift[:, None, :]
     x = linear(x, P, "proj_out")
-    oc = cfg["out_channels"]
-    x = x.reshape(B, h, w, ps, ps, oc).permute(0, 5, 1, 3, 2, 4)  # transformer_sd3.py:350-356
+    x = x.reshape(B, h, w, ps, ps, oc).permute(0, 5, 1, 3, 2, 4)
     return x.reshape(B, oc, h * ps, w * ps)
+
+
+def sd3_forward(cfg, P: Params, hidden_states, encoder_hidden_states, pooled_projections, timestep):
+    """SD3Transformer2DModel.forward, transformer_sd3.py:279-365. hidden_states [B,16,H,W]; timestep [B] float."""
+    ps, heads = cfg["patch_size"], cfg["num_attention_heads"]
+    x, c, temb = sd3_embed(cfg, P, hidden_states, encoder_hidden_states, pooled_projections, timestep)
+    for i in range(cfg["num_layers"]):
+        c, x = joint_block(x, c, temb, P, f"transformer_blocks.{i}", heads, i == cfg["num_layers"] - 1)
+    return sd3_final(cfg, P, x, temb, hidden_states.shape[2] // ps, hidden_states.shape[3] // ps)
 
 
 def sd3_flops(cfg, B, H, W, L):

@@ -106,6 +106,23 @@ def _check_mod_views(op, **mods):
         raise ValueError(f"{op}: {', '.join(given)} must share one row stride, got {sorted(lds)}")
 
 
+def _check_mod_groups(op, rows, rows_per_group, width, **mods):
+    """Row r of the output reads per-group vector r // rows_per_group (one group when rows_per_group is 0), columns
+    0..width-1. A [groups, *] view must cover every group and every column, and a view with several groups used with
+    rows_per_group = 0 would apply its first row to all rows."""
+    for name, v in mods.items():
+        if v is None or v.dim() < 2:
+            if v is not None and v.shape[-1] < width:
+                raise ValueError(f"{op}: {name} has {v.shape[-1]} columns, the output has {width}")
+            continue
+        groups = 1 if rows_per_group <= 0 else -(-rows // rows_per_group)
+        if rows_per_group <= 0 and v.shape[0] > 1:
+            raise ValueError(f"{op}: {name} holds {v.shape[0]} groups but rows_per_group is not set")
+        if v.shape[0] < groups or v.shape[-1] < width:
+            raise ValueError(f"{op}: {name} of shape {tuple(v.shape)} does not cover {groups} groups x {width} columns "
+                             f"({rows} rows, rows_per_group {rows_per_group})")
+
+
 def make_epilogue(bias=None, row_add=None, row_gate=None, ld_row=0, rows_per_group=0, residual=None, ldr=0,
                   act=ACT_NONE, glu=GLU_NONE, out_fp32=False, out_scale=1.0, residual_row_mod=0, stats_out=None,
                   ln=None) -> Epilogue:
@@ -251,6 +268,8 @@ def linear(a: torch.Tensor, w, bias=None, *, act=ACT_NONE, glu=GLU_NONE, residua
         return _linear_w8(a, w, bias, act, glu, residual, out_fp32, out)
     _req(a, bf16, "a"), _req(w, bf16, "w")
     K = a.shape[-1]
+    if w.dim() != 2 or w.shape[1] != K:
+        raise ValueError(f"linear: weight must be [N, {K}] for an input with {K} features, got {tuple(w.shape)}")
     a2 = a.reshape(-1, K)
     if a2.stride(-1) != 1:
         a2 = a2.contiguous()
@@ -264,6 +283,7 @@ def linear(a: torch.Tensor, w, bias=None, *, act=ACT_NONE, glu=GLU_NONE, residua
     mod = row_add if row_add is not None else row_gate
     if mod is not None:
         _check_mod_views("linear", row_add=row_add, row_gate=row_gate)
+        _check_mod_groups("linear", M, rows_per_group, N, row_add=row_add, row_gate=row_gate)
     rs = None
     want_stats = stats is not None and stats is not False
     if want_stats:
@@ -292,10 +312,19 @@ def linear_batched(a: torch.Tensor, w: torch.Tensor, bias=None, *, out: torch.Te
     _req(a, bf16, "a"), _req(w, bf16, "w")
     B, rows, K = a.shape
     N = w.shape[0]
-    assert a.stride(-1) == 1 and out.stride(-1) == 1 and out.shape[0] == B and out.shape[1] == rows
+    if w.dim() != 2 or w.shape[1] != K:
+        raise ValueError(f"linear_batched: weight must be [N, {K}] for an input with {K} features, got {tuple(w.shape)}")
+    n_out = N // 2 if glu else N
+    if out.dim() != 3 or tuple(out.shape) != (B, rows, n_out):
+        raise ValueError(f"linear_batched: out must be [{B}, {rows}, {n_out}], got {tuple(out.shape)}")
+    if residual is not None and tuple(residual.shape) != tuple(out.shape):
+        raise ValueError(f"linear_batched: residual must be {tuple(out.shape)}, got {tuple(residual.shape)}")
+    if a.stride(-1) != 1 or out.stride(-1) != 1 or (residual is not None and residual.stride(-1) != 1):
+        raise ValueError("linear_batched: a, out and residual need a contiguous last dimension")
     mod = row_add if row_add is not None else row_gate
     if mod is not None:
         _check_mod_views("linear_batched", row_add=row_add, row_gate=row_gate)
+        _check_mod_groups("linear_batched", B * rows, rows, n_out, row_add=row_add, row_gate=row_gate)
     e = make_epilogue(bias=bias, row_add=row_add, row_gate=row_gate, ld_row=0 if mod is None else mod.stride(0),
                       rows_per_group=rows, residual=residual, ldr=0 if residual is None else residual.stride(1),
                       act=act, glu=glu, out_fp32=(out.dtype == torch.float32))
@@ -498,6 +527,7 @@ def layernorm(x: torch.Tensor, weight=None, bias=None, *, eps=1e-5, rms=False, d
     mod = gate if gate is not None else (scale if scale is not None else shift)
     if mod is not None:
         _check_mod_views("layernorm", gate=gate, scale=scale, shift=shift)
+        _check_mod_groups("layernorm", M, rows_per_group, N, gate=gate, scale=scale, shift=shift)
     ld_mod = 0 if mod is None else mod.stride(0)
     nbytes = 2.0 * M * N * (2 + (1 if delta is not None else 0) + (1 if resid is not None else 0))
     with _Timed("layernorm", nbytes, "byte", lambda: f"ln {M}x{N}" + (" +delta" if delta is not None else "")):

@@ -402,7 +402,9 @@ class StableDiffusion3Pipeline:
                 raise ValueError("height/width (or latents) are required")
             g = generator or torch.Generator().manual_seed(0)
             latents = torch.randn(B, tr.config.in_channels, height // 8, width // 8, generator=g)
-        latents = latents.to(device=dev, dtype=torch.float32).contiguous()
+        # always a copy: the loop alternates between two buffers and would otherwise write its steps into the
+        # caller's tensor when that is already an fp32 tensor on the device
+        latents = latents.to(device=dev, dtype=torch.float32, copy=True).contiguous()
         ctx, pooled = prompt_embeds.to(device=dev, dtype=bf16), pooled_prompt_embeds.to(device=dev, dtype=bf16)
         if do_cfg:
             if negative_prompt_embeds is None:

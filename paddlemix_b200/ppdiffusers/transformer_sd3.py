@@ -160,20 +160,13 @@ class SD3Transformer2DModel:
             self._pos_cache[key] = t
         return t
 
-    def forward(self, hidden_states, encoder_hidden_states=None, pooled_projections=None, timestep=None,
-                joint_attention_kwargs: Optional[Dict[str, Any]] = None, return_dict: bool = True):
-        """Same signature as the reference (transformer_sd3.py:279-287). hidden_states [B,C,H,W] (fp32 / bf16),
-        encoder_hidden_states [B,L,joint_attention_dim], pooled_projections [B,pooled_dim], timestep [B] or scalar."""
+    def _embed(self, hidden_states, encoder_hidden_states, pooled_projections, timestep):
+        """PatchEmbed, CombinedTimestepTextProjEmbeddings, the context embedder and the one GEMM for every AdaLN
+        projection. Returns (x [B, n, D] bf16, context stream [B, L, D] bf16, temb [B, D] bf16, mod [B, sum] fp32,
+        (h, w))."""
         from .. import ops
-        from .._lib import ACT_GELU_TANH, ACT_SILU
-        if self.device is None:
-            raise RuntimeError("load_state_dict() must be called before forward()")
-        if joint_attention_kwargs:
-            extra = {k: v for k, v in joint_attention_kwargs.items() if k != "scale"}
-            if extra:
-                raise NotImplementedError(f"joint_attention_kwargs {list(extra)} are outside the hot path")
-        dev, c, D = self.device, self.config, self.inner_dim
-        Hh, hd = c.num_attention_heads, c.attention_head_dim
+        from .._lib import ACT_SILU
+        dev, c = self.device, self.config
         x_in = hidden_states.to(dev)
         if x_in.dtype not in (torch.float32, bf16):
             x_in = x_in.float()
@@ -182,7 +175,6 @@ class SD3Transformer2DModel:
         h, w = H // ps, Wd // ps
         n = h * w
         ctx = encoder_hidden_states.to(device=dev, dtype=bf16).contiguous()
-        L = ctx.shape[1]
         pooled = pooled_projections.to(device=dev, dtype=bf16).contiguous()
         t = timestep if torch.is_tensor(timestep) else torch.tensor([float(timestep)])
         t = t.to(device=dev, dtype=torch.float32).reshape(-1)
@@ -199,38 +191,68 @@ class SD3Transformer2DModel:
         temb = ops.linear(ops.linear(pooled, *self.p1, act=ACT_SILU), *self.p2, residual=t_emb)
         mod = ops.linear(ops.activation(temb, ACT_SILU), self.mod_w, self.mod_b, out_fp32=True)  # [B, sum] fp32
         cst = ops.linear(ctx, *self.ctx_emb)  # [B, L, D]
+        return x, cst, temb, mod, (h, w)
 
-        S = n + L
-        for blk in self.blocks:
-            last = blk["last"]
-            m1 = mod[:, blk["norm1_off"]:]
-            # AdaLayerNormZero chunk order: shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp
-            nx = ops.layernorm(x, eps=1e-6, scale=m1[:, D:], shift=m1[:, 0:], rows_per_group=n)
-            mc = mod[:, blk["norm1_context_off"]:]
-            if last:  # AdaLayerNormContinuous: (scale, shift); its LayerNorm carries a bias and no weight
-                nc = ops.layernorm(cst, None, blk["ctx_ln_bias"], eps=1e-6, scale=mc[:, 0:], shift=mc[:, D:], rows_per_group=L)
-            else:
-                nc = ops.layernorm(cst, eps=1e-6, scale=mc[:, D:], shift=mc[:, 0:], rows_per_group=L)
-            qkv = torch.empty(B, S, 3 * D, device=dev, dtype=bf16)
-            ops.linear_batched(nx, blk["w_qkv"], blk["b_qkv"], out=qkv[:, :n])
-            ops.linear_batched(nc, blk["w_cqkv"], blk["b_cqkv"], out=qkv[:, n:])
-            q, k, v = (qkv[:, :, i * D:(i + 1) * D].unflatten(-1, (Hh, hd)) for i in range(3))
-            o = ops.sdpa(q, k, v, scale=hd ** -0.5).reshape(B, S, D)
-            x_new = torch.empty_like(x)
-            ops.linear_batched(o[:, :n], blk["w_o"], blk["b_o"], out=x_new, row_gate=m1[:, 2 * D:], residual=x)
-            nx2 = ops.layernorm(x_new, eps=1e-6, scale=m1[:, 4 * D:], shift=m1[:, 3 * D:], rows_per_group=n)
-            ff = ops.linear(nx2, *blk["ff1"], act=ACT_GELU_TANH)
-            x = ops.linear(ff, *blk["ff2"], row_gate=m1[:, 5 * D:], rows_per_group=n, residual=x_new)
-            if not last:
-                c_new = torch.empty_like(cst)
-                ops.linear_batched(o[:, n:], blk["w_co"], blk["b_co"], out=c_new, row_gate=mc[:, 2 * D:], residual=cst)
-                nc2 = ops.layernorm(c_new, eps=1e-6, scale=mc[:, 4 * D:], shift=mc[:, 3 * D:], rows_per_group=L)
-                cff = ops.linear(nc2, *blk["cff1"], act=ACT_GELU_TANH)
-                cst = ops.linear(cff, *blk["cff2"], row_gate=mc[:, 5 * D:], rows_per_group=L, residual=c_new)
+    def _block(self, i, x, cst, mod, n, L):
+        """JointTransformerBlock i on the image stream x [B, n, D] and the context stream cst [B, L, D], with its AdaLN
+        vectors read from mod. Returns (x, cst); the last block (context_pre_only) returns cst unchanged."""
+        from .. import ops
+        from .._lib import ACT_GELU_TANH
+        c, D = self.config, self.inner_dim
+        Hh, hd = c.num_attention_heads, c.attention_head_dim
+        B, S = x.shape[0], n + L
+        blk = self.blocks[i]
+        last = blk["last"]
+        m1 = mod[:, blk["norm1_off"]:]
+        # AdaLayerNormZero chunk order: shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp
+        nx = ops.layernorm(x, eps=1e-6, scale=m1[:, D:], shift=m1[:, 0:], rows_per_group=n)
+        mc = mod[:, blk["norm1_context_off"]:]
+        if last:  # AdaLayerNormContinuous: (scale, shift); its LayerNorm carries a bias and no weight
+            nc = ops.layernorm(cst, None, blk["ctx_ln_bias"], eps=1e-6, scale=mc[:, 0:], shift=mc[:, D:], rows_per_group=L)
+        else:
+            nc = ops.layernorm(cst, eps=1e-6, scale=mc[:, D:], shift=mc[:, 0:], rows_per_group=L)
+        qkv = torch.empty(B, S, 3 * D, device=x.device, dtype=bf16)
+        ops.linear_batched(nx, blk["w_qkv"], blk["b_qkv"], out=qkv[:, :n])
+        ops.linear_batched(nc, blk["w_cqkv"], blk["b_cqkv"], out=qkv[:, n:])
+        q, k, v = (qkv[:, :, j * D:(j + 1) * D].unflatten(-1, (Hh, hd)) for j in range(3))
+        o = ops.sdpa(q, k, v, scale=hd ** -0.5).reshape(B, S, D)
+        x_new = torch.empty_like(x)
+        ops.linear_batched(o[:, :n], blk["w_o"], blk["b_o"], out=x_new, row_gate=m1[:, 2 * D:], residual=x)
+        nx2 = ops.layernorm(x_new, eps=1e-6, scale=m1[:, 4 * D:], shift=m1[:, 3 * D:], rows_per_group=n)
+        ff = ops.linear(nx2, *blk["ff1"], act=ACT_GELU_TANH)
+        x = ops.linear(ff, *blk["ff2"], row_gate=m1[:, 5 * D:], rows_per_group=n, residual=x_new)
+        if not last:
+            c_new = torch.empty_like(cst)
+            ops.linear_batched(o[:, n:], blk["w_co"], blk["b_co"], out=c_new, row_gate=mc[:, 2 * D:], residual=cst)
+            nc2 = ops.layernorm(c_new, eps=1e-6, scale=mc[:, 4 * D:], shift=mc[:, 3 * D:], rows_per_group=L)
+            cff = ops.linear(nc2, *blk["cff1"], act=ACT_GELU_TANH)
+            cst = ops.linear(cff, *blk["cff2"], row_gate=mc[:, 5 * D:], rows_per_group=L, residual=c_new)
+        return x, cst
+
+    def _final(self, x, mod, h, w):
+        """norm_out (AdaLayerNormContinuous), proj_out and unpatchify: bf16 [B, out_channels, h*p, w*p]."""
+        from .. import ops
+        D, n = self.inner_dim, h * w
         mo = mod[:, self.norm_out_off:]
         xn = ops.layernorm(x, None, self.norm_out_bias, eps=1e-6, scale=mo[:, 0:], shift=mo[:, D:], rows_per_group=n)
         y = ops.linear(xn, *self.proj_out)  # [B, n, p*p*oc]
-        out = ops.unpatchify(y, self.out_channels, h, w, ps, out_dtype=bf16)
+        return ops.unpatchify(y, self.out_channels, h, w, self.config.patch_size, out_dtype=bf16)
+
+    def forward(self, hidden_states, encoder_hidden_states=None, pooled_projections=None, timestep=None,
+                joint_attention_kwargs: Optional[Dict[str, Any]] = None, return_dict: bool = True):
+        """Same signature as the reference (transformer_sd3.py:279-287). hidden_states [B,C,H,W] (fp32 / bf16),
+        encoder_hidden_states [B,L,joint_attention_dim], pooled_projections [B,pooled_dim], timestep [B] or scalar."""
+        if self.device is None:
+            raise RuntimeError("load_state_dict() must be called before forward()")
+        if joint_attention_kwargs:
+            extra = {k: v for k, v in joint_attention_kwargs.items() if k != "scale"}
+            if extra:
+                raise NotImplementedError(f"joint_attention_kwargs {list(extra)} are outside the hot path")
+        x, cst, _, mod, (h, w) = self._embed(hidden_states, encoder_hidden_states, pooled_projections, timestep)
+        n, L = h * w, cst.shape[1]
+        for i in range(len(self.blocks)):
+            x, cst = self._block(i, x, cst, mod, n, L)
+        out = self._final(x, mod, h, w)
         if not return_dict:
             return (out,)
         return Transformer2DModelOutput(sample=out)
