@@ -56,7 +56,8 @@ class STDiT2:
     def __init__(self, config: Union[STDiT2Config, Dict[str, Any]]):
         self.config = config if isinstance(config, STDiT2Config) else STDiT2Config(**config)
         c = self.config
-        assert c.hidden_size % 3 == 0, "hidden_size must be divisible by 3"
+        if c.hidden_size % 3:
+            raise ValueError(f"STDiT2: hidden_size {c.hidden_size} must be divisible by 3")
         if c.patch_size[0] != 1 or c.patch_size[1] != c.patch_size[2]:
             raise NotImplementedError("STDiT2(b200): patch_size must be (1, p, p)")
         self.head_dim = c.hidden_size // c.num_heads

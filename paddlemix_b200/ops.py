@@ -78,12 +78,65 @@ def _p(t: Optional[torch.Tensor]):
     return None if t is None else ctypes.c_void_p(t.data_ptr())
 
 
-def _req(t, dtype, name):
-    if not t.is_cuda:
-        raise _lib.B200MixError(f"{name} must be a CUDA tensor (b200mix has no CPU path)")
-    if t.dtype != dtype:
-        raise TypeError(f"{name} must be {dtype}, got {t.dtype}")
-    return t
+def _launch(name, *args, kernels=1):
+    """Calls lib.<name>(*args, stream) with tensors passed as their device pointers; raises if it fails and adds the
+    `kernels` it starts to launches()."""
+    check(getattr(lib, name)(*(_p(a) if isinstance(a, torch.Tensor) else a for a in args), _stream()), name)
+    _count(kernels)
+
+
+F32, BF16, FLOAT, I32, I64 = (torch.float32,), (bf16,), (torch.float32, bf16), (torch.int32,), (torch.int64,)
+CONTIG = "contiguous"   # read flat: only a pointer reaches the kernel
+STRIDED = "strided"     # the last dimension contiguous; the other strides are passed on
+ROWS = "rows"           # STRIDED, with the passed strides multiples of 8 elements (16-byte TMA / vector strides)
+
+
+def _fits(shape, want):
+    if ... in want:
+        i = want.index(...)
+        head, tail = want[:i], want[i + 1:]
+        return (len(shape) >= len(head) + len(tail) and _fits(shape[:i], head)
+                and _fits(shape[len(shape) - len(tail):], tail))
+    return len(shape) == len(want) and all(w is None or s == w for s, w in zip(shape, want))
+
+
+class _Args:
+    """The tensors one call hands its kernels, checked against what the kernels read. The kernels see pointers and
+    the sizes and strides passed beside them, never the tensors, so these checks are what keeps a caller's mistake from
+    becoming an out-of-bounds access. c(name, t, dtypes, shape, layout, numel) checks one tensor (None passes) and
+    returns its shape; shape entries are sizes, None for any size, and at most one ... for any number of dimensions;
+    layout None leaves the layout to the wrapper, which copies the tensor or checks it itself. c.on_cuda() then checks that every tensor seen is on the device: placement comes last, so CPU tensors reach every
+    other refusal."""
+
+    def __init__(self, op):
+        self.op, self.seen = op, []
+
+    def __call__(self, name, t, dtypes, shape=None, layout=CONTIG, numel=None):
+        if t is None:
+            return None
+        op = self.op
+        if t.dtype not in dtypes:
+            raise TypeError(f"{op}: {name} must be {' or '.join(map(str, dtypes))}, got {t.dtype}")
+        if layout == CONTIG and not t.is_contiguous():
+            raise ValueError(f"{op}: {name} must be contiguous, got strides {t.stride()} for shape {tuple(t.shape)}")
+        elif layout is not None and t.dim() and (
+                (t.shape[-1] > 1 and t.stride(-1) != 1) or
+                (layout == ROWS and any(s % 8 for n, s in zip(t.shape[:-1], t.stride()) if n > 1))):
+            raise ValueError(f"{op}: {name} needs a contiguous last dimension"
+                             f"{' and strides that are multiples of 8' if layout == ROWS else ''}, got strides "
+                             f"{t.stride()} for shape {tuple(t.shape)}")
+        if shape is not None and not _fits(t.shape, shape):
+            want = ", ".join("..." if s is ... else "*" if s is None else str(s) for s in shape)
+            raise ValueError(f"{op}: {name} must be [{want}], got {tuple(t.shape)}")
+        if numel is not None and t.numel() != numel:
+            raise ValueError(f"{op}: {name} has {t.numel()} elements, expected {numel}")
+        self.seen.append((name, t))
+        return t.shape
+
+    def on_cuda(self):
+        for name, t in self.seen:
+            if not t.is_cuda:
+                raise _lib.B200MixError(f"{self.op}: {name} must be a CUDA tensor (b200mix has no CPU path)")
 
 
 def init(device: int = 0):
@@ -126,24 +179,21 @@ def _check_mod_groups(op, rows, rows_per_group, width, **mods):
 def make_epilogue(bias=None, row_add=None, row_gate=None, ld_row=0, rows_per_group=0, residual=None, ldr=0,
                   act=ACT_NONE, glu=GLU_NONE, out_fp32=False, out_scale=1.0, residual_row_mod=0, stats_out=None,
                   ln=None) -> Epilogue:
+    """The epilogue struct of tensors the calling wrapper has checked."""
+    ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
     e = Epilogue()
-    e.bias = None if bias is None else _req(bias, torch.float32, "bias").data_ptr()
-    e.row_add = None if row_add is None else _req(row_add, torch.float32, "row_add").data_ptr()
-    e.row_gate = None if row_gate is None else _req(row_gate, torch.float32, "row_gate").data_ptr()
+    e.bias, e.row_add, e.row_gate, e.residual, e.stats_out = map(ptr, (bias, row_add, row_gate, residual, stats_out))
     e.ld_row = int(ld_row)
     e.rows_per_group = int(rows_per_group)
-    e.residual = None if residual is None else _req(residual, bf16, "residual").data_ptr()
     e.ldr = int(ldr)
     e.act = int(act)
     e.glu = int(glu)
     e.out_fp32 = 1 if out_fp32 else 0
     e.out_scale = float(out_scale)
     e.residual_row_mod = int(residual_row_mod)
-    e.stats_out = None if stats_out is None else _req(stats_out, torch.int64, "stats_out").data_ptr()
     if ln is not None:  # folded LayerNorm, consumer side: (RowStats of the input rows, colsum [N] fp32, eps[, rms])
         stats, colsum, eps = ln[:3]
-        e.ln_stats = _req(stats.buf, torch.int64, "ln_stats").data_ptr()
-        e.ln_colsum = _req(colsum, torch.float32, "ln_colsum").data_ptr()
+        e.ln_stats, e.ln_colsum = stats.buf.data_ptr(), colsum.data_ptr()
         e.ln_eps, e.ln_rms = float(eps), int(bool(ln[3])) if len(ln) > 3 else 0
     return e
 
@@ -161,7 +211,7 @@ class RowStats:
     def arena(n: int, rows: int, device) -> torch.Tensor:
         """n zeroed [rows, 2] tables in one allocation / one memset (a transformer stack takes 1 + 3 per block)."""
         buf = torch.empty(n, rows, 2, device=device, dtype=torch.int64)
-        check(lib.b200mix_zero_bytes(_p(buf), buf.numel() * 8, _stream()), "b200mix_zero_bytes")
+        check(lib.b200mix_zero_bytes(_p(buf), buf.numel() * 8, _stream()), "b200mix_zero_bytes")  # a memset, not a kernel
         return buf
 
     def mean_rstd(self, eps: float):
@@ -208,45 +258,62 @@ def quantize_w8(w: torch.Tensor, workspace: Optional[torch.Tensor]) -> Int8Weigh
     """Weight-only int8 of w fp32 or bf16 [N, K] on the device (N % 16 == 0, K % 64 == 0): per row scale = absmax / 127,
     q = clip(round(w / scale), -127, 127), rounding half away from zero; an all-zero row gets scale 0. workspace: bf16
     with at least N * K elements, or None."""
-    if w.dtype not in (torch.float32, bf16):
-        raise TypeError(f"quantize_w8 takes an fp32 or bf16 weight, got {w.dtype}")
-    _req(w, w.dtype, "w")
-    if w.dim() != 2:
-        raise ValueError(f"quantize_w8 takes a [N, K] weight, got {tuple(w.shape)}")
-    N, K = w.shape
-    if workspace is not None and (_req(workspace, bf16, "workspace").numel() < N * K):
-        raise ValueError(f"the workspace holds {workspace.numel()} bf16 elements, a [{N}, {K}] weight needs {N * K}")
+    c = _Args("quantize_w8")
+    N, K = c("w", w, FLOAT, (None, None), layout=None)
+    c("workspace", workspace, BF16)
+    if workspace is not None and workspace.numel() < N * K:
+        raise ValueError(f"quantize_w8: the workspace holds {workspace.numel()} bf16 elements, a [{N}, {K}] weight "
+                         f"needs {N * K}")
+    c.on_cuda()
     w = w.contiguous()
     q = torch.empty(N * K, device=w.device, dtype=torch.int8)
     scale = torch.empty(N, device=w.device, dtype=torch.float32)
-    check(lib.b200mix_quantize_w8(_p(w), 1 if w.dtype == torch.float32 else 0, _p(q), _p(scale), N, K, _stream()),
-          "b200mix_quantize_w8")
-    _count()
+    _launch("b200mix_quantize_w8", w, 1 if w.dtype == torch.float32 else 0, q, scale, N, K)
     return Int8Weight(q, scale, N, K, workspace)
 
 
-def _linear_w8(a, w: Int8Weight, bias, act, glu, residual, out_fp32, out):
-    _req(a, bf16, "a")
-    K = a.shape[-1]
-    if K != w.K:
-        raise ValueError(f"input has {K} features, the weight takes {w.K}")
+def _linear_io(c, a, K, n_out, out_fp32, out, residual, residual_row_mod):
+    """Checks linear's a [..., K], out [..., n_out] and residual [rows, >= n_out] (rows >= M, or >= residual_row_mod
+    when that is set). Returns a as a [M, K] matrix and out as the [M, n_out] view the kernel writes (None if out is)."""
+    c("a", a, BF16, (..., K), layout=None)
     a2 = a.reshape(-1, K)
+    M = a2.shape[0]
+    c("out", out, F32 if out_fp32 else BF16, (..., n_out), STRIDED, numel=M * n_out)
+    try:
+        out2 = None if out is None else out.view(-1, n_out)
+    except RuntimeError:
+        raise ValueError(f"{c.op}: out of shape {tuple(out.shape)} and strides {out.stride()} cannot be viewed as "
+                         f"[{M}, {n_out}]") from None
+    res2 = None if residual is None else residual.reshape(-1, residual.shape[-1])
+    c("residual", res2, BF16, (None, None), STRIDED)
+    rows = residual_row_mod or M
+    if res2 is not None and (res2.shape[0] < rows or res2.shape[1] < n_out):
+        raise ValueError(f"{c.op}: residual of shape {tuple(residual.shape)} does not cover {rows} rows x {n_out} "
+                         f"columns")
+    return a2, out2, res2
+
+
+def _linear_w8(a, w: Int8Weight, bias, act, glu, residual, out_fp32, out):
+    c = _Args("linear")
+    N, K = w.N, w.K
+    n_out = N // 2 if glu else N
+    a2, out2, res2 = _linear_io(c, a, K, n_out, out_fp32, out, residual, 0)
+    c("bias", bias, F32, numel=N)
+    c.on_cuda()
     if a2.stride(-1) != 1 or a2.data_ptr() % 16 or a2.stride(0) % 8:
         a2 = a2.contiguous()
-    M, N = a2.shape[0], w.N
-    n_out = N // 2 if glu else N
+    M = a2.shape[0]
     if out is None:
         out = torch.empty(*a.shape[:-1], n_out, device=a.device, dtype=torch.float32 if out_fp32 else bf16)
-    res2 = None if residual is None else residual.reshape(-1, residual.shape[-1])
+        out2 = out.view(-1, n_out)
     e = make_epilogue(bias=bias, residual=res2, ldr=0 if res2 is None else res2.stride(0), act=act, glu=glu,
                       out_fp32=out_fp32)
-    out2 = out.reshape(-1, n_out)
     ws = w.workspace
+    need = ctypes.c_int64(0)  # above the weight-streaming range, the weight is expanded to bf16 first: two kernels
+    check(lib.b200mix_linear_w8_workspace_size(M, N, K, ctypes.byref(need)), "b200mix_linear_w8_workspace_size")
     with _Timed("w8gemm", 2.0 * M * N * K, "flop", lambda: f"w8 {M}x{N}x{K}" + _epi_tag(e)):
-        check(lib.b200mix_linear_w8(_p(a2), a2.stride(0), _p(w.q), _p(w.scale), _p(out2), out2.stride(0), M, N, K,
-                                    ctypes.byref(e), _p(ws), 0 if ws is None else 2 * ws.numel(), _stream()),
-              "b200mix_linear_w8")
-    _count()
+        _launch("b200mix_linear_w8", a2, a2.stride(0), w.q, w.scale, out2, out2.stride(0), M, N, K, ctypes.byref(e), ws,
+                0 if ws is None else 2 * ws.numel(), kernels=2 if need.value else 1)
     return out
 
 
@@ -266,42 +333,38 @@ def linear(a: torch.Tensor, w, bias=None, *, act=ACT_NONE, glu=GLU_NONE, residua
         if unsupported:
             raise ValueError(f"an Int8Weight linear does not support {', '.join(unsupported)}")
         return _linear_w8(a, w, bias, act, glu, residual, out_fp32, out)
-    _req(a, bf16, "a"), _req(w, bf16, "w")
+    c = _Args("linear")
     K = a.shape[-1]
-    if w.dim() != 2 or w.shape[1] != K:
-        raise ValueError(f"linear: weight must be [N, {K}] for an input with {K} features, got {tuple(w.shape)}")
-    a2 = a.reshape(-1, K)
-    if a2.stride(-1) != 1:
-        a2 = a2.contiguous()
-    M, N = a2.shape[0], w.shape[0]
+    N = c("weight", w, BF16, (None, K), ROWS)[0]
     n_out = N // 2 if glu else N
-    if out is None:
-        out = torch.empty(*a.shape[:-1], n_out, device=a.device, dtype=torch.float32 if out_fp32 else bf16)
-    res2 = None
-    if residual is not None:
-        res2 = residual.reshape(-1, residual.shape[-1])
+    a2, out2, res2 = _linear_io(c, a, K, n_out, out_fp32, out, residual, residual_row_mod)
+    M = a2.shape[0]
+    c("bias", bias, F32, numel=N)
+    c("row_add", row_add, F32, layout=None), c("row_gate", row_gate, F32, layout=None)
     mod = row_add if row_add is not None else row_gate
     if mod is not None:
         _check_mod_views("linear", row_add=row_add, row_gate=row_gate)
         _check_mod_groups("linear", M, rows_per_group, N, row_add=row_add, row_gate=row_gate)
-    rs = None
     want_stats = stats is not None and stats is not False
-    if want_stats:
-        buf = RowStats.arena(1, M, a.device)[0] if stats is True else stats
-        if tuple(buf.shape) != (M, 2):
-            raise ValueError(f"stats table must be int64 [{M}, 2], got {tuple(buf.shape)}")
-        rs = RowStats(buf, N)
-    if ln is not None and (ln[0].buf.shape[0] != M or ln[0].width != K):
-        raise ValueError(f"row statistics are for a [{ln[0].buf.shape[0]}, {ln[0].width}] tensor, the input is [{M}, {K}]")
+    if want_stats and stats is not True:
+        c("stats", stats, I64, (M, 2))
+    if ln is not None:
+        if ln[0].buf.shape[0] != M or ln[0].width != K:
+            raise ValueError(f"row statistics are for a [{ln[0].buf.shape[0]}, {ln[0].width}] tensor, the input is [{M}, {K}]")
+        c("ln stats", ln[0].buf, I64, (M, 2)), c("ln colsum", ln[1], F32, numel=N)
+    c.on_cuda()
+    if a2.stride(-1) != 1:
+        a2 = a2.contiguous()
+    if out is None:
+        out = torch.empty(*a.shape[:-1], n_out, device=a.device, dtype=torch.float32 if out_fp32 else bf16)
+        out2 = out.view(-1, n_out)
+    rs = RowStats(RowStats.arena(1, M, a.device)[0] if stats is True else stats, N) if want_stats else None
     e = make_epilogue(bias=bias, row_add=row_add, row_gate=row_gate, ld_row=0 if mod is None else mod.stride(0),
                       rows_per_group=rows_per_group, residual=res2, ldr=0 if res2 is None else res2.stride(0), act=act,
                       glu=glu, out_fp32=out_fp32, out_scale=out_scale, residual_row_mod=residual_row_mod,
                       stats_out=None if rs is None else rs.buf, ln=ln)
-    out2 = out.reshape(-1, n_out)
     with _Timed("igemm", 2.0 * M * N * K, "flop", lambda: f"lin {M}x{N}x{K}" + _epi_tag(e)):
-        check(lib.b200mix_linear(_p(a2), a2.stride(0), _p(w), w.stride(0), _p(out2), out2.stride(0), M, N, K,
-                                 ctypes.byref(e), _stream()), "b200mix_linear")
-    _count()
+        _launch("b200mix_linear", a2, a2.stride(0), w, w.stride(0), out2, out2.stride(0), M, N, K, ctypes.byref(e))
     return (out, rs) if want_stats else out
 
 
@@ -309,73 +372,68 @@ def linear_batched(a: torch.Tensor, w: torch.Tensor, bias=None, *, out: torch.Te
                    residual=None, row_add=None, row_gate=None) -> torch.Tensor:
     """a: bf16 [B, rows, K] view (last dim contiguous, arbitrary row / batch strides); out: [B, rows, N(/2)] view with
     last dim contiguous (e.g. a token range of a joint [B, n_img+n_txt, *] buffer). Per-batch row_add / row_gate."""
-    _req(a, bf16, "a"), _req(w, bf16, "w")
-    B, rows, K = a.shape
-    N = w.shape[0]
-    if w.dim() != 2 or w.shape[1] != K:
-        raise ValueError(f"linear_batched: weight must be [N, {K}] for an input with {K} features, got {tuple(w.shape)}")
+    c = _Args("linear_batched")
+    B, rows, K = c("a", a, BF16, (None, None, None), ROWS)
+    N = c("weight", w, BF16, (None, K), ROWS)[0]
     n_out = N // 2 if glu else N
-    if out.dim() != 3 or tuple(out.shape) != (B, rows, n_out):
-        raise ValueError(f"linear_batched: out must be [{B}, {rows}, {n_out}], got {tuple(out.shape)}")
-    if residual is not None and tuple(residual.shape) != tuple(out.shape):
-        raise ValueError(f"linear_batched: residual must be {tuple(out.shape)}, got {tuple(residual.shape)}")
-    if a.stride(-1) != 1 or out.stride(-1) != 1 or (residual is not None and residual.stride(-1) != 1):
-        raise ValueError("linear_batched: a, out and residual need a contiguous last dimension")
+    c("out", out, FLOAT, (B, rows, n_out), STRIDED)
+    c("residual", residual, BF16, (B, rows, n_out), STRIDED)
+    c("bias", bias, F32, numel=N)
+    c("row_add", row_add, F32, layout=None), c("row_gate", row_gate, F32, layout=None)
     mod = row_add if row_add is not None else row_gate
     if mod is not None:
         _check_mod_views("linear_batched", row_add=row_add, row_gate=row_gate)
         _check_mod_groups("linear_batched", B * rows, rows, n_out, row_add=row_add, row_gate=row_gate)
+    c.on_cuda()
     e = make_epilogue(bias=bias, row_add=row_add, row_gate=row_gate, ld_row=0 if mod is None else mod.stride(0),
                       rows_per_group=rows, residual=residual, ldr=0 if residual is None else residual.stride(1),
                       act=act, glu=glu, out_fp32=(out.dtype == torch.float32))
     with _Timed("igemm", 2.0 * B * rows * N * K, "flop", lambda: f"linb {B}*{rows}x{N}x{K}" + _epi_tag(e)):
-        check(lib.b200mix_linear_batched(_p(a), a.stride(1), a.stride(0), _p(w), w.stride(0), _p(out), out.stride(1),
-                                         out.stride(0), rows, B, N, K, ctypes.byref(e),
-                                         0 if residual is None else residual.stride(0), _stream()),
-              "b200mix_linear_batched")
-    _count()
+        _launch("b200mix_linear_batched", a, a.stride(1), a.stride(0), w, w.stride(0), out, out.stride(1), out.stride(0),
+                rows, B, N, K, ctypes.byref(e), 0 if residual is None else residual.stride(0))
     return out
 
 
 def patchify(x: torch.Tensor, p: int) -> torch.Tensor:
-    B, C, H, W = x.shape
-    assert x.is_contiguous() and x.dtype in (torch.float32, bf16)
+    c = _Args("patchify")
+    B, C, H, W = c("x", x, FLOAT, (None,) * 4)
+    c.on_cuda()
     out = torch.empty(B, (H // p) * (W // p), C * p * p, device=x.device, dtype=bf16)
-    check(lib.b200mix_patchify(_p(x), 1 if x.dtype == torch.float32 else 0, _p(out), B, C, H, W, p, _stream()),
-          "b200mix_patchify")
-    _count()
+    _launch("b200mix_patchify", x, 1 if x.dtype == torch.float32 else 0, out, B, C, H, W, p)
     return out
 
 
 def unpatchify(x: torch.Tensor, C: int, h: int, w: int, p: int, out_dtype=bf16) -> torch.Tensor:
+    c = _Args("unpatchify")
     B = x.shape[0]
-    assert x.is_contiguous() and x.dtype == bf16
+    c("x", x, BF16, numel=B * h * w * p * p * C)
     out = torch.empty(B, C, h * p, w * p, device=x.device, dtype=out_dtype)
-    check(lib.b200mix_unpatchify(_p(x), _p(out), 1 if out_dtype == torch.float32 else 0, B, C, h, w, p, _stream()),
-          "b200mix_unpatchify")
-    _count()
+    c("out", out, FLOAT)
+    c.on_cuda()
+    _launch("b200mix_unpatchify", x, out, 1 if out_dtype == torch.float32 else 0, B, C, h, w, p)
     return out
 
 
 def conv3x3(x: torch.Tensor, w: torch.Tensor, bias=None, *, stride=1, row_add=None, residual=None, act=ACT_NONE,
             out_scale=1.0, out=None) -> torch.Tensor:
     """x: bf16 NHWC [B,H,W,Cin] contiguous; w: bf16 [Cout,3,3,Cin] contiguous; returns bf16 NHWC."""
-    _req(x, bf16, "x"), _req(w, bf16, "w")
-    B, H, W, Cin = x.shape
-    Cout = w.shape[0]
-    assert x.is_contiguous() and w.is_contiguous()
+    c = _Args("conv3x3")
+    B, H, W, Cin = c("x", x, BF16, (None,) * 4)
+    Cout = c("w", w, BF16, (None, 3, 3, Cin))[0]
     Ho, Wo = H // stride, W // stride
-    if out is None:
-        out = torch.empty(B, Ho, Wo, Cout, device=x.device, dtype=bf16)
+    c("out", out, BF16, (B, Ho, Wo, Cout)), c("residual", residual, BF16, (B, Ho, Wo, Cout))
+    c("bias", bias, F32, numel=Cout), c("row_add", row_add, F32, layout=None)
     if row_add is not None:
         _check_mod_views("conv3x3", row_add=row_add)
+        _check_mod_groups("conv3x3", B * Ho * Wo, Ho * Wo, Cout, row_add=row_add)
+    c.on_cuda()
+    if out is None:
+        out = torch.empty(B, Ho, Wo, Cout, device=x.device, dtype=bf16)
     e = make_epilogue(bias=bias, row_add=row_add, ld_row=0 if row_add is None else row_add.stride(0),
                       rows_per_group=Ho * Wo, residual=residual, ldr=Cout, act=act, out_scale=out_scale)
     with _Timed("igemm", 2.0 * B * Ho * Wo * Cout * 9 * Cin, "flop",
                 lambda: f"conv{stride} {B * Ho * Wo}x{Cout}x{9 * Cin}" + _epi_tag(e)):
-        check(lib.b200mix_conv3x3(_p(x), _p(w), _p(out), B, H, W, Cin, Cout, stride, ctypes.byref(e), _stream()),
-              "b200mix_conv3x3")
-    _count()
+        _launch("b200mix_conv3x3", x, w, out, B, H, W, Cin, Cout, stride, ctypes.byref(e))
     return out
 
 
@@ -399,32 +457,33 @@ def conv3x3_up2x(x: torch.Tensor, w4: torch.Tensor, bias=None, *, row_add=None, 
                  out_scale=1.0, out=None) -> torch.Tensor:
     """conv3x3(nearest_upsample_2x(x)) from the low-resolution x: bf16 NHWC [B,H,W,Cin]; w4 = fold_upsample_conv_weight(w).
     Returns bf16 NHWC [B,2H,2W,Cout] (Upsample2D, resnet.py:169-218)."""
-    _req(x, bf16, "x"), _req(w4, bf16, "w4")
-    B, H, W, Cin = x.shape
-    Cout = w4.shape[0]
-    assert x.is_contiguous() and w4.is_contiguous() and tuple(w4.shape[1:]) == (16, Cin)
-    if out is None:
-        out = torch.empty(B, 2 * H, 2 * W, Cout, device=x.device, dtype=bf16)
+    c = _Args("conv3x3_up2x")
+    B, H, W, Cin = c("x", x, BF16, (None,) * 4)
+    Cout = c("w4", w4, BF16, (None, 16, Cin))[0]
+    c("out", out, BF16, (B, 2 * H, 2 * W, Cout)), c("residual", residual, BF16, (B, 2 * H, 2 * W, Cout))
+    c("bias", bias, F32, numel=Cout), c("row_add", row_add, F32, layout=None)
     if row_add is not None:
         _check_mod_views("conv3x3_up2x", row_add=row_add)
+        _check_mod_groups("conv3x3_up2x", B * 4 * H * W, 4 * H * W, Cout, row_add=row_add)
+    c.on_cuda()
+    if out is None:
+        out = torch.empty(B, 2 * H, 2 * W, Cout, device=x.device, dtype=bf16)
     e = make_epilogue(bias=bias, row_add=row_add, ld_row=0 if row_add is None else row_add.stride(0),
                       rows_per_group=4 * H * W, residual=residual, ldr=Cout, act=act, out_scale=out_scale)
     with _Timed("igemm", 2.0 * B * 4 * H * W * Cout * 4 * Cin, "flop",
                 lambda: f"convup {B * 4 * H * W}x{Cout}x{4 * Cin}" + _epi_tag(e)):
-        check(lib.b200mix_conv3x3_up2x(_p(x), _p(w4), _p(out), B, H, W, Cin, Cout, ctypes.byref(e), _stream()),
-              "b200mix_conv3x3_up2x")
-    _count()
+        _launch("b200mix_conv3x3_up2x", x, w4, out, B, H, W, Cin, Cout, ctypes.byref(e))
     return out
 
 
 def conv3x3_small_cin(x: torch.Tensor, w: torch.Tensor, bias=None) -> torch.Tensor:
-    B, H, W, Cin = x.shape
-    Cout = w.shape[0]
-    assert x.is_contiguous() and w.is_contiguous() and x.dtype in (torch.float32, bf16)
+    c = _Args("conv3x3_small_cin")
+    B, H, W, Cin = c("x", x, FLOAT, (None,) * 4)
+    Cout = c("w", w, BF16, (None, 3, 3, Cin))[0]
+    c("bias", bias, F32, numel=Cout)
+    c.on_cuda()
     out = torch.empty(B, H, W, Cout, device=x.device, dtype=bf16)
-    check(lib.b200mix_conv3x3_small_cin(_p(x), 1 if x.dtype == torch.float32 else 0, _p(w), _p(bias), _p(out), B, H, W,
-                                        Cin, Cout, _stream()), "b200mix_conv3x3_small_cin")
-    _count()
+    _launch("b200mix_conv3x3_small_cin", x, 1 if x.dtype == torch.float32 else 0, w, bias, out, B, H, W, Cin, Cout)
     return out
 
 
@@ -432,18 +491,16 @@ def conv3x3_narrow(x: torch.Tensor, w: torch.Tensor, bias=None, *, stride=1, act
     """act(conv3x3(x) + bias) for 1 <= Cin <= 128 (the ControlNet conditioning embedding). x: bf16 NHWC [B,H,W,Cin]
     contiguous; w: bf16 [Cout,3,3,Cin] contiguous; bias fp32 [Cout] or None; act ACT_NONE | ACT_SILU. Returns bf16 NHWC
     [B,H/stride,W/stride,Cout]."""
-    _req(x, bf16, "x"), _req(w, bf16, "w")
-    B, H, W, Cin = x.shape
-    Cout = w.shape[0]
-    assert x.is_contiguous() and w.is_contiguous() and tuple(w.shape[1:]) == (3, 3, Cin)
+    c = _Args("conv3x3_narrow")
+    B, H, W, Cin = c("x", x, BF16, (None,) * 4)
+    Cout = c("w", w, BF16, (None, 3, 3, Cin))[0]
+    c("bias", bias, F32, numel=Cout), c("out", out, BF16, (B, H // stride, W // stride, Cout))
+    c.on_cuda()
     if out is None:
         out = torch.empty(B, H // stride, W // stride, Cout, device=x.device, dtype=bf16)
     with _Timed("conv_narrow", 2.0 * B * (H // stride) * (W // stride) * Cout * 9 * Cin, "flop",
                 lambda: f"convn{stride} {B}x{H}x{W}x{Cin}->{Cout}"):
-        check(lib.b200mix_conv3x3_narrow(_p(x), _p(w), _p(None if bias is None else _req(bias, torch.float32, "bias")),
-                                         _p(out), B, H, W, Cin, Cout, int(stride), int(act), _stream()),
-              "b200mix_conv3x3_narrow")
-    _count()
+        _launch("b200mix_conv3x3_narrow", x, w, bias, out, B, H, W, Cin, Cout, int(stride), int(act))
     return out
 
 
@@ -453,36 +510,39 @@ def sdpa(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, *, scale: Optional[f
     """q: [B,Sq,Hq,D], k/v: [B,Sk,Hkv,D] bf16 views (head_dim contiguous; other strides arbitrary multiples of 8).
     attn_mask: additive bias (bf16 / fp32) broadcastable to [B,Hq,Sq,Sk] with a contiguous key axis (the reference's
     `attn_mask` argument, paddle_patch.py:418). Returns [B,Sq,Hq,D] (the layout of scaled_dot_product_attention_)."""
-    _req(q, bf16, "q"), _req(k, bf16, "k"), _req(v, bf16, "v")
-    B, Sq, Hq, D = q.shape
-    _, Sk, Hkv, _ = k.shape
-    assert q.stride(-1) == 1 and k.stride(-1) == 1 and v.stride(-1) == 1
-    if out is None:
-        out = torch.empty(B, Sq, Hq, D, device=q.device, dtype=bf16)
-    if scale is None:
-        scale = D ** -0.5
-    nseq = 0 if cu_seqlens is None else cu_seqlens.numel() - 1
+    c = _Args("sdpa")
+    B, Sq, Hq, D = c("q", q, BF16, (None,) * 4, ROWS)
+    _, Sk, Hkv, _ = c("k", k, BF16, (B, None, None, D), ROWS)
+    c("v", v, BF16, (B, Sk, Hkv, D), ROWS), c("out", out, BF16, (B, Sq, Hq, D), ROWS)
+    if Hq % Hkv:
+        raise ValueError(f"sdpa: {Hq} query heads cannot share {Hkv} key / value heads")
+    c("cu_seqlens", cu_seqlens, I32, (None,)), c("kv_lens", kv_lens, I32, numel=B)
     m_fp32, msb, msh, msq = 0, 0, 0, 0
     if attn_mask is not None:
-        if attn_mask.dtype not in (torch.float32, bf16):
+        if attn_mask.dtype not in FLOAT:
             raise TypeError(f"attn_mask must be an additive float32 / bfloat16 bias, got {attn_mask.dtype}")
         while attn_mask.dim() < 4:
             attn_mask = attn_mask.unsqueeze(0)
         if attn_mask.shape[-1] != Sk or any(a not in (1, n) for a, n in zip(attn_mask.shape[:3], (B, Hq, Sq))):
             raise ValueError(f"attn_mask shape {tuple(attn_mask.shape)} does not broadcast to {(B, Hq, Sq, Sk)}")
+        c("attn_mask", attn_mask, FLOAT, layout=None)
+    c.on_cuda()
+    if out is None:
+        out = torch.empty(B, Sq, Hq, D, device=q.device, dtype=bf16)
+    if scale is None:
+        scale = D ** -0.5
+    nseq = 0 if cu_seqlens is None else cu_seqlens.numel() - 1
+    if attn_mask is not None:
         if attn_mask.stride(-1) != 1 and Sk > 1:
             attn_mask = attn_mask.contiguous()
-        attn_mask = _req(attn_mask, attn_mask.dtype, "attn_mask")
         m_fp32 = 1 if attn_mask.dtype == torch.float32 else 0
         msb, msh, msq = (0 if attn_mask.shape[i] == 1 else attn_mask.stride(i) for i in range(3))
     with _Timed("attention", 4.0 * B * Hq * Sq * Sk * D * (0.5 if causal else 1.0), "flop",
                 lambda: f"attn B{B} H{Hq} Sq{Sq} Sk{Sk} D{D}" + (" causal" if causal else "")):
-        check(lib.b200mix_sdpa(_p(q), _p(k), _p(v), _p(out), B, Hq, Hkv, Sq, Sk, D, q.stride(0), q.stride(1),
-                               q.stride(2), k.stride(0), k.stride(1), k.stride(2), v.stride(0), v.stride(1),
-                               v.stride(2), out.stride(0), out.stride(1), out.stride(2), float(scale),
-                               1 if causal else 0, _p(cu_seqlens), nseq, _p(kv_lens), _p(attn_mask), m_fp32, msb, msh,
-                               msq, _stream()), "b200mix_sdpa")
-    _count()
+        _launch("b200mix_sdpa", q, k, v, out, B, Hq, Hkv, Sq, Sk, D, q.stride(0), q.stride(1), q.stride(2), k.stride(0),
+                k.stride(1), k.stride(2), v.stride(0), v.stride(1), v.stride(2), out.stride(0), out.stride(1),
+                out.stride(2), float(scale), 1 if causal else 0, cu_seqlens, nseq, kv_lens, attn_mask, m_fp32, msb, msh,
+                msq)
     return out
 
 
@@ -491,13 +551,16 @@ _gn_scratch = {}
 
 def groupnorm_nhwc(x1: torch.Tensor, gamma, beta, *, x2=None, groups=32, eps=1e-5, silu=False, out=None):
     """x1: bf16 [B,H,W,C1] (optionally concatenated on channels with x2 [B,H,W,C2]); returns bf16 [B,H,W,C1+C2]."""
-    _req(x1, bf16, "x1")
+    c = _Args("groupnorm_nhwc")
+    pix = c("x1", x1, BF16, (None, ...))[:-1]
     B, C1 = x1.shape[0], x1.shape[-1]
+    C2 = 0 if x2 is None else c("x2", x2, BF16, (*pix, None))[-1]
+    c("gamma", gamma, F32, numel=C1 + C2), c("beta", beta, F32, numel=C1 + C2)
+    c("out", out, BF16, (*pix, C1 + C2))
+    c.on_cuda()
     HW = x1.numel() // (B * C1)
-    C2 = 0 if x2 is None else x2.shape[-1]
-    assert x1.is_contiguous() and (x2 is None or x2.is_contiguous())
     if out is None:
-        out = torch.empty(*x1.shape[:-1], C1 + C2, device=x1.device, dtype=bf16)
+        out = torch.empty(*pix, C1 + C2, device=x1.device, dtype=bf16)
     # per-(device, stream, B, groups) scratch: two streams never share partial sums, and the size is exact for the key
     key = (x1.device, torch.cuda.current_stream().cuda_stream, B, groups)
     st = _gn_scratch.get(key)
@@ -506,9 +569,8 @@ def groupnorm_nhwc(x1: torch.Tensor, gamma, beta, *, x2=None, groups=32, eps=1e-
         st = torch.zeros(512 + (1024 + 2 * B) * groups * 2, device=x1.device, dtype=torch.float64)
         _gn_scratch[key] = st
     with _Timed("groupnorm", 2.0 * 2 * B * HW * (C1 + C2), "byte", lambda: f"gn {B}x{HW}x{C1 + C2}"):  # algorithmic: read once + write once (bf16)
-        check(lib.b200mix_groupnorm_nhwc(_p(x1), C1, _p(x2), C2, _p(gamma), _p(beta), _p(out), _p(st), st.numel() * 8, B,
-                                         HW, groups, float(eps), 1 if silu else 0, _stream()), "b200mix_groupnorm_nhwc")
-    _count(2)
+        _launch("b200mix_groupnorm_nhwc", x1, C1, x2, C2, gamma, beta, out, st, st.numel() * 8, B, HW, groups,
+                float(eps), 1 if silu else 0, kernels=2)
     return out
 
 
@@ -516,25 +578,27 @@ def layernorm(x: torch.Tensor, weight=None, bias=None, *, eps=1e-5, rms=False, d
               shift=None, rows_per_group=0, want_resid=False, out=None):
     """Row-wise (RMS/Layer)Norm with optional fused residual update x + gate*delta and AdaLN modulation.
     Returns y, or (resid, y) when want_resid."""
-    _req(x, bf16, "x")
-    N = x.shape[-1]
-    x2 = x.reshape(-1, N)
-    assert x2.is_contiguous()
-    M = x2.shape[0]
-    if out is None:
-        out = torch.empty_like(x)
-    resid = torch.empty_like(x) if (want_resid and delta is not None) else None
+    c = _Args("layernorm")
+    N = c("x", x, BF16, (..., None), layout=None)[-1]
+    M = x.numel() // N
+    c("delta", delta, BF16, x.shape), c("out", out, BF16, x.shape)
+    c("weight", weight, F32, numel=N), c("bias", bias, F32, numel=N)
+    for name, v in (("gate", gate), ("scale", scale), ("shift", shift)):
+        c(name, v, F32, layout=None)
     mod = gate if gate is not None else (scale if scale is not None else shift)
     if mod is not None:
         _check_mod_views("layernorm", gate=gate, scale=scale, shift=shift)
         _check_mod_groups("layernorm", M, rows_per_group, N, gate=gate, scale=scale, shift=shift)
+    c.on_cuda()
+    x2 = x.reshape(-1, N).contiguous()
+    if out is None:
+        out = torch.empty_like(x2).view(x.shape)
+    resid = torch.empty_like(x2).view(x.shape) if (want_resid and delta is not None) else None
     ld_mod = 0 if mod is None else mod.stride(0)
     nbytes = 2.0 * M * N * (2 + (1 if delta is not None else 0) + (1 if resid is not None else 0))
     with _Timed("layernorm", nbytes, "byte", lambda: f"ln {M}x{N}" + (" +delta" if delta is not None else "")):
-        check(lib.b200mix_layernorm(_p(x2), _p(delta), _p(gate), _p(resid), _p(out), _p(weight), _p(bias), _p(scale),
-                                    _p(shift), ld_mod, rows_per_group, M, N, float(eps), 1 if rms else 0, _stream()),
-              "b200mix_layernorm")
-    _count()
+        _launch("b200mix_layernorm", x2, delta, gate, resid, out, weight, bias, scale, shift, ld_mod, rows_per_group, M,
+                N, float(eps), 1 if rms else 0)
     if want_resid:
         return (resid if resid is not None else x), out
     return out
@@ -542,95 +606,99 @@ def layernorm(x: torch.Tensor, weight=None, bias=None, *, eps=1e-5, rms=False, d
 
 def softmax_rows(x: torch.Tensor, scale: float = 1.0, out=None) -> torch.Tensor:
     """x: fp32 [M, N] (row stride arbitrary multiple of 4) -> bf16 softmax(x * scale) [M, N]."""
-    _req(x, torch.float32, "x")
-    M, N = x.shape
-    assert x.stride(1) == 1
+    c = _Args("softmax_rows")
+    M, N = c("x", x, F32, (None, None), STRIDED)
+    c("out", out, BF16, (M, N), STRIDED)
+    c.on_cuda()
     if out is None:
         out = torch.empty(M, N, device=x.device, dtype=bf16)
     with _Timed("softmax", 4.0 * M * N + 2.0 * M * N, "byte", lambda: f"softmax {M}x{N}"):
-        check(lib.b200mix_softmax_rows(_p(x), _p(out), M, N, x.stride(0), out.stride(0), float(scale), _stream()),
-              "b200mix_softmax_rows")
-    _count()
+        _launch("b200mix_softmax_rows", x, out, M, N, x.stride(0), out.stride(0), float(scale))
     return out
 
 
 def timestep_embedding(t: torch.Tensor, dim: int, *, flip_sin_to_cos=True, downscale_freq_shift=0.0, scale=1.0,
                        max_period=10000.0, out=None, col0=0, out_dtype=bf16):
-    _req(t, torch.float32, "t")
+    c = _Args("timestep_embedding")
+    c("t", t, F32)
     B = t.numel()
     if out is None:
         out = torch.empty(B, dim, device=t.device, dtype=out_dtype)
-    check(lib.b200mix_timestep_embedding(_p(t), _p(out), 1 if out.dtype == torch.float32 else 0, B, dim, out.stride(0),
-                                         col0, 1 if flip_sin_to_cos else 0, float(downscale_freq_shift), float(scale),
-                                         float(max_period), _stream()), "b200mix_timestep_embedding")
-    _count()
+    width = c("out", out, FLOAT, (B, None), STRIDED)[1]
+    if col0 < 0 or col0 + dim > width:
+        raise ValueError(f"timestep_embedding: columns [{col0}, {col0 + dim}) do not fit out's {width}")
+    c.on_cuda()
+    _launch("b200mix_timestep_embedding", t, out, 1 if out.dtype == torch.float32 else 0, B, dim, out.stride(0), col0,
+            1 if flip_sin_to_cos else 0, float(downscale_freq_shift), float(scale), float(max_period))
     return out
 
 
 def activation(x: torch.Tensor, act: int, out_dtype=None):
-    assert x.is_contiguous() and x.dtype in (torch.float32, bf16)
+    c = _Args("activation")
+    c("x", x, FLOAT)
     out = torch.empty_like(x, dtype=out_dtype or x.dtype)
-    check(lib.b200mix_activation(_p(x), _p(out), x.numel(), act, 1 if x.dtype == torch.float32 else 0,
-                                 1 if out.dtype == torch.float32 else 0, _stream()), "b200mix_activation")
-    _count()
+    c("out", out, FLOAT)
+    c.on_cuda()
+    _launch("b200mix_activation", x, out, x.numel(), act, 1 if x.dtype == torch.float32 else 0,
+            1 if out.dtype == torch.float32 else 0)
     return out
 
 
 def upsample_nearest2x(x: torch.Tensor):
-    _req(x, bf16, "x")
-    B, H, W, C = x.shape
+    c = _Args("upsample_nearest2x")
+    B, H, W, C = c("x", x, BF16, (None,) * 4)
+    c.on_cuda()
     out = torch.empty(B, 2 * H, 2 * W, C, device=x.device, dtype=bf16)
-    check(lib.b200mix_upsample_nearest2x_nhwc(_p(x), _p(out), B, H, W, C, _stream()), "b200mix_upsample")
-    _count()
+    _launch("b200mix_upsample_nearest2x_nhwc", x, out, B, H, W, C)
     return out
 
 
 def concat_channels(x1: torch.Tensor, x2: torch.Tensor):
-    C1, C2 = x1.shape[-1], x2.shape[-1]
-    rows = x1.numel() // C1
+    c = _Args("concat_channels")
+    C1 = c("x1", x1, BF16, (..., None))[-1]
+    C2 = c("x2", x2, BF16, (*x1.shape[:-1], None))[-1]
+    c.on_cuda()
     out = torch.empty(*x1.shape[:-1], C1 + C2, device=x1.device, dtype=bf16)
-    check(lib.b200mix_concat_channels(_p(x1), C1, _p(x2), C2, _p(out), rows, _stream()), "b200mix_concat_channels")
-    _count()
+    _launch("b200mix_concat_channels", x1, C1, x2, C2, out, x1.numel() // C1)
     return out
 
 
 def nchw_to_nhwc(x: torch.Tensor):
-    B, C, H, W = x.shape
-    assert x.is_contiguous() and x.dtype in (torch.float32, bf16)
+    c = _Args("nchw_to_nhwc")
+    B, C, H, W = c("x", x, FLOAT, (None,) * 4)
+    c.on_cuda()
     out = torch.empty(B, H, W, C, device=x.device, dtype=bf16)
-    check(lib.b200mix_nchw_to_nhwc(_p(x), 1 if x.dtype == torch.float32 else 0, _p(out), B, C, H, W, _stream()),
-          "b200mix_nchw_to_nhwc")
-    _count()
+    _launch("b200mix_nchw_to_nhwc", x, 1 if x.dtype == torch.float32 else 0, out, B, C, H, W)
     return out
 
 
 def nhwc_to_nchw(x: torch.Tensor, out_dtype=torch.float32, out=None):
-    B, H, W, C = x.shape
-    _req(x, bf16, "x")
+    c = _Args("nhwc_to_nchw")
+    B, H, W, C = c("x", x, BF16, (None,) * 4)
     if out is None:
         out = torch.empty(B, C, H, W, device=x.device, dtype=out_dtype)
-    check(lib.b200mix_nhwc_to_nchw(_p(x), _p(out), 1 if out.dtype == torch.float32 else 0, B, C, H, W, _stream()),
-          "b200mix_nhwc_to_nchw")
-    _count()
+    c("out", out, FLOAT, (B, C, H, W))
+    c.on_cuda()
+    _launch("b200mix_nhwc_to_nchw", x, out, 1 if out.dtype == torch.float32 else 0, B, C, H, W)
     return out
 
 
 def add_residual_nhwc(a: torch.Tensor, r: torch.Tensor, *, r_nchw: bool, out=None) -> torch.Tensor:
     """a: bf16 NHWC [B,H,W,C]; r: the same values as NHWC bf16, or NCHW fp32 / bf16 [B,C,H,W] (r_nchw). Returns a + r."""
-    _req(a, bf16, "a")
-    B, H, W, C = a.shape
+    c = _Args("add_residual_nhwc")
+    B, H, W, C = c("a", a, BF16, (None,) * 4)
     want = (B, C, H, W) if r_nchw else (B, H, W, C)
     if tuple(r.shape) != want:
         raise ValueError(f"residual shape {tuple(r.shape)} does not match the activation {want}")
-    if r.dtype not in (torch.float32, bf16):
+    c("out", out, BF16, (B, H, W, C))
+    c.on_cuda()
+    if r.dtype not in FLOAT:
         r = r.float()
     r = r.to(a.device).contiguous()
-    assert a.is_contiguous()
     if out is None:
         out = torch.empty_like(a)
-    check(lib.b200mix_add_residual_nhwc(_p(a), _p(r), 1 if r.dtype == torch.float32 else 0, 1 if r_nchw else 0, _p(out),
-                                        B, C, H, W, _stream()), "b200mix_add_residual_nhwc")
-    _count()
+    _launch("b200mix_add_residual_nhwc", a, r, 1 if r.dtype == torch.float32 else 0, 1 if r_nchw else 0, out, B, C, H,
+            W)
     return out
 
 
@@ -639,21 +707,13 @@ def _step_tensors(op, x, m_u, m_c, out, **fp32_bufs):
     like x (like m_u when x is None) if it is None. The kernels read every tensor flat over x's element count (m_u's
     when x is None) and m_c with m_u's dtype flag, so each given tensor must be contiguous, have that many elements and
     the dtype below: x, out and fp32_bufs fp32, m_u fp32 or bf16, m_c m_u's dtype."""
-    f32 = (torch.float32,)
-    want = {"x": (x, f32), "model output": (m_u, (torch.float32, bf16)), "model_output_cond": (m_c, (m_u.dtype,)),
-            "out": (out, f32), **{k: (t, f32) for k, t in fp32_bufs.items()}}
-    given = {k: v for k, v in want.items() if v[0] is not None}
+    c = _Args(op)
     n = (m_u if x is None else x).numel()
-    for name, (t, dtypes) in given.items():
-        if t.dtype not in dtypes:
-            raise TypeError(f"{op}: {name} must be {' or '.join(map(str, dtypes))}, got {t.dtype}")
-        if t.numel() != n:
-            raise ValueError(f"{op}: {name} has {t.numel()} elements, expected {n}")
-        if not t.is_contiguous():
-            raise ValueError(f"{op}: {name} must be contiguous, got strides {t.stride()} for shape {tuple(t.shape)}")
-    for name, (t, _) in given.items():
-        if not t.is_cuda:
-            raise _lib.B200MixError(f"{op}: {name} must be a CUDA tensor (b200mix has no CPU path)")
+    c("x", x, F32, numel=n), c("model output", m_u, FLOAT, numel=n)
+    c("model_output_cond", m_c, (m_u.dtype,), numel=n), c("out", out, F32, numel=n)
+    for name, t in fp32_bufs.items():
+        c(name, t, F32, numel=n)
+    c.on_cuda()
     if out is None:
         like = m_u if x is None else x
         out = torch.empty(like.shape, device=like.device, dtype=torch.float32)
@@ -666,10 +726,8 @@ PRED_TYPES = {"epsilon": 0, "sample": 1, "v_prediction": 2}
 def ddim_step(m_u, m_c, guidance, x, sa_t, sb_t, sa_p, sb_p, prediction_type="epsilon", clip_sample_range=0.0, out=None):
     """DDIM step for any prediction_type, optional x0 clipping (clip_sample_range > 0), fused CFG combine."""
     fp32, out = _step_tensors("ddim_step", x, m_u, m_c, out)
-    check(lib.b200mix_ddim_step_ex(_p(m_u), _p(m_c), fp32, float(guidance), _p(x), _p(out), x.numel(), float(sa_t),
-                                   float(sb_t), float(sa_p), float(sb_p), PRED_TYPES[prediction_type],
-                                   float(clip_sample_range), _stream()), "b200mix_ddim_step_ex")
-    _count()
+    _launch("b200mix_ddim_step_ex", m_u, m_c, fp32, float(guidance), x, out, x.numel(), float(sa_t), float(sb_t),
+            float(sa_p), float(sb_p), PRED_TYPES[prediction_type], float(clip_sample_range))
     return out
 
 
@@ -677,10 +735,9 @@ def lcm_step(m_u, m_c, guidance, x, noise, sa_t, sb_t, c_skip, c_out, sa_p, sb_p
              clip_sample_range=0.0, out=None, denoised=None):
     """LCMScheduler.step; noise None = final step (x_prev = denoised)."""
     fp32, out = _step_tensors("lcm_step", x, m_u, m_c, out, noise=noise, denoised=denoised)
-    check(lib.b200mix_lcm_step(_p(m_u), _p(m_c), fp32, float(guidance), _p(x), _p(noise), _p(out), _p(denoised),
-                               x.numel(), float(sa_t), float(sb_t), float(c_skip), float(c_out), float(sa_p), float(sb_p),
-                               PRED_TYPES[prediction_type], float(clip_sample_range), _stream()), "b200mix_lcm_step")
-    _count()
+    _launch("b200mix_lcm_step", m_u, m_c, fp32, float(guidance), x, noise, out, denoised, x.numel(), float(sa_t),
+            float(sb_t), float(c_skip), float(c_out), float(sa_p), float(sb_p), PRED_TYPES[prediction_type],
+            float(clip_sample_range))
     return out
 
 
@@ -689,28 +746,16 @@ def iddpm_step(model_out, x, cfg_scale, cfg_channel, scalars, add_noise, seed=0,
     the conditional rows first; x fp32 [B, C, ...]; scalars = (sqrt_recip_ac, sqrt_recipm1_ac, coef1, coef2, max_log,
     min_log) as fp32 values; noise fp32 like x, or None for Philox noise keyed by (seed, step). out may be x itself;
     out_dup receives a second copy of the result. Returns out."""
-    _req(x, torch.float32, "x")
-    B, C = x.shape[:2]
-    if model_out.dtype not in (torch.float32, bf16) or not model_out.is_contiguous():
-        raise ValueError("model_out must be contiguous fp32 or bf16")
-    if tuple(model_out.shape) != (2 * B, 2 * C, *x.shape[2:]):
-        raise ValueError(f"model_out {tuple(model_out.shape)} must be [2B, 2C, ...] for x {tuple(x.shape)}")
-    if noise is not None:
-        _req(noise, torch.float32, "noise")
-        assert noise.shape == x.shape
+    c = _Args("iddpm_step")
+    B, C = c("x", x, F32, (None, None, ...))[:2]
+    c("model_out", model_out, FLOAT, (2 * B, 2 * C, *x.shape[2:]))
+    c("noise", noise, F32, x.shape), c("out", out, F32, x.shape), c("out_dup", out_dup, F32, x.shape)
+    c.on_cuda()
     if out is None:
         out = torch.empty_like(x)
-    for t in (out, out_dup):
-        if t is not None:
-            _req(t, torch.float32, "out")
-            assert t.shape == x.shape
-    if not all(t is None or t.is_contiguous() for t in (x, noise, out, out_dup)):
-        raise ValueError("iddpm_step: x, noise and the outputs must be contiguous")
-    check(lib.b200mix_iddpm_step(_p(model_out), 1 if model_out.dtype == torch.float32 else 0, _p(x), _p(noise), _p(out),
-                                 _p(out_dup), B, C, x.numel() // (B * C), float(cfg_scale), int(cfg_channel),
-                                 *(float(v) for v in scalars), 1 if add_noise else 0, int(seed), int(step), _stream()),
-          "b200mix_iddpm_step")
-    _count()
+    _launch("b200mix_iddpm_step", model_out, 1 if model_out.dtype == torch.float32 else 0, x, noise, out, out_dup, B, C,
+            x.numel() // (B * C), float(cfg_scale), int(cfg_channel), *(float(v) for v in scalars),
+            1 if add_noise else 0, int(seed), int(step))
     return out
 
 
@@ -725,60 +770,57 @@ def cfg_combine(eps_u, eps_c, guidance, guidance_rescale=0.0, out=None):
     ratio = None
     if guidance_rescale > 0.0:
         ratio = torch.empty(B, device=eps_u.device, dtype=torch.float32)
-        check(lib.b200mix_cfg_rescale_ratio(_p(eps_u), _p(eps_c), fp32, float(guidance), _p(ratio), B, nps, _stream()),
-              "b200mix_cfg_rescale_ratio")
-        _count()
-    check(lib.b200mix_cfg_combine(_p(eps_u), _p(eps_c), fp32, float(guidance), _p(ratio), float(guidance_rescale), nps,
-                                  _p(out), eps_u.numel(), _stream()), "b200mix_cfg_combine")
-    _count()
+        _launch("b200mix_cfg_rescale_ratio", eps_u, eps_c, fp32, float(guidance), ratio, B, nps)
+    _launch("b200mix_cfg_combine", eps_u, eps_c, fp32, float(guidance), ratio, float(guidance_rescale), nps, out,
+            eps_u.numel())
     return out
 
 
 def euler_step(v_u, v_c, guidance, x, sigma, dt, out=None):
     fp32, out = _step_tensors("euler_step", x, v_u, v_c, out)
-    check(lib.b200mix_euler_step(_p(v_u), _p(v_c), fp32, float(guidance), _p(x), _p(out), x.numel(), float(sigma),
-                                 float(dt), _stream()), "b200mix_euler_step")
-    _count()
+    _launch("b200mix_euler_step", v_u, v_c, fp32, float(guidance), x, out, x.numel(), float(sigma), float(dt))
     return out
 
 
 def dpmpp_2m_step(eps_u, eps_c, guidance, x, m_prev, m_out, sigma_cur, alpha_cur, A, C, halfC, inv_r0, out=None):
     """DPM-Solver++ 2M update (see include/b200mix.h); m_prev None = first-order step; m_out receives x0."""
     fp32, out = _step_tensors("dpmpp_2m_step", x, eps_u, eps_c, out, m_prev=m_prev, m_out=m_out)
-    check(lib.b200mix_dpmpp_2m_step(_p(eps_u), _p(eps_c), fp32, float(guidance), _p(x), _p(m_prev), _p(out), _p(m_out),
-                                    x.numel(), float(sigma_cur), float(alpha_cur), float(A), float(C), float(halfC),
-                                    float(inv_r0), _stream()), "b200mix_dpmpp_2m_step")
-    _count()
+    _launch("b200mix_dpmpp_2m_step", eps_u, eps_c, fp32, float(guidance), x, m_prev, out, m_out, x.numel(),
+            float(sigma_cur), float(alpha_cur), float(A), float(C), float(halfC), float(inv_r0))
     return out
 
 
 def scale_model_input(x: torch.Tensor, denom: float, out=None) -> torch.Tensor:
     """EulerDiscreteScheduler.scale_model_input: x / denom in fp32 (IEEE division)."""
-    _req(x, torch.float32, "x")
-    assert x.is_contiguous()
+    c = _Args("scale_model_input")
+    c("x", x, F32), c("out", out, F32, numel=x.numel())
+    c.on_cuda()
     if out is None:
         out = torch.empty_like(x)
-    check(lib.b200mix_scale_model_input(_p(x), _p(out), x.numel(), float(denom), _stream()), "b200mix_scale_model_input")
-    _count()
+    _launch("b200mix_scale_model_input", x, out, x.numel(), float(denom))
     return out
 
 
 def cast(x: torch.Tensor, dtype):
-    assert x.is_contiguous()
+    c = _Args("cast")
+    c("x", x, FLOAT)
     out = torch.empty_like(x, dtype=dtype)
-    check(lib.b200mix_cast(_p(x), _p(out), x.numel(), 1 if x.dtype == torch.float32 else 0,
-                           1 if dtype == torch.float32 else 0, _stream()), "b200mix_cast")
-    _count()
+    c("out", out, FLOAT)
+    c.on_cuda()
+    _launch("b200mix_cast", x, out, x.numel(), 1 if x.dtype == torch.float32 else 0, 1 if dtype == torch.float32 else 0)
     return out
 
 
 def rope_inplace(x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, rot_dim: Optional[int] = None):
     """x: bf16 [T, H, Dpad] view (last dim contiguous); cos/sin fp32 [T, rot_dim]."""
-    T, H, Dp = x.shape
+    c = _Args("rope_inplace")
+    T, H, Dp = c("x", x, BF16, (None, None, None), STRIDED)
     D = rot_dim or Dp
-    check(lib.b200mix_rope_inplace(_p(x), T, H, D, x.stride(0), x.stride(1), _p(cos), _p(sin), _stream()),
-          "b200mix_rope_inplace")
-    _count()
+    if D > Dp:
+        raise ValueError(f"rope_inplace: rot_dim {D} is wider than the {Dp} channels of a head")
+    c("cos", cos, F32, (T, D)), c("sin", sin, F32, (T, D))
+    c.on_cuda()
+    _launch("b200mix_rope_inplace", x, T, H, D, x.stride(0), x.stride(1), cos, sin)
     return x
 
 
@@ -786,12 +828,13 @@ def decode_rope_cache(qkv: torch.Tensor, heads: int, kv_heads: int, head_dim: in
                       rows: torch.Tensor, cache_k: torch.Tensor, cache_v: torch.Tensor):
     """qkv bf16 [B, (heads + 2*kv_heads) * head_dim] of a single-token step: RoPE on the q heads in place, RoPE'd k heads and
     the v heads written into row rows[b] (int64, device) of the flattened caches [*, kv_heads * head_dim]."""
-    _req(qkv, bf16, "qkv"), _req(rows, torch.int64, "rows"), _req(cache_k, bf16, "cache_k"), _req(cache_v, bf16, "cache_v")
-    assert qkv.stride(1) == 1 and qkv.shape[1] == (heads + 2 * kv_heads) * head_dim
-    assert cache_k.is_contiguous() and cache_v.is_contiguous() and cos.is_contiguous() and sin.is_contiguous()
-    check(lib.b200mix_decode_rope_cache(_p(qkv), qkv.stride(0), qkv.shape[0], heads, kv_heads, head_dim, _p(cos), _p(sin),
-                                        _p(rows), _p(cache_k), _p(cache_v), _stream()), "b200mix_decode_rope_cache")
-    _count()
+    c = _Args("decode_rope_cache")
+    B = c("qkv", qkv, BF16, (None, (heads + 2 * kv_heads) * head_dim), ROWS)[0]
+    c("cos", cos, F32, (B, head_dim)), c("sin", sin, F32, (B, head_dim)), c("rows", rows, I64, numel=B)
+    c("cache_k", cache_k, BF16, (None, kv_heads * head_dim)), c("cache_v", cache_v, BF16, (None, kv_heads * head_dim))
+    c.on_cuda()
+    _launch("b200mix_decode_rope_cache", qkv, qkv.stride(0), B, heads, kv_heads, head_dim, cos, sin, rows, cache_k,
+            cache_v)
 
 
 def sample_tokens(logits: torch.Tensor, presence: torch.Tensor, finished: torch.Tensor, state: torch.Tensor,
@@ -802,27 +845,17 @@ def sample_tokens(logits: torch.Tensor, presence: torch.Tensor, finished: torch.
     [B, ceil(V/32)] bitmap of the ids seen so far; finished int32 [B]; state int64 [4] (step, arrivals, all finished,
     step of the last finish; zero before the first step); out int64 [B, max_new]; next_ids int64 [B]; eos_ids int64
     [n] on the device or None. Every buffer except logits is updated on the device."""
-    _req(logits, torch.float32, "logits"), _req(presence, torch.int32, "presence"), _req(finished, torch.int32, "finished")
-    _req(state, torch.int64, "state"), _req(out, torch.int64, "out"), _req(next_ids, torch.int64, "next_ids")
-    B, V = logits.shape
-    if logits.stride(1) != 1 and V > 1:
-        raise ValueError("logits must have a contiguous vocabulary axis")
-    words = (V + 31) // 32
-    if tuple(presence.shape) != (B, words) or not presence.is_contiguous():
-        raise ValueError(f"presence must be a contiguous int32 [{B}, {words}] bitmap, got {tuple(presence.shape)}")
-    if finished.numel() != B or next_ids.numel() != B or state.numel() != 4 or out.shape[0] != B or out.stride(1) != 1:
-        raise ValueError("finished / next_ids must have B entries, state 4, out [B, max_new] with contiguous rows")
-    n_eos = 0
-    if eos_ids is not None:
-        _req(eos_ids, torch.int64, "eos_ids")
-        n_eos = eos_ids.numel()
+    c = _Args("sample_tokens")
+    B, V = c("logits", logits, F32, (None, None), STRIDED)
+    c("presence", presence, I32, (B, (V + 31) // 32)), c("finished", finished, I32, numel=B)
+    c("state", state, I64, numel=4), c("out", out, I64, (B, None), STRIDED), c("next_ids", next_ids, I64, numel=B)
+    c("eos_ids", eos_ids, I64)
+    c.on_cuda()
     with _Timed("sampling", 4.0 * B * V, "byte", lambda: f"sample {B}x{V}"):
-        check(lib.b200mix_sample_tokens(_p(logits), logits.stride(0), B, V, _p(presence), _p(finished), _p(state),
-                                        _p(out), out.stride(0), out.shape[1], _p(next_ids), _p(eos_ids), n_eos,
-                                        int(pad_token_id), 1 if do_sample else 0, float(temperature), int(top_k),
-                                        float(top_p), float(repetition_penalty), int(seed) & (2 ** 64 - 1), _stream()),
-              "b200mix_sample_tokens")
-    _count()
+        _launch("b200mix_sample_tokens", logits, logits.stride(0), B, V, presence, finished, state, out, out.stride(0),
+                out.shape[1], next_ids, eos_ids, 0 if eos_ids is None else eos_ids.numel(), int(pad_token_id),
+                1 if do_sample else 0, float(temperature), int(top_k), float(top_p), float(repetition_penalty),
+                int(seed) & (2 ** 64 - 1))
 
 
 def beam_search_workspace_bytes(B: int, num_beams: int, V: int) -> int:
@@ -840,38 +873,29 @@ def beam_search_step(logits: torch.Tensor, num_beams: int, workspace: torch.Tens
     int64 / parents int32 [max_new, B*nb]; hyp_score fp64 / hyp_step, hyp_slot int32 [B, nb]; hyp_count int32 [B];
     hyp_worst fp64 [B]; done int32 [B]; presence int32 [2, B*nb, ceil(V/32)] or None (penalty 1); workspace uint8 of
     beam_search_workspace_bytes(B, nb, V). Everything but logits is updated on the device; eos_token_id -1 = none."""
-    _req(logits, torch.float32, "logits")
-    rows, V = logits.shape
+    c = _Args("beam_search_step")
+    rows, V = c("logits", logits, F32, (None, None), STRIDED)
     nb = int(num_beams)
-    if logits.stride(1) != 1 or rows % nb:
-        raise ValueError(f"logits must be [B * {nb}, V] with a contiguous vocabulary axis, got {tuple(logits.shape)}")
+    if rows % nb:
+        raise ValueError(f"beam_search_step: logits must be [B * {nb}, V], got {tuple(logits.shape)}")
     B = rows // nb
-    for t, dt, n, name in ((state, torch.int64, 4, "state"), (next_ids, torch.int64, rows, "next_ids"),
-                           (beam_scores, torch.float32, rows, "beam_scores"), (hyp_score, torch.float64, B * nb, "hyp_score"),
-                           (hyp_step, torch.int32, B * nb, "hyp_step"), (hyp_slot, torch.int32, B * nb, "hyp_slot"),
-                           (hyp_count, torch.int32, B, "hyp_count"), (hyp_worst, torch.float64, B, "hyp_worst"),
-                           (done, torch.int32, B, "done")):
-        _req(t, dt, name)
-        if t.numel() != n or not t.is_contiguous():
-            raise ValueError(f"{name} must be a contiguous tensor of {n} elements, got {tuple(t.shape)}")
-    _req(tokens, torch.int64, "tokens"), _req(parents, torch.int32, "parents"), _req(workspace, torch.uint8, "workspace")
-    max_new = tokens.shape[0]
-    if tuple(tokens.shape) != (max_new, rows) or tuple(parents.shape) != (max_new, rows) or not (
-            tokens.is_contiguous() and parents.is_contiguous()):
-        raise ValueError(f"tokens / parents must be contiguous [max_new, {rows}]")
-    if presence is not None:
-        _req(presence, torch.int32, "presence")
-        if tuple(presence.shape) != (2, rows, (V + 31) // 32) or not presence.is_contiguous():
-            raise ValueError(f"presence must be a contiguous int32 [2, {rows}, {(V + 31) // 32}] bitmap pair")
+    for name, t, dt, n in (("state", state, I64, 4), ("next_ids", next_ids, I64, rows),
+                           ("beam_scores", beam_scores, F32, rows), ("hyp_score", hyp_score, (torch.float64,), rows),
+                           ("hyp_step", hyp_step, I32, rows), ("hyp_slot", hyp_slot, I32, rows),
+                           ("hyp_count", hyp_count, I32, B), ("hyp_worst", hyp_worst, (torch.float64,), B),
+                           ("done", done, I32, B)):
+        c(name, t, dt, numel=n)
+    max_new = c("tokens", tokens, I64, (None, rows))[0]
+    c("parents", parents, I32, (max_new, rows)), c("workspace", workspace, (torch.uint8,))
+    c("presence", presence, I32, (2, rows, (V + 31) // 32))
+    c.on_cuda()
     st = _lib.BeamState(*(t.data_ptr() for t in (state, next_ids, beam_scores, tokens, parents, hyp_score, hyp_step,
                                                  hyp_slot, hyp_count, hyp_worst, done)),
                         None if presence is None else presence.data_ptr())
     with _Timed("beam_search", 4.0 * rows * V, "byte", lambda: f"beam {B}x{nb}x{V}"):
-        check(lib.b200mix_beam_search_step(_p(logits), logits.stride(0), B, nb, V, ctypes.byref(st), _p(workspace),
-                                           workspace.numel(), max_new, int(eos_token_id), int(pad_token_id),
-                                           float(repetition_penalty), float(diversity_rate), float(length_penalty),
-                                           1 if early_stopping else 0, _stream()), "b200mix_beam_search_step")
-    _count(3)
+        _launch("b200mix_beam_search_step", logits, logits.stride(0), B, nb, V, ctypes.byref(st), workspace,
+                workspace.numel(), max_new, int(eos_token_id), int(pad_token_id), float(repetition_penalty),
+                float(diversity_rate), float(length_penalty), 1 if early_stopping else 0, kernels=3)
 
 
 def kv_reorder(layer_kv: torch.Tensor, cache_k, num_beams: int, prompt_len: int, parents: torch.Tensor,
@@ -880,55 +904,60 @@ def kv_reorder(layer_kv: torch.Tensor, cache_k, num_beams: int, prompt_len: int,
     shaped like cache_k (bf16 [B * nb, max_len, kv_heads, head_dim], contiguous); moves the generated positions
     [prompt_len, prompt_len + state[3]) from parent beam to child (parents int32 [max_new, B * nb], column state[0] - 1)
     for every item whose done flag is 0."""
-    _req(layer_kv, torch.int64, "layer_kv"), _req(cache_k, bf16, "cache_k"), _req(parents, torch.int32, "parents")
-    _req(state, torch.int64, "state"), _req(done, torch.int32, "done")
-    rows, max_len = cache_k.shape[:2]
+    c = _Args("kv_reorder")
+    rows, max_len = c("cache_k", cache_k, BF16, (None, None, ...))[:2]
     nb = int(num_beams)
-    if rows % nb or not cache_k.is_contiguous() or layer_kv.numel() % 2 or parents.shape[1] != rows:
-        raise ValueError("kv_reorder: cache / parents shapes do not match num_beams")
-    check(lib.b200mix_kv_reorder(_p(layer_kv), layer_kv.numel() // 2, rows // nb, nb, max_len,
-                                 cache_k[0, 0].numel(), int(prompt_len), parents.shape[0], _p(parents), _p(state),
-                                 _p(done), _stream()), "b200mix_kv_reorder")
-    _count()
+    if rows % nb or layer_kv.numel() % 2:
+        raise ValueError(f"kv_reorder: {rows} cache rows are not a multiple of {nb} beams, or layer_kv holds an odd "
+                         f"number of caches")
+    c("layer_kv", layer_kv, I64), c("parents", parents, I32, (None, rows)), c("state", state, I64, numel=4)
+    c("done", done, I32, numel=rows // nb)
+    c.on_cuda()
+    _launch("b200mix_kv_reorder", layer_kv, layer_kv.numel() // 2, rows // nb, nb, max_len, cache_k[0, 0].numel(),
+            int(prompt_len), parents.shape[0], parents, state, done)
 
 
 def gather_rows(table: torch.Tensor, ids: torch.Tensor) -> torch.Tensor:
     """table bf16 [V, D], ids int64 [n] (device) -> bf16 [n, D]."""
-    _req(table, bf16, "table"), _req(ids, torch.int64, "ids")
-    n, D = ids.numel(), table.shape[1]
-    out = torch.empty(n, D, device=table.device, dtype=bf16)
-    check(lib.b200mix_gather_rows(_p(table), _p(ids), _p(out), n, D, _stream()), "b200mix_gather_rows")
-    _count()
+    c = _Args("gather_rows")
+    D = c("table", table, BF16, (None, None))[1]
+    c("ids", ids, I64)
+    c.on_cuda()
+    out = torch.empty(ids.numel(), D, device=table.device, dtype=bf16)
+    _launch("b200mix_gather_rows", table, ids, out, ids.numel(), D)
     return out
 
 
 def scatter_rows(src: torch.Tensor, idx: torch.Tensor, dst: torch.Tensor) -> torch.Tensor:
     """dst[idx[i]] = src[i]; src bf16 [n, D], idx int64 [n] (device), dst bf16 [*, D] (in place)."""
-    _req(src, bf16, "src"), _req(idx, torch.int64, "idx"), _req(dst, bf16, "dst")
-    check(lib.b200mix_scatter_rows(_p(src), _p(idx), _p(dst), idx.numel(), src.shape[-1], _stream()),
-          "b200mix_scatter_rows")
-    _count()
+    c = _Args("scatter_rows")
+    n, D = c("src", src, BF16, (None, None))
+    c("idx", idx, I64, numel=n), c("dst", dst, BF16, (None, D))
+    c.on_cuda()
+    _launch("b200mix_scatter_rows", src, idx, dst, n, D)
     return dst
 
 
 def broadcast_add(x: torch.Tensor, table: torch.Tensor) -> torch.Tensor:
     """x fp32 [B, N], table fp32 [G, N] -> fp32 [B, G, N]."""
-    _req(x, torch.float32, "x"), _req(table, torch.float32, "table")
-    B, N = x.shape
-    G = table.shape[0]
+    c = _Args("broadcast_add")
+    B, N = c("x", x, F32, (None, None))
+    G = c("table", table, F32, (None, N))[0]
+    c.on_cuda()
     out = torch.empty(B, G, N, device=x.device, dtype=torch.float32)
-    check(lib.b200mix_broadcast_add(_p(x), _p(table), _p(out), B, G, N, _stream()), "b200mix_broadcast_add")
-    _count()
+    _launch("b200mix_broadcast_add", x, table, out, B, G, N)
     return out
 
 
 def head_rmsnorm_inplace(x: torch.Tensor, weight: torch.Tensor, d: int, eps: float = 1e-6) -> torch.Tensor:
     """x bf16 [rows, H, Dpad] view (last dim contiguous): RMSNorm over the first d channels of every head."""
-    _req(x, bf16, "x"), _req(weight, torch.float32, "weight")
-    rows, H, _ = x.shape
-    check(lib.b200mix_head_rmsnorm_inplace(_p(x), rows, H, d, x.stride(0), x.stride(1), _p(weight), float(eps), _stream()),
-          "b200mix_head_rmsnorm_inplace")
-    _count()
+    c = _Args("head_rmsnorm_inplace")
+    rows, H, Dp = c("x", x, BF16, (None, None, None), STRIDED)
+    if d > Dp:
+        raise ValueError(f"head_rmsnorm_inplace: d = {d} is wider than the {Dp} channels of a head")
+    c("weight", weight, F32, numel=d)
+    c.on_cuda()
+    _launch("b200mix_head_rmsnorm_inplace", x, rows, H, d, x.stride(0), x.stride(1), weight, float(eps))
     return x
 
 
@@ -936,34 +965,36 @@ def small_attention(qkv: torch.Tensor, B: int, T: int, S: int, H: int, d: int, *
                     rope_sin=None, q_norm_w=None, k_norm_w=None, eps: float = 1e-6, out=None) -> torch.Tensor:
     """qkv bf16 [B*T*S, 3*H*d] (row = (b*T+t)*S+s) -> bf16 [B*T*S, H*d]; attention along the T axis. qkv and out may
     be row-strided views (last dim contiguous)."""
-    _req(qkv, bf16, "qkv")
+    c = _Args("small_attention")
+    rows = B * T * S
+    for name, t, width in (("qkv", qkv, 3 * H * d), ("out", out, H * d)):
+        if c(name, t, BF16, (rows, None), STRIDED) is not None and t.shape[1] < width:
+            raise ValueError(f"small_attention: {name} has {t.shape[1]} columns, fewer than {width}")
+    c("rope_cos", rope_cos, F32, (T, d // 2)), c("rope_sin", rope_sin, F32, (T, d // 2))
+    c("q_norm_w", q_norm_w, F32, numel=d), c("k_norm_w", k_norm_w, F32, numel=d)
+    c.on_cuda()
     if out is None:
-        out = torch.empty(qkv.shape[0], H * d, device=qkv.device, dtype=bf16)
-    _req(out, bf16, "out")
-    if qkv.stride(-1) != 1 or out.stride(-1) != 1:
-        raise ValueError("small_attention: qkv and out need a contiguous last dimension")
-    with _Timed("small_attention", 2.0 * 2 * qkv.shape[0] * 4 * H * d, "byte"):
-        check(lib.b200mix_small_attention(_p(qkv), _p(out), B, T, S, H, d, qkv.stride(0), out.stride(0), _p(rope_cos),
-                                          _p(rope_sin), _p(q_norm_w), _p(k_norm_w), float(eps), float(scale), _stream()),
-              "b200mix_small_attention")
-    _count()
+        out = torch.empty(rows, H * d, device=qkv.device, dtype=bf16)
+    with _Timed("small_attention", 2.0 * 2 * rows * 4 * H * d, "byte"):
+        _launch("b200mix_small_attention", qkv, out, B, T, S, H, d, qkv.stride(0), out.stride(0), rope_cos, rope_sin,
+                q_norm_w, k_norm_w, float(eps), float(scale))
     return out
 
 
 def patchify3d(x: torch.Tensor, p: int) -> torch.Tensor:
-    B, C, T, H, W = x.shape
-    assert x.is_contiguous() and x.dtype in (torch.float32, bf16)
+    c = _Args("patchify3d")
+    B, C, T, H, W = c("x", x, FLOAT, (None,) * 5)
+    c.on_cuda()
     out = torch.empty(B, T * (H // p) * (W // p), C * p * p, device=x.device, dtype=bf16)
-    check(lib.b200mix_patchify3d(_p(x), 1 if x.dtype == torch.float32 else 0, _p(out), B, C, T, H, W, p, _stream()),
-          "b200mix_patchify3d")
-    _count()
+    _launch("b200mix_patchify3d", x, 1 if x.dtype == torch.float32 else 0, out, B, C, T, H, W, p)
     return out
 
 
 def unpatchify3d(x: torch.Tensor, C: int, T: int, h: int, w: int, p: int) -> torch.Tensor:
+    c = _Args("unpatchify3d")
     B = x.shape[0]
-    assert x.is_contiguous() and x.dtype == bf16
+    c("x", x, BF16, numel=B * T * h * w * p * p * C)
+    c.on_cuda()
     out = torch.empty(B, C, T, h * p, w * p, device=x.device, dtype=torch.float32)
-    check(lib.b200mix_unpatchify3d(_p(x), _p(out), B, C, T, h, w, p, _stream()), "b200mix_unpatchify3d")
-    _count()
+    _launch("b200mix_unpatchify3d", x, out, B, C, T, h, w, p)
     return out

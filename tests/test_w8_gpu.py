@@ -223,6 +223,25 @@ def test_linear_w8_refusals(ops):
         ops.quantize_w8(rnd(24, 128, seed=15), None)
 
 
+@pytest.mark.parametrize("M,kernels", [(8, 1), (128, 2)])
+def test_linear_w8_counts_its_launches(ops, M, kernels):
+    """ops.launches() (bench.py's gpu_launches) counts what an int8 linear starts: the weight-streaming kernel up to
+    SMALL_MAX rows, the bf16 expansion and the GEMM above."""
+    wq = ops.quantize_w8(rnd(256, 128, seed=30), torch.empty(256 * 128, device="cuda", dtype=bf16))
+    a = rnd(M, 128, seed=31)
+    ops.linear(a, wq)
+    torch.cuda.synchronize()
+    before = ops.launches()
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        torch.zeros(1, device="cuda")  # a torch kernel first: the trace can miss the first kernel of its window
+        torch.cuda.synchronize()
+        ops.linear(a, wq)
+        torch.cuda.synchronize()
+    names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
+    seen = [n for n in names if "at::" not in n]
+    assert ops.launches() - before == len(seen) == kernels, names
+
+
 # ---- the decoder with quant_type="weight_only_int8" ------------------------------------------------------------------
 def _padded(cfg, grid, n_text, seed=7):
     g = torch.Generator().manual_seed(seed)
