@@ -32,7 +32,9 @@ typedef enum b200mix_status {
   B200MIX_ERR_UNSUPPORTED = -4
 } b200mix_status;
 
-enum { B200MIX_ACT_NONE = 0, B200MIX_ACT_SILU = 1, B200MIX_ACT_GELU_ERF = 2, B200MIX_ACT_GELU_TANH = 3, B200MIX_ACT_QUICK_GELU = 4 };
+/* B200MIX_ACT_RELU is taken by b200mix_activation only; the GEMM epilogues cover NONE .. QUICK_GELU. */
+enum { B200MIX_ACT_NONE = 0, B200MIX_ACT_SILU = 1, B200MIX_ACT_GELU_ERF = 2, B200MIX_ACT_GELU_TANH = 3, B200MIX_ACT_QUICK_GELU = 4,
+       B200MIX_ACT_RELU = 5 };
 enum { B200MIX_GLU_NONE = 0, B200MIX_GLU_GEGLU = 1, B200MIX_GLU_SWIGLU = 2 };
 
 /* Fused GEMM epilogue, applied in this order on the fp32 accumulator of element (m, n):
@@ -231,7 +233,8 @@ int b200mix_timestep_embedding(const float* t, void* out, int32_t out_fp32, int6
                                int64_t col0, int32_t flip_sin_to_cos, float downscale_freq_shift, float scale,
                                float max_period, void* stream);
 
-/* y = act(x) elementwise for bf16/fp32 vectors (SiLU on temb, resnet.py:772-776). */
+/* y = act(x) elementwise for bf16/fp32 vectors (SiLU on temb, resnet.py:772-776; ReLU = max(x, 0), the nn.ReLU of the
+ * T2I-Adapter resnet blocks, models/adapter.py:450,571). act is any B200MIX_ACT_*; y may alias x. */
 int b200mix_activation(const void* x, void* y, int64_t n, int32_t act, int32_t x_fp32, int32_t y_fp32, void* stream);
 
 /* Nearest-neighbour x2 upsample NHWC bf16 (F.interpolate(scale_factor=2, mode="nearest"), resnet.py:197-199). */
@@ -246,6 +249,26 @@ int b200mix_nchw_to_nhwc(const void* x, int32_t x_fp32, void* y, int64_t B, int6
                          void* stream);
 int b200mix_nhwc_to_nchw(const void* x, void* y, int32_t y_fp32, int64_t B, int64_t C, int64_t H, int64_t W,
                          void* stream);
+
+/* T2I-Adapter input, nn.PixelUnshuffle(f) + the cast to the model dtype (models/adapter.py:306,328): x fp32|bf16 NCHW
+ * [B,C,H,W] -> y bf16 NHWC [B,H/f,W/f,C*f*f] with y[b,h,w,c*f*f + i*f + j] = x[b,c,h*f+i,w*f+j]. f is 8 or 16; H and W
+ * must be multiples of f; x and y 16-byte aligned. Each input pixel is read once, each thread writes one 16-byte piece
+ * (8 channels = 8 neighbouring pixels of one input row). */
+int b200mix_pixel_unshuffle(const void* x, int32_t x_fp32, void* y, int64_t B, int64_t C, int64_t H, int64_t W, int32_t f,
+                            void* stream);
+
+/* nn.AvgPool2D(kernel_size=2, stride=2, ceil_mode=True) with Paddle's default exclusive=True (models/adapter.py:411,537)
+ * on bf16 NHWC: y [B,ceil(H/2),ceil(W/2),C]; a window that overhangs an odd edge averages its valid pixels only. Sums
+ * in fp32, rounded once. C % 8 == 0, x and y 16-byte aligned. */
+int b200mix_avgpool2x2_nhwc(const void* x, void* y, int64_t B, int64_t H, int64_t W, int64_t C, void* stream);
+
+/* T2I-Adapter residuals (MultiAdapter.forward, models/adapter.py:85-100, and the scale / tile / CFG concat of
+ * pipeline_stable_diffusion_adapter.py:823-836) in one pass over bf16 row-major tensors:
+ *   y[r, :] = sum_k weight[k] * x_k[r mod rows_k, :]     (r < rows_out, fp32 sum in k order, rounded once)
+ * n inputs (1..8) given as host arrays of device pointers, row counts and weights; each x_k is [rows_k, row_elems].
+ * row_elems % 8 == 0, every pointer 16-byte aligned; y must not alias an input. */
+int b200mix_weighted_sum_rows(int32_t n, const void* const* x, const int64_t* rows_in, const float* weight, void* y,
+                              int64_t rows_out, int64_t row_elems, void* stream);
 
 /* y = a + r for an NHWC bf16 activation a [B,H,W,C]; r is NHWC bf16 (r_nchw = 0) or the caller's NCHW fp32|bf16 tensor
  * (r_nchw = 1). The ControlNet / T2I-Adapter residual adds of UNet2DConditionModel.forward:

@@ -47,7 +47,8 @@ class BeamState(Structure):
                                               "hyp_step", "hyp_slot", "hyp_count", "hyp_worst", "done", "presence")]
 
 
-ACT_NONE, ACT_SILU, ACT_GELU_ERF, ACT_GELU_TANH, ACT_QUICK_GELU = 0, 1, 2, 3, 4
+ACT_NONE, ACT_SILU, ACT_GELU_ERF, ACT_GELU_TANH, ACT_QUICK_GELU, ACT_RELU = 0, 1, 2, 3, 4, 5
+GEMM_ACTS = (ACT_NONE, ACT_SILU, ACT_GELU_ERF, ACT_GELU_TANH, ACT_QUICK_GELU)  # what the GEMM epilogues implement
 GLU_NONE, GLU_GEGLU, GLU_SWIGLU = 0, 1, 2
 
 # name -> argtypes; every function returns int except the two string getters.
@@ -93,6 +94,10 @@ SIGNATURES = {
     "b200mix_concat_channels": [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p],
     "b200mix_nchw_to_nhwc": [c_void_p, c_int32, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p],
     "b200mix_nhwc_to_nchw": [c_void_p, c_void_p, c_int32, c_int64, c_int64, c_int64, c_int64, c_void_p],
+    "b200mix_pixel_unshuffle": [c_void_p, c_int32, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int32, c_void_p],
+    "b200mix_avgpool2x2_nhwc": [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p],
+    "b200mix_weighted_sum_rows": [c_int32, POINTER(c_void_p), POINTER(c_int64), POINTER(c_float), c_void_p, c_int64,
+                                  c_int64, c_void_p],
     "b200mix_add_residual_nhwc": [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int64, c_int64, c_int64, c_int64,
                                   c_void_p],
     "b200mix_ddim_step_ex": [c_void_p, c_void_p, c_int32, c_float, c_void_p, c_void_p, c_int64, c_float, c_float,

@@ -16,6 +16,7 @@ __device__ __forceinline__ float ew_act(float v, int act) {
       return 0.5f * v * (1.0f + tanhf(u));
     }
     case B200MIX_ACT_QUICK_GELU: return v / (1.0f + expf(-1.702f * v));
+    case B200MIX_ACT_RELU: return v < 0.0f ? 0.0f : v;  // NaN passes through, as in max(x, 0) on the host
     default: return v;
   }
 }
@@ -548,6 +549,110 @@ __global__ void scatter_rows_kernel(const uint4* __restrict__ src, const long lo
   }
 }
 
+// ---- T2I-Adapter (models/adapter.py) -------------------------------------------------------------------------------
+__device__ __forceinline__ void bf16x8_to_f32(const uint4& v, float* f) {
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) f[2 * k] = bf16_lo(w[k]), f[2 * k + 1] = bf16_hi(w[k]);
+}
+__device__ __forceinline__ uint4 f32x8_to_bf16(const float* f) {
+  return make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
+}
+
+// nn.PixelUnshuffle(F): y[b, ho, wo, c*F*F + i*F + j] = x[b, c, ho*F + i, wo*F + j]. One thread per 16-byte output piece:
+// 8 consecutive output channels are 8 neighbouring pixels (j0 .. j0+7) of one input row, read as one or two 16-byte
+// loads. Consecutive threads write consecutive pieces of one output pixel.
+template <int F>
+__global__ void __launch_bounds__(256) pixel_unshuffle_kernel(const void* __restrict__ x, int x_fp32,
+                                                              uint4* __restrict__ y, long long total, int C, int H,
+                                                              int W) {
+  pdl_wait();
+  pdl_launch_dependents();
+  constexpr int RV = F / 8;      // pieces per input row segment
+  constexpr int PV = F * RV;     // pieces per input channel
+  const int Ho = H / F, Wo = W / F, pieces = C * PV;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int p = (int)(i % pieces);
+    long long q = i / pieces;
+    const int wo = (int)(q % Wo);
+    q /= Wo;
+    const int ho = (int)(q % Ho);
+    const long long b = q / Ho;
+    const int c = p / PV, r = p - c * PV;
+    const int row = r / RV, j0 = (r - row * RV) * 8;
+    const long long src = ((b * C + c) * H + (long long)ho * F + row) * W + (long long)wo * F + j0;
+    uint4 out;
+    if (x_fp32) {
+      const float4* s = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(x) + src);
+      const float4 a = __ldg(s), e = __ldg(s + 1);
+      out = make_uint4(pack_bf16x2(a.x, a.y), pack_bf16x2(a.z, a.w), pack_bf16x2(e.x, e.y), pack_bf16x2(e.z, e.w));
+    } else {
+      out = __ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(x) + src));
+    }
+    y[i] = out;
+  }
+}
+
+// nn.AvgPool2D(2, 2, ceil_mode=True, exclusive=True) on bf16 NHWC: one thread per 16-byte piece of an output pixel. The
+// valid pixels of the window are summed in fp32 in row-major order and divided by their count (1, 2 or 4: exact).
+__global__ void __launch_bounds__(256) avgpool2x2_nhwc_kernel(const uint4* __restrict__ x, uint4* __restrict__ y,
+                                                              long long total, int H, int W, int CV) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int Ho = (H + 1) / 2, Wo = (W + 1) / 2;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int cv = (int)(i % CV);
+    long long q = i / CV;
+    const int wo = (int)(q % Wo);
+    q /= Wo;
+    const int ho = (int)(q % Ho);
+    const long long b = q / Ho;
+    const int nh = min(2, H - 2 * ho), nw = min(2, W - 2 * wo);
+    float acc[8] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
+    for (int dy = 0; dy < nh; ++dy) {
+      for (int dx = 0; dx < nw; ++dx) {
+        float v[8];
+        bf16x8_to_f32(__ldg(x + ((b * H + 2 * ho + dy) * W + 2 * wo + dx) * CV + cv), v);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) acc[k] = __fadd_rn(acc[k], v[k]);
+      }
+    }
+    const float inv = 1.0f / (float)(nh * nw);  // a power of two: the product is the exact quotient
+#pragma unroll
+    for (int k = 0; k < 8; ++k) acc[k] = __fmul_rn(acc[k], inv);
+    y[i] = f32x8_to_bf16(acc);
+  }
+}
+
+// y[r, :] = sum_k w[k] * x_k[r mod rows_k, :], one thread per 16-byte piece; products and sums rounded separately in k
+// order, then once to bf16.
+constexpr int kWsumMax = 8;
+struct WsumArgs {
+  const uint4* x[kWsumMax];
+  long long rows[kWsumMax];
+  float w[kWsumMax];
+  int n;
+};
+__global__ void __launch_bounds__(256) weighted_sum_rows_kernel(WsumArgs a, uint4* __restrict__ y, long long total,
+                                                                long long RV) {
+  pdl_wait();
+  pdl_launch_dependents();
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const long long r = i / RV, v = i - r * RV;
+    float acc[8] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
+    for (int k = 0; k < a.n; ++k) {
+      float f[8];
+      bf16x8_to_f32(__ldg(a.x[k] + (r % a.rows[k]) * RV + v), f);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) acc[e] = __fadd_rn(acc[e], __fmul_rn(a.w[k], f[e]));
+    }
+    y[i] = f32x8_to_bf16(acc);
+  }
+}
+
 static inline unsigned ew_grid(long long n, int threads) {
   long long g = (n + threads - 1) / threads;
   const long long cap = (long long)num_sms() * 16;
@@ -576,6 +681,7 @@ extern "C" int b200mix_activation(const void* x, void* y, int64_t n, int32_t act
                                   void* stream) {
   if (int rc = ensure_device()) return rc;
   B200_CHECK_ARG(x && y && n > 0, "activation: bad arguments");
+  B200_CHECK_ARG(act >= B200MIX_ACT_NONE && act <= B200MIX_ACT_RELU, "activation: unknown act %d", (int)act);
   activation_kernel<<<ew_grid(n, 256), 256, 0, ST(stream)>>>(x, y, n, act, x_fp32, y_fp32);
   B200_LAUNCH_CHECK();
   return 0;
@@ -1116,3 +1222,60 @@ extern "C" int b200mix_unpatchify3d(const void* x, float* y, int64_t B, int64_t 
   return 0;
 }
 
+static inline bool aligned16(const void* p) { return reinterpret_cast<uintptr_t>(p) % 16 == 0; }
+
+// nn.PixelUnshuffle + cast, models/adapter.py:306,328 (FullAdapter / FullAdapterXL / LightAdapter.forward)
+extern "C" int b200mix_pixel_unshuffle(const void* x, int32_t x_fp32, void* y, int64_t B, int64_t C, int64_t H,
+                                       int64_t W, int32_t f, void* stream) {
+  if (int rc = ensure_device()) return rc;
+  B200_CHECK_ARG(x && y && aligned16(x) && aligned16(y), "pixel_unshuffle: x and y must be 16-byte aligned device pointers");
+  B200_CHECK_ARG(f == 8 || f == 16, "pixel_unshuffle: downscale factor must be 8 or 16, got %d", (int)f);
+  B200_CHECK_ARG(B > 0 && C > 0 && H > 0 && W > 0, "pixel_unshuffle: bad shape");
+  B200_CHECK_ARG(H % f == 0 && W % f == 0, "pixel_unshuffle: H=%lld and W=%lld must be multiples of %d", (long long)H,
+                 (long long)W, (int)f);
+  B200_CHECK_ARG(B * C * H * W < (1ll << 40) && C * f * f < (1ll << 31) && H < (1ll << 31) && W < (1ll << 31),
+                 "pixel_unshuffle: tensor too large");
+  const long long total = B * C * H * W / 8;
+  auto kernel = f == 8 ? pixel_unshuffle_kernel<8> : pixel_unshuffle_kernel<16>;
+  B200_CUDA(launch_pdl(kernel, dim3(ew_grid(total, 256)), dim3(256), 0, ST(stream), 1, x, (int)(x_fp32 ? 1 : 0),
+                       reinterpret_cast<uint4*>(y), total, (int)C, (int)H, (int)W));
+  return 0;
+}
+
+// nn.AvgPool2D(kernel_size=2, stride=2, ceil_mode=True), models/adapter.py:411,537 (AdapterBlock / LightAdapterBlock)
+extern "C" int b200mix_avgpool2x2_nhwc(const void* x, void* y, int64_t B, int64_t H, int64_t W, int64_t C, void* stream) {
+  if (int rc = ensure_device()) return rc;
+  B200_CHECK_ARG(x && y && aligned16(x) && aligned16(y), "avgpool2x2_nhwc: x and y must be 16-byte aligned device pointers");
+  B200_CHECK_ARG(B > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0, "avgpool2x2_nhwc: bad shape (C must be a multiple of 8)");
+  B200_CHECK_ARG(H < (1ll << 30) && W < (1ll << 30) && C < (1ll << 31), "avgpool2x2_nhwc: tensor too large");
+  const long long total = B * ((H + 1) / 2) * ((W + 1) / 2) * (C / 8);
+  B200_CUDA(launch_pdl(avgpool2x2_nhwc_kernel, dim3(ew_grid(total, 256)), dim3(256), 0, ST(stream), 1,
+                       reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y), total, (int)H, (int)W,
+                       (int)(C / 8)));
+  return 0;
+}
+
+// MultiAdapter.forward's weighted sum (models/adapter.py:85-100) fused with the pipelines' scale, tile and CFG concat
+// (pipeline_stable_diffusion_adapter.py:823-836)
+extern "C" int b200mix_weighted_sum_rows(int32_t n, const void* const* x, const int64_t* rows_in, const float* weight,
+                                         void* y, int64_t rows_out, int64_t row_elems, void* stream) {
+  if (int rc = ensure_device()) return rc;
+  B200_CHECK_ARG(n >= 1 && n <= kWsumMax && x && rows_in && weight, "weighted_sum_rows: 1 to %d inputs", kWsumMax);
+  B200_CHECK_ARG(y && aligned16(y) && rows_out > 0 && row_elems > 0 && row_elems % 8 == 0,
+                 "weighted_sum_rows: y must be 16-byte aligned, rows_out > 0, row_elems a positive multiple of 8");
+  const char* y0 = static_cast<const char*>(y);
+  const char* y1 = y0 + rows_out * row_elems * 2;
+  WsumArgs a = {};
+  a.n = n;
+  for (int k = 0; k < n; ++k) {
+    B200_CHECK_ARG(x[k] && aligned16(x[k]) && rows_in[k] > 0, "weighted_sum_rows: input %d is null, unaligned or empty", k);
+    const char* x0 = static_cast<const char*>(x[k]);
+    const char* x1 = x0 + rows_in[k] * row_elems * 2;
+    B200_CHECK_ARG(x1 <= y0 || y1 <= x0, "weighted_sum_rows: y overlaps input %d", k);
+    a.x[k] = static_cast<const uint4*>(x[k]), a.rows[k] = rows_in[k], a.w[k] = weight[k];
+  }
+  const long long total = rows_out * (row_elems / 8);
+  B200_CUDA(launch_pdl(weighted_sum_rows_kernel, dim3(ew_grid(total, 256)), dim3(256), 0, ST(stream), 1, a,
+                       reinterpret_cast<uint4*>(y), total, (long long)(row_elems / 8)));
+  return 0;
+}

@@ -7,8 +7,8 @@ from typing import Optional
 import torch
 
 from . import _lib
-from ._lib import (ACT_GELU_ERF, ACT_GELU_TANH, ACT_NONE, ACT_QUICK_GELU, ACT_SILU, GLU_GEGLU, GLU_NONE, GLU_SWIGLU,
-                   Epilogue, check, lib)
+from ._lib import (ACT_GELU_ERF, ACT_GELU_TANH, ACT_NONE, ACT_QUICK_GELU, ACT_RELU, ACT_SILU, GEMM_ACTS, GLU_GEGLU,
+                   GLU_NONE, GLU_SWIGLU, Epilogue, check, lib)
 
 bf16 = torch.bfloat16
 _launches = 0  # number of our kernels launched (bench.py reports it as gpu_launches)
@@ -137,6 +137,18 @@ class _Args:
         for name, t in self.seen:
             if not t.is_cuda:
                 raise _lib.B200MixError(f"{self.op}: {name} must be a CUDA tensor (b200mix has no CPU path)")
+
+
+def _gemm_act(op, act):
+    """The GEMM epilogues implement ACT_NONE .. ACT_QUICK_GELU; ACT_RELU is an element-wise pass (activation())."""
+    if act not in GEMM_ACTS:
+        raise ValueError(f"{op}: act {act} is not a GEMM epilogue activation (ReLU runs through ops.activation)")
+
+
+def _aligned16(op, **tensors):
+    for name, t in tensors.items():
+        if t is not None and t.data_ptr() % 16:
+            raise ValueError(f"{op}: {name} must start on a 16-byte boundary")
 
 
 def init(device: int = 0):
@@ -325,6 +337,7 @@ def linear(a: torch.Tensor, w, bias=None, *, act=ACT_NONE, glu=GLU_NONE, residua
     stats=True or a ZEROED int64 [M, 2] tensor (RowStats.arena): also returns the RowStats of the output rows
     (-> (out, RowStats)); ln=(RowStats of a's rows, colsum, eps[, rms]): a is the UN-normalised tensor and w / bias carry
     the folded affine (fold_layernorm_into_linear)."""
+    _gemm_act("linear", act)
     if isinstance(w, Int8Weight):
         unsupported = [n for n, on in (("row_add", row_add is not None), ("row_gate", row_gate is not None),
                                        ("rows_per_group", rows_per_group), ("out_scale", out_scale != 1.0),
@@ -373,6 +386,7 @@ def linear_batched(a: torch.Tensor, w: torch.Tensor, bias=None, *, out: torch.Te
     """a: bf16 [B, rows, K] view (last dim contiguous, arbitrary row / batch strides); out: [B, rows, N(/2)] view with
     last dim contiguous (e.g. a token range of a joint [B, n_img+n_txt, *] buffer). Per-batch row_add / row_gate."""
     c = _Args("linear_batched")
+    _gemm_act("linear_batched", act)
     B, rows, K = c("a", a, BF16, (None, None, None), ROWS)
     N = c("weight", w, BF16, (None, K), ROWS)[0]
     n_out = N // 2 if glu else N
@@ -418,6 +432,7 @@ def conv3x3(x: torch.Tensor, w: torch.Tensor, bias=None, *, stride=1, row_add=No
             out_scale=1.0, out=None) -> torch.Tensor:
     """x: bf16 NHWC [B,H,W,Cin] contiguous; w: bf16 [Cout,3,3,Cin] contiguous; returns bf16 NHWC."""
     c = _Args("conv3x3")
+    _gemm_act("conv3x3", act)
     B, H, W, Cin = c("x", x, BF16, (None,) * 4)
     Cout = c("w", w, BF16, (None, 3, 3, Cin))[0]
     Ho, Wo = H // stride, W // stride
@@ -458,6 +473,7 @@ def conv3x3_up2x(x: torch.Tensor, w4: torch.Tensor, bias=None, *, row_add=None, 
     """conv3x3(nearest_upsample_2x(x)) from the low-resolution x: bf16 NHWC [B,H,W,Cin]; w4 = fold_upsample_conv_weight(w).
     Returns bf16 NHWC [B,2H,2W,Cout] (Upsample2D, resnet.py:169-218)."""
     c = _Args("conv3x3_up2x")
+    _gemm_act("conv3x3_up2x", act)
     B, H, W, Cin = c("x", x, BF16, (None,) * 4)
     Cout = c("w4", w4, BF16, (None, 16, Cin))[0]
     c("out", out, BF16, (B, 2 * H, 2 * W, Cout)), c("residual", residual, BF16, (B, 2 * H, 2 * W, Cout))
@@ -634,7 +650,10 @@ def timestep_embedding(t: torch.Tensor, dim: int, *, flip_sin_to_cos=True, downs
 
 
 def activation(x: torch.Tensor, act: int, out_dtype=None):
+    """act(x) element-wise, bf16 / fp32 in and out; act is any ACT_* (ACT_RELU only here, not in the GEMMs)."""
     c = _Args("activation")
+    if act not in GEMM_ACTS + (ACT_RELU,):
+        raise ValueError(f"activation: unknown act {act}")
     c("x", x, FLOAT)
     out = torch.empty_like(x, dtype=out_dtype or x.dtype)
     c("out", out, FLOAT)
@@ -681,6 +700,74 @@ def nhwc_to_nchw(x: torch.Tensor, out_dtype=torch.float32, out=None):
     c.on_cuda()
     _launch("b200mix_nhwc_to_nchw", x, out, 1 if out.dtype == torch.float32 else 0, B, C, H, W)
     return out
+
+
+def pixel_unshuffle(x: torch.Tensor, f: int) -> torch.Tensor:
+    """nn.PixelUnshuffle(f) + the cast to bf16: x fp32 / bf16 NCHW [B,C,H,W] (H, W multiples of f; f 8 or 16) ->
+    bf16 NHWC [B,H/f,W/f,C*f*f], channel c*f*f + i*f + j = x[b, c, h*f + i, w*f + j]."""
+    c = _Args("pixel_unshuffle")
+    B, C, H, W = c("x", x, FLOAT, (None,) * 4)
+    if f not in (8, 16):
+        raise ValueError(f"pixel_unshuffle: downscale factor must be 8 or 16, got {f}")
+    if H % f or W % f:
+        raise ValueError(f"pixel_unshuffle: H={H} and W={W} must be multiples of {f}")
+    _aligned16("pixel_unshuffle", x=x)
+    c.on_cuda()
+    out = torch.empty(B, H // f, W // f, C * f * f, device=x.device, dtype=bf16)
+    nbytes = x.numel() * x.element_size() + out.numel() * 2
+    with _Timed("adapter_io", nbytes, "byte", lambda: f"unshuffle{f} {B}x{C}x{H}x{W}"):
+        _launch("b200mix_pixel_unshuffle", x, 1 if x.dtype == torch.float32 else 0, out, B, C, H, W, int(f))
+    return out
+
+
+def avgpool2x2_nhwc(x: torch.Tensor) -> torch.Tensor:
+    """nn.AvgPool2D(kernel_size=2, stride=2, ceil_mode=True) (exclusive: a window over an odd edge averages its valid
+    pixels) on bf16 NHWC [B,H,W,C], C % 8 == 0. Returns bf16 NHWC [B,ceil(H/2),ceil(W/2),C]."""
+    c = _Args("avgpool2x2_nhwc")
+    B, H, W, C = c("x", x, BF16, (None,) * 4)
+    if C % 8:
+        raise ValueError(f"avgpool2x2_nhwc: C={C} must be a multiple of 8")
+    _aligned16("avgpool2x2_nhwc", x=x)
+    c.on_cuda()
+    out = torch.empty(B, (H + 1) // 2, (W + 1) // 2, C, device=x.device, dtype=bf16)
+    with _Timed("adapter_io", 2.0 * (x.numel() + out.numel()), "byte", lambda: f"avgpool {B}x{H}x{W}x{C}"):
+        _launch("b200mix_avgpool2x2_nhwc", x, out, B, H, W, C)
+    return out
+
+
+def weighted_sum_rows(xs, weights, out: torch.Tensor) -> torch.Tensor:
+    """out[r] = sum_k weights[k] * xs[k][r % xs[k].shape[0]], summed in fp32 and rounded to bf16 once. xs: 1 to 8 bf16
+    contiguous tensors [rows_k, ...] with out's trailing shape; out: bf16 contiguous [rows, ...], not overlapping any
+    input; the row size a multiple of 8. The T2I-Adapter residual write: weighted sum, scale, tile and CFG doubling."""
+    c = _Args("weighted_sum_rows")
+    xs, weights = list(xs), [float(w) for w in weights]
+    if not 1 <= len(xs) <= 8 or len(weights) != len(xs):
+        raise ValueError(f"weighted_sum_rows: 1 to 8 inputs with one weight each, got {len(xs)} and {len(weights)}")
+    tail = c("out", out, BF16, (None, ...))[1:]
+    for k, x in enumerate(xs):
+        c(f"xs[{k}]", x, BF16, (None, *tail))
+    row = out[0].numel()
+    if row % 8:
+        raise ValueError(f"weighted_sum_rows: {row} elements per row, must be a multiple of 8")
+    _aligned16("weighted_sum_rows", out=out, **{f"xs[{k}]": x for k, x in enumerate(xs)})
+    c.on_cuda()
+    n = len(xs)
+    ptrs = (ctypes.c_void_p * n)(*[x.data_ptr() for x in xs])
+    rows = (ctypes.c_int64 * n)(*[x.shape[0] for x in xs])
+    ws = (ctypes.c_float * n)(*weights)
+    with _Timed("adapter_io", 2.0 * (sum(x.numel() for x in xs) + out.numel()), "byte",
+                lambda: f"wsum {n}x{out.shape[0]}x{row}"):
+        _launch("b200mix_weighted_sum_rows", n, ptrs, rows, ws, out, out.shape[0], row)
+    return out
+
+
+def zero_(t: torch.Tensor) -> torch.Tensor:
+    """Sets a contiguous device tensor to zero (a memset on the current stream, not a kernel)."""
+    c = _Args("zero_")
+    c("t", t, (bf16, torch.float32, torch.int32, torch.int64))
+    c.on_cuda()
+    check(lib.b200mix_zero_bytes(_p(t), t.numel() * t.element_size(), _stream()), "b200mix_zero_bytes")
+    return t
 
 
 def add_residual_nhwc(a: torch.Tensor, r: torch.Tensor, *, r_nchw: bool, out=None) -> torch.Tensor:

@@ -17,6 +17,7 @@ from typing import Any, Dict, List, Optional, Union
 
 import torch
 
+from .adapter import MultiAdapter
 from .controlnet import MultiControlNetModel, controlnet_keep
 from .schedulers import DDIMScheduler
 from .unet_2d_condition import UNet2DConditionModel
@@ -31,10 +32,11 @@ class GraphedUNet:
     residuals to the UNet; the conditioning embeddings and the fp32 scale tables are static buffers too
     (`cond_embeddings` / `scale_tables` of __call__), so new scales need no new capture. `controlnet_rows` < rows:
     the ControlNet runs on the last `controlnet_rows` rows only (guess mode with CFG) and the residuals of the other
-    rows stay zero."""
+    rows stay zero. With `intrablock_residuals` (bf16 NHWC [rows, h, w, c] device buffers) the graph hands them to the
+    UNet as down_intrablock_additional_residuals (T2I-Adapter); the caller writes new values into them between replays."""
 
     def __init__(self, unet: UNet2DConditionModel, sample_shape, ctx_shape, added_cond_shapes: Optional[Dict[str, Any]] = None,
-                 warmup: int = 2, controlnet=None, controlnet_rows: Optional[int] = None):
+                 warmup: int = 2, controlnet=None, controlnet_rows: Optional[int] = None, intrablock_residuals=None):
         from .. import ops
         dev = unet.device
         self.unet = unet
@@ -48,12 +50,16 @@ class GraphedUNet:
         self.cn = None
         if controlnet is not None:
             self.cn = controlnet_state(controlnet, sample_shape, controlnet_rows or sample_shape[0], dev)
+        self.intra = None if intrablock_residuals is None else list(intrablock_residuals)
         self.out = None
         self.launches_per_replay = 0
 
         def run():
             x = ops.nchw_to_nhwc(self.sample)
-            if controlnet is None:
+            if self.intra is not None:
+                y = unet.forward_nhwc(x, self.t, self.ctx, self.added, down_intrablock_additional_residuals=self.intra,
+                                      residuals_nchw=False)
+            elif controlnet is None:
                 y = unet.forward_nhwc(x, self.t, self.ctx, self.added)
             else:
                 y = denoise_with_controlnet(unet, controlnet, x, self.t, self.ctx, self.added, self.cn)
@@ -368,6 +374,117 @@ class StableDiffusionControlNetPipeline(StableDiffusionPipeline):
         tt = torch.full((model_in.shape[0],), float(t), device=self.unet.device, dtype=torch.float32)
         y = denoise_with_controlnet(self.unet, self.controlnet, ops.nchw_to_nhwc(model_in), tt, ctx, added, st)
         return ops.nhwc_to_nchw(y, out_dtype=bf16)
+
+
+class StableDiffusionAdapterPipeline(StableDiffusionPipeline):
+    """Loop-only mirror of ppdiffusers.StableDiffusionAdapterPipeline / StableDiffusionXLAdapterPipeline.__call__
+    (pipeline_stable_diffusion_adapter.py:757-870, pipeline_stable_diffusion_xl_adapter.py:1019-1050). The adapter
+    does not depend on the timestep: it runs once per call, and one b200mix_weighted_sum_rows pass per feature writes
+    w * features into static bf16 NHWC residual buffers [rows, h, w, c]. That pass applies adapter_conditioning_scale
+    (the MultiAdapter weights), the tile to the prompt batch and the CFG doubling at once. Each step is then the UNet
+    with those residuals (one CUDA graph per shape and adapter) and the CFG combine + scheduler kernel. Steps
+    i >= int(num_inference_steps * adapter_conditioning_factor) run with the buffers zeroed: bf16 h + 0 is h, so the
+    same graph serves them.
+    `adapter`: a T2IAdapter, a MultiAdapter or a list of T2IAdapters."""
+
+    def __init__(self, unet: UNet2DConditionModel, adapter, scheduler: DDIMScheduler, use_cuda_graph: bool = True,
+                 vae=None):
+        super().__init__(unet, scheduler, use_cuda_graph=use_cuda_graph, vae=vae)
+        if isinstance(adapter, (list, tuple)):
+            adapter = MultiAdapter(adapter)
+        self.adapter = adapter
+        self._adapter = None  # the adapter arguments of the call in progress
+
+    @torch.no_grad()
+    def __call__(self, prompt=None, height: Optional[int] = None, width: Optional[int] = None,
+                 image: Union[torch.Tensor, List[torch.Tensor]] = None, num_inference_steps: int = 50,
+                 guidance_scale: float = 7.5, negative_prompt=None, eta: float = 0.0,
+                 latents: Optional[torch.Tensor] = None, prompt_embeds: Optional[torch.Tensor] = None,
+                 negative_prompt_embeds: Optional[torch.Tensor] = None, output_type: str = "latent",
+                 adapter_conditioning_scale: Union[float, List[float]] = 1.0, adapter_conditioning_factor: float = 1.0,
+                 added_cond_kwargs: Optional[Dict[str, torch.Tensor]] = None,
+                 negative_added_cond_kwargs: Optional[Dict[str, torch.Tensor]] = None, callback_on_step_end=None,
+                 generator: Optional[torch.Generator] = None, guidance_rescale: float = 0.0):
+        """`image`: the adapter input, fp32 [B | 1, C, H, W] in [0, 1] (a list of them, one per adapter, for a
+        MultiAdapter), with H and W 8x the latent size; loading and resizing images is the caller's job.
+        `adapter_conditioning_scale`: a float, or for a MultiAdapter a list of one weight per adapter.
+        Other arguments as StableDiffusionPipeline.__call__."""
+        multi = isinstance(self.adapter, MultiAdapter)
+        if image is None:
+            raise ValueError("`image` (the adapter input) is required")
+        if multi:  # pipeline_stable_diffusion_adapter.py:543-552
+            if not isinstance(image, list):
+                raise ValueError("MultiAdapter is enabled, but `image` is not a list. Please pass a list of images to "
+                                 "`image`.")
+            if len(image) != self.adapter.num_adapter:
+                raise ValueError(f"MultiAdapter requires passing the same number of images as adapters. Given "
+                                 f"{len(image)} images and {self.adapter.num_adapter} adapters.")
+            images, weights = image, self.adapter.weights(adapter_conditioning_scale)  # passed as weights (:823-826)
+        else:
+            if not torch.is_tensor(image):
+                raise ValueError(f"a single T2IAdapter takes one image tensor, got {type(image).__name__}")
+            images, weights = [image], [float(adapter_conditioning_scale)]  # v * scale (:827-830)
+        self._adapter = dict(images=images, weights=weights,
+                             cut=int(num_inference_steps * adapter_conditioning_factor))  # xl :1029-1032
+        try:
+            return super().__call__(prompt=prompt, height=height, width=width, num_inference_steps=num_inference_steps,
+                                    guidance_scale=guidance_scale, negative_prompt=negative_prompt, eta=eta,
+                                    latents=latents, prompt_embeds=prompt_embeds,
+                                    negative_prompt_embeds=negative_prompt_embeds, output_type=output_type,
+                                    added_cond_kwargs=added_cond_kwargs,
+                                    negative_added_cond_kwargs=negative_added_cond_kwargs,
+                                    callback_on_step_end=callback_on_step_end, generator=generator,
+                                    guidance_rescale=guidance_rescale)
+        finally:
+            self._adapter = None
+
+    def _begin(self, sample_shape, ctx, added, B, do_cfg):
+        from .. import ops
+        c = self._adapter
+        dev = self.unet.device
+        rows, _, H, W = sample_shape
+        adapters = self.adapter.adapters if isinstance(self.adapter, MultiAdapter) else [self.adapter]
+        feats = []
+        for adapter, img in zip(adapters, c["images"]):
+            if img.dim() != 4 or img.shape[0] not in (1, B):
+                raise ValueError(f"adapter image of shape {tuple(img.shape)} must be [1 or {B}, C, H, W]")
+            if tuple(img.shape[2:]) != (8 * H, 8 * W):
+                raise ValueError(f"adapter image {tuple(img.shape[2:])} does not match the latents {(H, W)} (8x)")
+            feats.append(adapter.forward(img.to(device=dev, dtype=torch.float32)))
+        shapes = [tuple(f.shape[1:]) for f in feats[0]]
+        den = None
+        if self.use_cuda_graph:
+            key = ("adapter", id(self.adapter), tuple(sample_shape), tuple(ctx.shape), tuple(shapes),
+                   None if added is None else tuple((k, tuple(v.shape)) for k, v in added.items()))
+            den = self._graphed.get(key)
+            if den is None:
+                bufs = [torch.zeros((rows,) + s, device=dev, dtype=bf16) for s in shapes]
+                den = GraphedUNet(self.unet, sample_shape, ctx.shape,
+                                  None if added is None else {k: v.shape for k, v in added.items()},
+                                  intrablock_residuals=bufs)
+                self._graphed[key] = den
+            c["bufs"] = den.intra
+        else:
+            c["bufs"] = [torch.empty((rows,) + s, device=dev, dtype=bf16) for s in shapes]
+        for k, buf in enumerate(c["bufs"]):
+            ops.weighted_sum_rows([f[k] for f in feats], c["weights"], out=buf)
+        return den
+
+    def _predict(self, den, i, t, model_in, ctx, added, first):
+        from .. import ops
+        c = self._adapter
+        if i == c["cut"]:  # from here on without residuals
+            for buf in c["bufs"]:
+                ops.zero_(buf)
+        if den is not None:
+            return den(model_in, float(t), ctx if first else None, added if first else None)
+        tt = torch.full((model_in.shape[0],), float(t), device=self.unet.device, dtype=torch.float32)
+        y = self.unet.forward_nhwc(ops.nchw_to_nhwc(model_in), tt, ctx, added,
+                                   down_intrablock_additional_residuals=c["bufs"], residuals_nchw=False)
+        return ops.nhwc_to_nchw(y, out_dtype=bf16)
+
+
+StableDiffusionXLAdapterPipeline = StableDiffusionAdapterPipeline  # the SDXL loop is the same class (added_cond_kwargs)
 
 
 class StableDiffusion3Pipeline:
