@@ -153,6 +153,15 @@ __device__ __forceinline__ void wgmma_fence_operands(float (&d)[R]) {
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// Same for the bf16x2 A fragments of a register-operand wgmma: they are read asynchronously until wgmma_wait
+template <int R, int C>
+__device__ __forceinline__ void wgmma_fence_operands(uint32_t (&a)[R][C]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i)
+#pragma unroll
+    for (int j = 0; j < C; ++j) asm volatile("" : "+r"(a[i][j])::"memory");
+}
+
 // D[64 x N] (+)= A[64 x 16] B[16 x N]: A and B K-major in shared memory (scale_d = 0 overwrites D)
 __device__ __forceinline__ void wgmma_ss(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
@@ -302,6 +311,10 @@ __device__ __forceinline__ void setmaxnreg_inc() {
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+// Signal a named barrier without waiting on it: the other nthreads - (this warp group) threads complete it with bar.sync
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
 }  // namespace b200
