@@ -191,7 +191,7 @@ def get_timestep_embedding(timesteps, embedding_dim, flip_sin_to_cos=False, down
     """ppdiffusers/models/embeddings.py:26-64."""
     assert timesteps.ndim == 1
     half_dim = embedding_dim // 2
-    exponent = -math.log(max_period) * torch.arange(0, half_dim, dtype=torch.float32)
+    exponent = -math.log(max_period) * torch.arange(0, half_dim, dtype=torch.float32, device=timesteps.device)
     exponent = exponent / (half_dim - downscale_freq_shift)
     emb = torch.exp(exponent)
     emb = timesteps[:, None].to(torch.float32) * emb[None, :]

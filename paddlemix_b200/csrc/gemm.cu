@@ -58,7 +58,7 @@ struct IGemmParams {
   const float* ln_colsum;     // consumer: [N] sum_k W'[n, k]
   int ln_rms;
   float ln_eps;
-  float ln_inv_k;             // 2^-24 / K
+  double ln_inv_k;            // 2^-24 / K
   // stream-K head (see SegIter): the first sk_tiles super-tiles are cut into equal k-block ranges, one per cluster
   int sk_tiles;
   float4* sk_ws;          // [cluster][cta rank][n8 block][consumer thread] fp32 partial accumulators (fragment layout)
@@ -416,15 +416,14 @@ __global__ void __launch_bounds__(IG_THREADS, 1)
       named_bar_sync(2 + grp, 128);
       float ln_rstd[2] = {1.0f, 1.0f}, ln_shift[2] = {0.0f, 0.0f};
       if (LNM == LNM_CONSUMER) {  // mean / rstd of my rows from the totals the producing GEMM's epilogues accumulated
-        // fp32 on purpose (FP64 is slow on the epilogue's critical path). E[x^2] - mean^2 in fp32 is good to
-        // ~1e-7 * mean^2 / var relative: below the bf16 resolution of the inputs themselves for any row bf16 can
-        // represent (|mean| / std < 2^8).
+        // in fp64: E[x^2] - mean^2 cancels mean^2 / var, so fp32 loses ~2^-24 * mean^2 / var of the variance (2^-8 at
+        // |mean| / std = 2^8). A handful of fp64 operations per row and tile, off the MMA critical path.
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const float mean = p.ln_rms ? 0.0f : __ll2float_rn(t_stats[h].x) * p.ln_inv_k;
-          const float var = fmaxf(fmaf(-mean, mean, __ll2float_rn(t_stats[h].y) * p.ln_inv_k), 0.0f);
-          ln_rstd[h] = rsqrtf(var + p.ln_eps);
-          ln_shift[h] = -ln_rstd[h] * mean;
+          const double mean = p.ln_rms ? 0.0 : __ll2double_rn(t_stats[h].x) * p.ln_inv_k;
+          const double var = fmax(fma(-mean, mean, __ll2double_rn(t_stats[h].y) * p.ln_inv_k), 0.0);
+          ln_rstd[h] = rsqrtf(static_cast<float>(var) + p.ln_eps);
+          ln_shift[h] = static_cast<float>(-static_cast<double>(ln_rstd[h]) * mean);
         }
       }
       float st_sum[2] = {0.0f, 0.0f}, st_sq[2] = {0.0f, 0.0f};  // producer side: my rows' sum / sum of squares over my columns
@@ -1025,7 +1024,7 @@ static int fill_epilogue(IGemmParams& p, const b200mix_epilogue* e, void* C, lon
   p.ln_stats = reinterpret_cast<const long long*>(e->ln_stats);
   p.ln_colsum = e->ln_colsum;
   p.ln_rms = e->ln_rms, p.ln_eps = e->ln_eps;
-  p.ln_inv_k = static_cast<float>(1.0 / 16777216.0 / static_cast<double>(p.Kc));
+  p.ln_inv_k = 1.0 / 16777216.0 / static_cast<double>(p.Kc);
   B200_CHECK_ARG(!(p.ln_stats || p.stats_out) || p.ntaps == 1, "row statistics (folded LayerNorm) are a Linear feature");
   B200_CHECK_ARG(!p.ln_stats || p.ln_colsum, "ln_stats needs ln_colsum");
   B200_CHECK_ARG(!p.ln_stats || reinterpret_cast<uintptr_t>(p.ln_stats) % 16 == 0, "ln_stats must be 16-byte aligned");
