@@ -346,6 +346,54 @@ int b200mix_euler_step(const void* v_u, const void* v_c, int32_t v_fp32, float g
  * host computes that denominator in fp32, this applies an IEEE fp32 division. */
 int b200mix_scale_model_input(const float* x, float* y, int64_t n, float denom, void* stream);
 
+/* EulerAncestralDiscreteScheduler.step ("Euler a", scheduling_euler_ancestral_discrete.py:268-357), fused with the CFG
+ * combine, fp32 state, one rounding per operation in this order:
+ *   m = m_u + g*(m_c - m_u)   (m_c NULL => m = m_u); m_u, m_c bf16 or fp32 (m_fp32)
+ *   prediction_type 0 (epsilon):      x0 = x - sigma*m
+ *   prediction_type 2 (v_prediction): x0 = m*c_out + x/s2p1   (c_out = -sigma/(sigma^2+1)^0.5, s2p1 = sigma^2+1)
+ *   d = (x - x0)/sigma;  x_prev = x + d*dt;  x_prev = x_prev + z*sigma_up
+ * The same arithmetic as b200mix_euler_step up to the noise term. The host computes in fp32, in the order of
+ * :339-347, sigma_up = (sigma_to^2*(sigma_from^2 - sigma_to^2)/sigma_from^2)^0.5,
+ * sigma_down = (sigma_to^2 - sigma_up^2)^0.5 and dt = sigma_down - sigma. z is noise[i] (fp32, x's element count) or,
+ * with noise NULL, the Philox stream of b200mix_iddpm_step keyed by (seed, step): element group g = elements
+ * 4g .. 4g+3 takes the four normals of philox4x32_10(counter = (step, g mod 2^32, g div 2^32, 0),
+ * key = (seed mod 2^32, seed div 2^32)). x_prev may alias x. */
+int b200mix_euler_ancestral_step(const void* m_u, const void* m_c, int32_t m_fp32, float guidance, const float* x,
+                                 const float* noise, float* x_prev, int64_t n, int32_t prediction_type, float sigma,
+                                 float c_out, float s2p1, float dt, float sigma_up, uint64_t seed, int64_t step,
+                                 void* stream);
+
+/* Host-computed fp32 scalars of one b200mix_unipc_step (see there). */
+typedef struct {
+  float alpha_t, sigma_t;       /* convert_model_output at the current sigma (_sigma_to_alpha_sigma_t) */
+  float A_c, K_c, E_c, rc_last; /* UniC: sigma_t/sigma_s0, alpha_t*h_phi_1, alpha_t*B_h, rhos_c[-1] */
+  float rc[2], rk_c[2];         /* UniC history terms k = 0, 1: rhos_c[k], rks[k] */
+  float A_p, K_p, E_p;          /* UniP: sigma_t/sigma_s0, alpha_t*h_phi_1, alpha_t*B_h */
+  float rp[2], rk_p[2];         /* UniP history terms k = 0, 1: rhos_p[k], rks[k] */
+} b200mix_unipc_coeffs;
+
+/* UniPCMultistepScheduler.step with predict_x0 = True, solver_type bh1 / bh2, orders 1-3
+ * (scheduling_unipc_multistep.py:720-804, convert_model_output :368-437, UniC :567-701, UniP :438-565), one launch,
+ * fp32 state, one rounding per operation in this order (c = *coeffs):
+ *   m  = m_u + g*(m_c - m_u)   (m_c NULL => m = m_u); m_u, m_c bf16 or fp32 (m_fp32)
+ *   m0 = x0 of m at the uncorrected sample x, as b200mix_ddim_step_ex with sa_t = c.alpha_t, sb_t = c.sigma_t
+ *        (prediction_type 0 epsilon, 1 sample, 2 v_prediction)
+ *   UniC (last_sample != NULL; m_prev = the previous step's m0):
+ *     res = c.rc_last*(m0 - m_prev);  corr = sum over present k of c.rc[k]*((hc_k - m_prev)/c.rk_c[k]);
+ *     res = corr + res (only if some hc_k is present);  x_c = (c.A_c*last_sample - c.K_c*m_prev) - c.E_c*res
+ *   else x_c = x
+ *   UniP: x_next = c.A_p*x_c - c.K_p*m0;  pred = sum over present k of c.rp[k]*((hp_k - m0)/c.rk_p[k]);
+ *     x_next = x_next - c.E_p*pred (only if some hp_k is present)
+ * Each sum runs over k = 0, 1 in that order: acc = t_0, then acc = acc + t_1. hc0 / hc1 are the x0 of the steps
+ * before m_prev (most recent first), hp0 / hp1 those before m0 (hp0 = m_prev); a NULL pointer is an absent term and
+ * is not read. Writes m_out = m0 (the history ring's next entry), x_corr = x_c (the next step's last_sample) and
+ * x_next. Every tensor is fp32 with x's element count except m_u / m_c. x_next may alias x and x_corr may alias
+ * last_sample; m_out aliases none of the inputs. */
+int b200mix_unipc_step(const void* m_u, const void* m_c, int32_t m_fp32, float guidance, const float* x,
+                       const float* last_sample, const float* m_prev, const float* hc0, const float* hc1,
+                       const float* hp0, const float* hp1, float* x_next, float* x_corr, float* m_out, int64_t n,
+                       int32_t prediction_type, const b200mix_unipc_coeffs* coeffs, void* stream);
+
 /* DPMSolverMultistepScheduler.step for "dpmsolver++" / midpoint / epsilon prediction ("DPM-Solver++ 2M",
  * scheduling_dpmsolver_multistep.py:801-873), fused with the CFG combine, fp32 state:
  *   x0 = (x - sigma_cur*eps) / alpha_cur                                   (convert_model_output, :446-453)

@@ -47,6 +47,14 @@ class BeamState(Structure):
                                               "hyp_step", "hyp_slot", "hyp_count", "hyp_worst", "done", "presence")]
 
 
+class UnipcCoeffs(Structure):
+    """Mirror of `b200mix_unipc_coeffs` (include/b200mix.h)."""
+
+    _fields_ = [(name, c_float) for name in ("alpha_t", "sigma_t", "A_c", "K_c", "E_c", "rc_last")] + [
+        ("rc", c_float * 2), ("rk_c", c_float * 2), ("A_p", c_float), ("K_p", c_float), ("E_p", c_float),
+        ("rp", c_float * 2), ("rk_p", c_float * 2)]
+
+
 ACT_NONE, ACT_SILU, ACT_GELU_ERF, ACT_GELU_TANH, ACT_QUICK_GELU, ACT_RELU = 0, 1, 2, 3, 4, 5
 GEMM_ACTS = (ACT_NONE, ACT_SILU, ACT_GELU_ERF, ACT_GELU_TANH, ACT_QUICK_GELU)  # what the GEMM epilogues implement
 GLU_NONE, GLU_GEGLU, GLU_SWIGLU = 0, 1, 2
@@ -111,6 +119,10 @@ SIGNATURES = {
     "b200mix_cfg_combine": [c_void_p, c_void_p, c_int32, c_float, c_void_p, c_float, c_int64, c_void_p, c_int64, c_void_p],
     "b200mix_euler_step": [c_void_p, c_void_p, c_int32, c_float, c_void_p, c_void_p, c_int64, c_float, c_float,
                            c_void_p],
+    "b200mix_euler_ancestral_step": [c_void_p, c_void_p, c_int32, c_float, c_void_p, c_void_p, c_void_p, c_int64, c_int32,
+                                     c_float, c_float, c_float, c_float, c_float, c_uint64, c_int64, c_void_p],
+    "b200mix_unipc_step": [c_void_p, c_void_p, c_int32, c_float] + [c_void_p] * 10 + [c_int64, c_int32,
+                                                                                     POINTER(UnipcCoeffs), c_void_p],
     "b200mix_scale_model_input": [c_void_p, c_void_p, c_int64, c_float, c_void_p],
     "b200mix_dpmpp_2m_step": [c_void_p, c_void_p, c_int32, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_float,
                               c_float, c_float, c_float, c_float, c_float, c_void_p],

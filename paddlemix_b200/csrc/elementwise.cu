@@ -1,5 +1,6 @@
 // Small HBM-/latency-bound kernels around the denoiser: timestep embedding, activation, nearest upsample, channel
-// concat, NCHW<->NHWC, conv_in (tiny C_in), fused CFG + DDIM / flow-match Euler / IDDPM step, casts, rotary embedding.
+// concat, NCHW<->NHWC, conv_in (tiny C_in), fused CFG + DDIM / LCM / Euler / Euler-ancestral / DPM-Solver++ / UniPC /
+// IDDPM step, casts, rotary embedding.
 // Reference call sites are cited per function in include/b200mix.h.
 #include "common.cuh"
 #include "philox.cuh"
@@ -425,16 +426,106 @@ __global__ void scale_model_input_kernel(const float* __restrict__ x, float* __r
     y[i] = __fdiv_rn(x[i], denom);
 }
 
+// The deterministic Euler update shared by b200mix_euler_step and b200mix_euler_ancestral_step
+// (scheduling_flow_match_euler_discrete.py:262-270, scheduling_euler_discrete.py:433-463,
+// scheduling_euler_ancestral_discrete.py:327-349), one rounding per operation in this order:
+//   v_pred == 0 (epsilon / flow):  x0 = x - m*sigma
+//   v_pred != 0:                   x0 = m*c_out + x/s2p1     (c_out = -sigma/(sigma^2+1)^0.5, s2p1 = sigma^2+1: host fp32)
+//   d = (x - x0)/sigma;  returns x + d*dt
+__device__ __forceinline__ float euler_update(int v_pred, float m, float x, float sigma, float c_out, float s2p1,
+                                              float dt) {
+  const float x0 = v_pred ? __fadd_rn(__fmul_rn(m, c_out), __fdiv_rn(x, s2p1)) : __fsub_rn(x, __fmul_rn(m, sigma));
+  const float d = __fdiv_rn(__fsub_rn(x, x0), sigma);
+  return __fadd_rn(x, __fmul_rn(d, dt));
+}
+
 __global__ void euler_step_kernel(const void* __restrict__ v_u, const void* __restrict__ v_c, int v_fp32, float guidance,
                                   const float* __restrict__ x, float* __restrict__ x_prev, long long n, float sigma,
                                   float dt) {
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const float v = load_guided(v_u, v_c, i, v_fp32, guidance);
-    // scheduling_flow_match_euler_discrete.py:262-270: denoised = x - v*sigma; derivative = (x - denoised)/sigma_hat
-    const float xi = x[i];
-    const float den = __fsub_rn(xi, __fmul_rn(v, sigma));
-    const float der = __fdiv_rn(__fsub_rn(xi, den), sigma);
-    x_prev[i] = __fadd_rn(xi, __fmul_rn(der, dt));
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    x_prev[i] = euler_update(0, load_guided(v_u, v_c, i, v_fp32, guidance), x[i], sigma, 0.0f, 1.0f, dt);
+}
+
+// EulerAncestralDiscreteScheduler.step: euler_update with dt = sigma_down - sigma, then + z*sigma_up. One thread per
+// group of 4 consecutive elements, which is one Philox call (philox_normal4) when noise is NULL. x_prev may alias x.
+// The minimum of 4 CTAs per SM gives ptxas the registers to keep the fp64 Box-Muller out of local memory.
+__global__ void __launch_bounds__(256, 4) euler_ancestral_step_kernel(
+    const void* __restrict__ m_u, const void* __restrict__ m_c, int m_fp32, float guidance, const float* x,
+    const float* __restrict__ noise, float* x_prev, long long n, int v_pred, float sigma, float c_out, float s2p1,
+    float dt, float sigma_up, unsigned long long seed, uint32_t step) {
+  const long long groups = (n + 3) >> 2;
+  for (long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x; g < groups; g += (long long)gridDim.x * blockDim.x) {
+    float z[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+    if (!noise) philox_normal4(seed, step, (unsigned long long)g, z);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const long long i = 4 * g + k;
+      if (i >= n) break;
+      const float xp = euler_update(v_pred, load_guided(m_u, m_c, i, m_fp32, guidance), x[i], sigma, c_out, s2p1, dt);
+      x_prev[i] = __fadd_rn(xp, __fmul_rn(noise ? noise[i] : z[k], sigma_up));
+    }
+  }
+}
+
+// UniPCMultistepScheduler.step with predict_x0 (scheduling_unipc_multistep.py:720-804): convert_model_output
+// (:368-437), the optional UniC corrector (:567-701) and the UniP predictor (:438-565), one rounding per operation in
+// the order documented at b200mix_unipc_step. The pointers without __restrict__ may alias as documented there.
+struct UnipcArgs {
+  const void* m_u;
+  const void* m_c;
+  const float* x;
+  const float* last;
+  const float* m_prev;
+  const float* hc[2];
+  const float* hp[2];
+  float* x_next;
+  float* x_corr;
+  float* m_out;
+  long long n;
+  int m_fp32, pred_type;
+  float guidance;
+  b200mix_unipc_coeffs k;
+};
+
+// sum_k r[k] * ((h[k][i] - base) / rk[k]) over the present terms in ascending k; `have` tells whether any was present
+__device__ __forceinline__ float unipc_history_sum(const float* const h[2], const float r[2], const float rk[2],
+                                                   long long i, float base, bool& have) {
+  float acc = 0.0f;
+  have = false;
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    if (!h[k]) continue;
+    const float t = __fmul_rn(r[k], __fdiv_rn(__fsub_rn(h[k][i], base), rk[k]));
+    acc = have ? __fadd_rn(acc, t) : t;
+    have = true;
+  }
+  return acc;
+}
+
+__global__ void __launch_bounds__(256) unipc_step_kernel(UnipcArgs a) {
+  const b200mix_unipc_coeffs& k = a.k;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < a.n; i += (long long)gridDim.x * blockDim.x) {
+    const float xi = a.x[i];
+    float m0, unused;
+    predict_x0_eps(a.pred_type, load_guided(a.m_u, a.m_c, i, a.m_fp32, a.guidance), xi, k.alpha_t, k.sigma_t, m0,
+                   unused);
+    float xc = xi;
+    if (a.last) {
+      const float mp = a.m_prev[i];
+      const float base = __fsub_rn(__fmul_rn(k.A_c, a.last[i]), __fmul_rn(k.K_c, mp));
+      float res = __fmul_rn(k.rc_last, __fsub_rn(m0, mp));
+      bool have;
+      const float corr = unipc_history_sum(a.hc, k.rc, k.rk_c, i, mp, have);
+      if (have) res = __fadd_rn(corr, res);
+      xc = __fsub_rn(base, __fmul_rn(k.E_c, res));
+    }
+    float xn = __fsub_rn(__fmul_rn(k.A_p, xc), __fmul_rn(k.K_p, m0));
+    bool have;
+    const float pred = unipc_history_sum(a.hp, k.rp, k.rk_p, i, m0, have);
+    if (have) xn = __fsub_rn(xn, __fmul_rn(k.E_p, pred));
+    a.m_out[i] = m0;
+    a.x_corr[i] = xc;
+    a.x_next[i] = xn;
   }
 }
 
@@ -856,6 +947,41 @@ extern "C" int b200mix_euler_step(const void* v_u, const void* v_c, int32_t v_fp
   if (int rc = ensure_device()) return rc;
   B200_CHECK_ARG(v_u && x && x_prev && n > 0, "euler_step: bad arguments");
   euler_step_kernel<<<ew_grid(n, 256), 256, 0, ST(stream)>>>(v_u, v_c, v_fp32, guidance, x, x_prev, n, sigma, dt);
+  B200_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int b200mix_euler_ancestral_step(const void* m_u, const void* m_c, int32_t m_fp32, float guidance,
+                                            const float* x, const float* noise, float* x_prev, int64_t n,
+                                            int32_t prediction_type, float sigma, float c_out, float s2p1, float dt,
+                                            float sigma_up, uint64_t seed, int64_t step, void* stream) {
+  if (int rc = ensure_device()) return rc;
+  B200_CHECK_ARG(m_u && x && x_prev && n > 0, "euler_ancestral_step: bad arguments");
+  B200_CHECK_ARG(prediction_type == 0 || prediction_type == 2,
+                 "euler_ancestral_step: prediction_type must be 0 (epsilon) or 2 (v_prediction)");
+  B200_CHECK_ARG(step >= 0 && step <= 0xFFFFFFFFll, "euler_ancestral_step: step must fit 32 bits");
+  euler_ancestral_step_kernel<<<ew_grid((n + 3) / 4, 256), 256, 0, ST(stream)>>>(
+      m_u, m_c, m_fp32, guidance, x, noise, x_prev, n, prediction_type == 2, sigma, c_out, s2p1, dt, sigma_up, seed,
+      (uint32_t)step);
+  B200_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int b200mix_unipc_step(const void* m_u, const void* m_c, int32_t m_fp32, float guidance, const float* x,
+                                  const float* last_sample, const float* m_prev, const float* hc0, const float* hc1,
+                                  const float* hp0, const float* hp1, float* x_next, float* x_corr, float* m_out,
+                                  int64_t n, int32_t prediction_type, const b200mix_unipc_coeffs* coeffs, void* stream) {
+  if (int rc = ensure_device()) return rc;
+  B200_CHECK_ARG(m_u && x && x_next && x_corr && m_out && coeffs && n > 0, "unipc_step: bad arguments");
+  B200_CHECK_ARG(prediction_type >= 0 && prediction_type <= 2, "unipc_step: prediction_type must be 0, 1 or 2");
+  B200_CHECK_ARG(!last_sample == !m_prev, "unipc_step: last_sample and m_prev go together (the corrector)");
+  B200_CHECK_ARG(last_sample || (!hc0 && !hc1), "unipc_step: corrector history without the corrector");
+  UnipcArgs a;
+  a.m_u = m_u, a.m_c = m_c, a.x = x, a.last = last_sample, a.m_prev = m_prev;
+  a.hc[0] = hc0, a.hc[1] = hc1, a.hp[0] = hp0, a.hp[1] = hp1;
+  a.x_next = x_next, a.x_corr = x_corr, a.m_out = m_out;
+  a.n = n, a.m_fp32 = m_fp32, a.pred_type = prediction_type, a.guidance = guidance, a.k = *coeffs;
+  unipc_step_kernel<<<ew_grid(n, 256), 256, 0, ST(stream)>>>(a);
   B200_LAUNCH_CHECK();
   return 0;
 }

@@ -877,6 +877,48 @@ def dpmpp_2m_step(eps_u, eps_c, guidance, x, m_prev, m_out, sigma_cur, alpha_cur
     return out
 
 
+def euler_ancestral_step(m_u, m_c, guidance, x, noise, sigma, c_out, s2p1, dt, sigma_up, prediction_type="epsilon",
+                         seed=0, step=0, out=None):
+    """EulerAncestralDiscreteScheduler.step (b200mix_euler_ancestral_step, see include/b200mix.h): noise fp32 like x,
+    or None for Philox normals keyed by (seed, step). out may be x itself."""
+    if prediction_type not in ("epsilon", "v_prediction"):
+        raise ValueError(f"euler_ancestral_step: prediction_type {prediction_type!r} must be epsilon or v_prediction")
+    fp32, out = _step_tensors("euler_ancestral_step", x, m_u, m_c, out, noise=noise)
+    _launch("b200mix_euler_ancestral_step", m_u, m_c, fp32, float(guidance), x, noise, out, x.numel(),
+            PRED_TYPES[prediction_type], float(sigma), float(c_out), float(s2p1), float(dt), float(sigma_up),
+            int(seed) & 0xFFFFFFFFFFFFFFFF, int(step))
+    return out
+
+
+def unipc_step(m_u, m_c, guidance, x, coeffs, m_out, x_corr, last_sample=None, m_prev=None, hist_c=(), hist_p=(),
+               prediction_type="epsilon", out=None):
+    """UniPCMultistepScheduler.step (b200mix_unipc_step, see include/b200mix.h). coeffs: dict of the fp32 scalars of
+    `b200mix_unipc_coeffs` (rc / rk_c / rp / rk_p: one value per history term); last_sample and m_prev (both or neither)
+    switch the corrector on; hist_c / hist_p: at most two x0 tensors each, most recent first. m_out receives x0 and
+    x_corr the corrected sample. Every tensor but the model outputs is fp32 with x's element count."""
+    hist_c, hist_p = list(hist_c), list(hist_p)
+    if len(hist_c) > 2 or len(hist_p) > 2:
+        raise ValueError("unipc_step: at most two history terms each for the corrector and the predictor (order <= 3)")
+    if (last_sample is None) != (m_prev is None) or (hist_c and last_sample is None):
+        raise ValueError("unipc_step: last_sample, m_prev and the corrector history go together")
+    bufs = dict(m_out=m_out, x_corr=x_corr, last_sample=last_sample, m_prev=m_prev)
+    bufs.update({f"corrector history {k}": t for k, t in enumerate(hist_c)})
+    bufs.update({f"predictor history {k}": t for k, t in enumerate(hist_p)})
+    if m_out is None or x_corr is None:
+        raise ValueError("unipc_step: m_out and x_corr are required")
+    fp32, out = _step_tensors("unipc_step", x, m_u, m_c, out, **bufs)
+    k = _lib.UnipcCoeffs()
+    for name in ("alpha_t", "sigma_t", "A_c", "K_c", "E_c", "rc_last", "A_p", "K_p", "E_p"):
+        setattr(k, name, float(coeffs.get(name, 0.0)))
+    for name in ("rc", "rk_c", "rp", "rk_p"):
+        vals = [float(v) for v in coeffs.get(name, ())]
+        getattr(k, name)[:len(vals)] = vals
+    hc, hp = hist_c + [None] * (2 - len(hist_c)), hist_p + [None] * (2 - len(hist_p))
+    _launch("b200mix_unipc_step", m_u, m_c, fp32, float(guidance), x, last_sample, m_prev, *hc, *hp, out, x_corr, m_out,
+            x.numel(), PRED_TYPES[prediction_type], ctypes.byref(k))
+    return out
+
+
 def scale_model_input(x: torch.Tensor, denom: float, out=None) -> torch.Tensor:
     """EulerDiscreteScheduler.scale_model_input: x / denom in fp32 (IEEE division)."""
     c = _Args("scale_model_input")

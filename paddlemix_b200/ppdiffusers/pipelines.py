@@ -19,7 +19,7 @@ import torch
 
 from .adapter import MultiAdapter
 from .controlnet import MultiControlNetModel, controlnet_keep
-from .schedulers import DDIMScheduler
+from .schedulers import DDIMScheduler, EulerAncestralDiscreteScheduler
 from .unet_2d_condition import UNet2DConditionModel
 
 bf16 = torch.bfloat16
@@ -196,11 +196,14 @@ class StableDiffusionPipeline:
         do_cfg = guidance_scale > 1.0  # pipeline_stable_diffusion.py:781
         if do_cfg and negative_prompt_embeds is None:
             negative_prompt_embeds = torch.zeros_like(prompt_embeds)
+        g = generator or torch.Generator().manual_seed(0)
         if latents is None:
             if height is None or width is None:
                 raise ValueError("height/width (or latents) are required")
-            g = generator or torch.Generator().manual_seed(0)
             latents = torch.randn(B, self.unet.config.in_channels, height // 8, width // 8, generator=g)
+        # prepare_extra_step_kwargs (pipeline_stable_diffusion.py:466-483): the stochastic Euler-ancestral step takes
+        # the call's generator (its Philox seed is drawn from it); every other scheduler's step is called as before
+        extra = {"generator": g} if isinstance(self.scheduler, EulerAncestralDiscreteScheduler) else {}
         # timesteps first (pipeline_stable_diffusion.py:808-811), then prepare_latents scales the initial noise by the
         # scheduler's init_noise_sigma (:813-824, :583): for EulerDiscrete that value depends on the chosen timesteps
         self.scheduler.set_timesteps(num_inference_steps)
@@ -238,11 +241,12 @@ class StableDiffusionPipeline:
                 # rescale_noise_cfg (pipeline_stable_diffusion.py:69-80, :886-888; SDXL :1061-1067): the guided
                 # prediction is rescaled to the text branch's per-sample std before the scheduler step
                 guided = ops.cfg_combine(eps[:B], eps[B:], guidance_scale, guidance_rescale)
-                self.scheduler.step(guided, t, latents, out=nxt)
+                self.scheduler.step(guided, t, latents, out=nxt, **extra)
             elif do_cfg:  # noise_pred_uncond + g*(noise_pred_text - noise_pred_uncond) (:882-884), fused with the step
-                self.scheduler.step(eps[:B], t, latents, model_output_cond=eps[B:], guidance_scale=guidance_scale, out=nxt)
+                self.scheduler.step(eps[:B], t, latents, model_output_cond=eps[B:], guidance_scale=guidance_scale, out=nxt,
+                                    **extra)
             else:
-                self.scheduler.step(eps, t, latents, out=nxt)
+                self.scheduler.step(eps, t, latents, out=nxt, **extra)
             latents, nxt = nxt, latents
             if callback_on_step_end is not None:
                 callback_on_step_end(self, i, t, {"latents": latents})

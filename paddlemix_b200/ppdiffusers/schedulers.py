@@ -58,6 +58,47 @@ def _sigma_to_t(sigma, log_sigmas):
     return ((1 - w) * low_idx + w * high_idx).reshape(np.shape(sigma))
 
 
+def _multistep_schedule(ac, num_inference_steps, timestep_spacing, steps_offset, use_karras_sigmas, use_lu_lambdas=False,
+                        last_timestep=None):
+    """(int64 timesteps, fp32 sigmas with one trailing entry) of the multistep solvers' set_timesteps
+    (scheduling_dpmsolver_multistep.py:226-296, scheduling_unipc_multistep.py:210-271) over the training
+    alphas_cumprod `ac`; `last_timestep` (default: every training step) is DPM-Solver's lambda_min_clipped bound. The
+    Karras / Lu schedules repeat their last sigma as the trailing entry, so their final step has h = 0."""
+    N = len(ac)
+    last_timestep = N if last_timestep is None else last_timestep
+    if timestep_spacing == "linspace":
+        timesteps = np.linspace(0, last_timestep - 1, num_inference_steps + 1).round()[::-1][:-1].copy().astype(np.int64)
+    elif timestep_spacing == "leading":
+        step_ratio = last_timestep // (num_inference_steps + 1)
+        timesteps = (np.arange(0, num_inference_steps + 1) * step_ratio).round()[::-1][:-1].copy().astype(np.int64)
+        timesteps += steps_offset
+    elif timestep_spacing == "trailing":
+        step_ratio = N / num_inference_steps
+        timesteps = np.arange(last_timestep, 0, -step_ratio).round().copy().astype(np.int64)
+        timesteps -= 1
+    else:
+        raise ValueError(f"{timestep_spacing} is not supported. Please make sure to choose one of 'linspace', "
+                         "'leading' or 'trailing'.")
+    sigmas = _train_sigmas(ac)
+    log_sigmas = np.log(sigmas)
+    if use_karras_sigmas:
+        sigmas = _karras_sigmas(sigmas[0].item(), sigmas[-1].item(), num_inference_steps)  # training sigmas ascend
+        timesteps = np.array([_sigma_to_t(s, log_sigmas) for s in sigmas]).round()
+        sigmas = np.concatenate([sigmas, sigmas[-1:]]).astype(f32)
+    elif use_lu_lambdas:
+        lambdas = np.flip(log_sigmas.copy())
+        lmin, lmax = lambdas[-1].item(), lambdas[0].item()
+        ramp = np.linspace(0, 1, num_inference_steps)
+        sigmas = np.exp(lmax + ramp * (lmin - lmax))
+        timesteps = np.array([_sigma_to_t(s, log_sigmas) for s in sigmas]).round()
+        sigmas = np.concatenate([sigmas, sigmas[-1:]]).astype(f32)
+    else:
+        sigmas = np.interp(timesteps, np.arange(0, len(sigmas)), sigmas)
+        sigma_last = np.sqrt(f32((f32(1.0) - ac[0]) / ac[0]), dtype=f32)
+        sigmas = np.concatenate([sigmas, [sigma_last]]).astype(f32)
+    return np.asarray(timesteps).astype(np.int64), sigmas
+
+
 class DDIMScheduler:
     """ppdiffusers.DDIMScheduler (scheduling_ddim.py:131) restricted to the deterministic sampling path."""
 
@@ -485,40 +526,9 @@ class DPMSolverMultistepScheduler:
         else:
             lam = np.log(np.sqrt(ac, dtype=f32), dtype=f32) - np.log(np.sqrt((f32(1.0) - ac).astype(f32), dtype=f32), dtype=f32)
             clipped_idx = int(np.searchsorted(np.flip(lam), f32(self.lambda_min_clipped)))
-        last_timestep = N - clipped_idx
-        if self.timestep_spacing == "linspace":
-            timesteps = np.linspace(0, last_timestep - 1, num_inference_steps + 1).round()[::-1][:-1].copy().astype(np.int64)
-        elif self.timestep_spacing == "leading":
-            step_ratio = last_timestep // (num_inference_steps + 1)
-            timesteps = (np.arange(0, num_inference_steps + 1) * step_ratio).round()[::-1][:-1].copy().astype(np.int64)
-            timesteps += self.steps_offset
-        elif self.timestep_spacing == "trailing":
-            step_ratio = N / num_inference_steps
-            timesteps = np.arange(last_timestep, 0, -step_ratio).round().copy().astype(np.int64)
-            timesteps -= 1
-        else:
-            raise ValueError(f"{self.timestep_spacing} is not supported. Please make sure to choose one of 'linspace', "
-                             "'leading' or 'trailing'.")
-        sigmas = _train_sigmas(ac)
-        log_sigmas = np.log(sigmas)
-        if self.use_karras_sigmas:
-            sigmas = _karras_sigmas(sigmas[0].item(), sigmas[-1].item(), num_inference_steps)  # training sigmas ascend
-            timesteps = np.array([_sigma_to_t(s, log_sigmas) for s in sigmas]).round()
-            sigmas = np.concatenate([sigmas, sigmas[-1:]]).astype(f32)
-        elif self.use_lu_lambdas:
-            lambdas = np.flip(log_sigmas.copy())
-            lmin, lmax = lambdas[-1].item(), lambdas[0].item()
-            ramp = np.linspace(0, 1, num_inference_steps)
-            sigmas = np.exp(lmax + ramp * (lmin - lmax))
-            timesteps = np.array([_sigma_to_t(s, log_sigmas) for s in sigmas]).round()
-            sigmas = np.concatenate([sigmas, sigmas[-1:]]).astype(f32)
-        else:
-            sigmas = np.interp(timesteps, np.arange(0, len(sigmas)), sigmas)
-            sigma_last = np.sqrt(f32((f32(1.0) - ac[0]) / ac[0]), dtype=f32)
-            sigmas = np.concatenate([sigmas, [sigma_last]]).astype(f32)
-        self.sigmas = sigmas
-        self.timesteps = np.asarray(timesteps).astype(np.int64)
-        self.num_inference_steps = len(timesteps)
+        self.timesteps, self.sigmas = _multistep_schedule(ac, num_inference_steps, self.timestep_spacing, self.steps_offset,
+                                                          self.use_karras_sigmas, self.use_lu_lambdas, N - clipped_idx)
+        self.num_inference_steps = len(self.timesteps)
         self.lower_order_nums = 0
         self._step_index = None
         self._m_prev = None
@@ -571,3 +581,216 @@ class DPMSolverMultistepScheduler:
         self._m_slot ^= 1
         return ops.dpmpp_2m_step(model_output, model_output_cond, guidance_scale, sample, m_prev if order == 2 else None,
                                  m_out, sigma_cur, alpha_cur, A, C, halfC, inv_r0, out=out)
+
+
+class EulerAncestralDiscreteScheduler(EulerDiscreteScheduler):
+    """ppdiffusers.EulerAncestralDiscreteScheduler ("Euler a", scheduling_euler_ancestral_discrete.py:130-389):
+    EulerDiscreteScheduler's schedule, init_noise_sigma and scale_model_input (the reference's set_timesteps :210-250
+    is EulerDiscrete's linear-interpolation path), epsilon / v_prediction. sigma_up / sigma_down (:339-347) and the
+    v-prediction factors are fp32 host scalars; `step` is one fused kernel (b200mix_euler_ancestral_step): CFG
+    combine, x0, the Euler move to sigma_down and the ancestral noise times sigma_up.
+
+    The noise is a standard normal per element. `step(..., noise=...)` uses the given fp32 tensor; otherwise the first
+    step after set_timesteps draws one 63-bit seed from `generator` (torch's default generator when None) and every step
+    takes counter-based Philox normals keyed by (seed, step index), drawn inside the kernel. One generator state
+    therefore gives one result, on any GPU and with or without CUDA graphs; the draws cannot reproduce Paddle's RNG,
+    so images differ from the reference's for the same seed, as between any two RNGs."""
+
+    def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.0001, beta_end: float = 0.02,
+                 beta_schedule: str = "linear", trained_betas=None, prediction_type: str = "epsilon",
+                 timestep_spacing: str = "linspace", steps_offset: int = 0):
+        if trained_betas is not None:
+            raise NotImplementedError("EulerAncestralDiscreteScheduler(b200): trained_betas are not supported")
+        if prediction_type == "sample":
+            raise NotImplementedError("prediction_type not implemented yet: sample")
+        if prediction_type not in ("epsilon", "v_prediction"):
+            raise ValueError(f"prediction_type given as {prediction_type} must be one of `epsilon`, or `v_prediction`")
+        # the parent's schedule does not depend on prediction_type; its own step covers epsilon only
+        super().__init__(num_train_timesteps, beta_start, beta_end, beta_schedule, timestep_spacing=timestep_spacing,
+                         steps_offset=steps_offset)
+        self.prediction_type = prediction_type
+        self._seed: Optional[int] = None
+
+    def set_timesteps(self, num_inference_steps: int):
+        super().set_timesteps(num_inference_steps)
+        self._seed = None
+
+    def step_scalars(self, timestep):
+        """(sigma, c_out, s2p1, dt, sigma_up) of this step as fp32 values, advancing the step index:
+        c_out = -sigma/(sigma^2+1)^0.5 and s2p1 = sigma^2+1 (v-prediction), sigma_up, and dt = sigma_down - sigma."""
+        if isinstance(timestep, (int, np.integer)):
+            raise ValueError("Passing integer indices (e.g. from `enumerate(timesteps)`) as timesteps to "
+                             "`EulerDiscreteScheduler.step()` is not supported. Make sure to pass one of the "
+                             "`scheduler.timesteps` as a timestep.")
+        if self._step_index is None:
+            self._init_step_index(timestep)
+        s_from, s_to = self.sigmas[self._step_index], self.sigmas[self._step_index + 1]
+        f2, t2 = f32(s_from * s_from), f32(s_to * s_to)
+        sigma_up = np.sqrt(f32(f32(t2 * f32(f2 - t2)) / f2), dtype=f32)
+        sigma_down = np.sqrt(f32(t2 - f32(sigma_up * sigma_up)), dtype=f32)
+        s2p1 = f32(f2 + f32(1.0))
+        c_out = f32(f32(-s_from) / np.sqrt(s2p1, dtype=f32))
+        self._step_index += 1
+        return float(s_from), float(c_out), float(s2p1), float(f32(sigma_down - s_from)), float(sigma_up)
+
+    def step(self, model_output, timestep, sample, generator=None, noise=None, model_output_cond=None,
+             guidance_scale=0.0, out=None):
+        """sample / result: fp32 CUDA tensors (out may be sample); model_output (and model_output_cond, same dtype, for
+        the fused CFG combine) bf16 / fp32 with sample's element count. noise: fp32 standard normals like sample, or None
+        for the Philox stream described in the class docstring."""
+        from .. import ops
+        from ..sampling import seed_from
+        if self._step_index is None:
+            self._init_step_index(timestep)
+        index = self._step_index
+        if noise is None and self._seed is None:
+            self._seed = seed_from(generator)
+        sigma, c_out, s2p1, dt, sigma_up = self.step_scalars(timestep)
+        return ops.euler_ancestral_step(model_output, model_output_cond, guidance_scale, sample, noise, sigma, c_out, s2p1,
+                                        dt, sigma_up, self.prediction_type, seed=self._seed or 0, step=index, out=out)
+
+
+class UniPCMultistepScheduler:
+    """ppdiffusers.UniPCMultistepScheduler (scheduling_unipc_multistep.py:138-843) with predict_x0 = True: solver_type
+    bh1 / bh2, solver_order 1-3, lower_order_final, disable_corrector, Karras sigmas, the three spacings,
+    epsilon / sample / v_prediction. The schedule is DPM-Solver's (_multistep_schedule); the per-step scalars of
+    convert_model_output, UniC and UniP (:368-701, including the order-3 linalg.solve) are computed on the host in
+    numpy fp32 like the reference's 0-d tensors, and `step` runs ONE fused kernel (b200mix_unipc_step): CFG combine, x0,
+    corrector, predictor. The x0 history (solver_order + 1 device buffers used as a ring) and last_sample live on the
+    device, are owned by the scheduler and never alias the caller's tensors; set_timesteps resets them."""
+
+    order = 1
+    init_noise_sigma = 1.0
+
+    def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.0001, beta_end: float = 0.02,
+                 beta_schedule: str = "linear", trained_betas=None, solver_order: int = 2,
+                 prediction_type: str = "epsilon", thresholding: bool = False,
+                 dynamic_thresholding_ratio: float = 0.995, sample_max_value: float = 1.0, predict_x0: bool = True,
+                 solver_type: str = "bh2", lower_order_final: bool = True, disable_corrector=(), solver_p=None,
+                 use_karras_sigmas: Optional[bool] = False, timestep_spacing: str = "linspace", steps_offset: int = 0):
+        if trained_betas is not None or thresholding or not predict_x0 or solver_p is not None:
+            raise NotImplementedError("UniPCMultistepScheduler(b200): the device step covers predict_x0 = True without "
+                                      "thresholding, solver_p or trained_betas")
+        if solver_order not in (1, 2, 3):
+            raise NotImplementedError("UniPCMultistepScheduler(b200): the device step covers solver_order 1-3")
+        if prediction_type not in ("epsilon", "sample", "v_prediction"):
+            raise ValueError(f"prediction_type given as {prediction_type} must be one of `epsilon`, `sample`, or"
+                             " `v_prediction` for the UniPCMultistepScheduler.")
+        self.betas, self.alphas, self.alphas_cumprod = _beta_tables(beta_schedule, beta_start, beta_end,
+                                                                    num_train_timesteps, type(self))
+        if solver_type not in ("bh1", "bh2"):
+            if solver_type not in ("midpoint", "heun", "logrho"):
+                raise NotImplementedError(f"{solver_type} does is not implemented for {type(self)}")
+            solver_type = "bh2"  # :184-188
+        self.num_train_timesteps, self.solver_order, self.solver_type = num_train_timesteps, solver_order, solver_type
+        self.prediction_type, self.lower_order_final = prediction_type, lower_order_final
+        self.disable_corrector = list(disable_corrector)
+        self.use_karras_sigmas, self.timestep_spacing, self.steps_offset = use_karras_sigmas, timestep_spacing, steps_offset
+        self.num_inference_steps: Optional[int] = None
+        self.timesteps = np.linspace(0, num_train_timesteps - 1, num_train_timesteps, dtype=f32)[::-1].copy()
+        self._reset()
+
+    def _reset(self):
+        self.lower_order_nums = 0
+        self.this_order = None
+        self._step_index: Optional[int] = None
+        self._has_last = False  # the reference's `last_sample is not None`
+        self._bufs = None       # solver_order + 1 x0 buffers, then last_sample (device fp32)
+        self._hist = []         # indices into _bufs of the x0 history, oldest first
+
+    @property
+    def step_index(self):
+        return self._step_index
+
+    def scale_model_input(self, sample, *args, **kwargs):
+        return sample
+
+    def set_timesteps(self, num_inference_steps: int):
+        self.timesteps, self.sigmas = _multistep_schedule(self.alphas_cumprod, num_inference_steps, self.timestep_spacing,
+                                                          self.steps_offset, self.use_karras_sigmas)
+        self.num_inference_steps = len(self.timesteps)
+        self._reset()
+
+    def _init_step_index(self, timestep):  # :703-718
+        cand = np.nonzero(self.timesteps == int(timestep))[0]
+        self._step_index = len(self.timesteps) - 1 if len(cand) == 0 else int(cand[1] if len(cand) > 1 else cand[0])
+
+    def _bh_coefficients(self, i_t, i_s0, hist, order, corrector):
+        """(A, K, E, rks, rhos) of multistep_uni_c_bh_update (corrector) / multistep_uni_p_bh_update from sigma index
+        i_s0 to i_t with history sigma indices `hist`: A = sigma_t/sigma_s0, K = alpha_t*h_phi_1, E = alpha_t*B_h.
+        Karras schedules repeat their last sigma: the final step has h = 0, rk = +-inf and h_phi_k = 0/0 = nan, and
+        the order-1 / order-2 updates reduce to x' = x exactly like the reference's 0-d tensor arithmetic (K = E = -0,
+        (m_k - m0)/rk = 0); a solve over nan (order 3 without lower_order_final) gives nan there, as in the reference."""
+        alpha_t, sigma_t, lam_t = DPMSolverMultistepScheduler._alpha_sigma_lambda(self.sigmas[i_t])
+        _, sigma_s0, lam_s0 = DPMSolverMultistepScheduler._alpha_sigma_lambda(self.sigmas[i_s0])
+        with np.errstate(divide="ignore", invalid="ignore"):
+            h = f32(lam_t - lam_s0)
+            rks = [f32(f32(DPMSolverMultistepScheduler._alpha_sigma_lambda(self.sigmas[si])[2] - lam_s0) / h) for si in hist]
+            r = np.array(rks + [f32(1.0)], dtype=f32)
+            hh = f32(-h)
+            h_phi_1 = np.expm1(hh, dtype=f32)
+            h_phi_k = f32(f32(h_phi_1 / hh) - f32(1.0))
+            B_h = hh if self.solver_type == "bh1" else np.expm1(hh, dtype=f32)
+            R, b, fact = [], [], 1
+            for k in range(1, order + 1):
+                R.append(r ** (k - 1))
+                b.append(f32(f32(h_phi_k * f32(fact)) / B_h))
+                fact *= k + 1
+                h_phi_k = f32(f32(h_phi_k / hh) - f32(1 / fact))
+            R, b = np.stack(R).astype(f32), np.array(b, dtype=f32)
+            if corrector:
+                rhos = [f32(0.5)] if order == 1 else list(np.linalg.solve(R, b).astype(f32))
+            else:
+                rhos = [] if order == 1 else [f32(0.5)] if order == 2 else list(np.linalg.solve(R[:-1, :-1], b[:-1]).astype(f32))
+            return (f32(sigma_t / sigma_s0), f32(alpha_t * h_phi_1), f32(alpha_t * B_h), rks, rhos)
+
+    def step_scalars(self, timestep):
+        """The fp32 scalars of this step as a dict (the fields of b200mix_unipc_coeffs, with rc / rk_c / rp / rk_p one
+        entry per history term, plus `corrector`, `order_c` and `order_p`), advancing the scheduler's state."""
+        if self.num_inference_steps is None:
+            raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after creating the "
+                             "scheduler")
+        if self._step_index is None:
+            self._init_step_index(timestep)
+        i, n = self._step_index, len(self.timesteps)
+        alpha_t, sigma_t, _ = DPMSolverMultistepScheduler._alpha_sigma_lambda(self.sigmas[i])
+        c = dict(alpha_t=float(alpha_t), sigma_t=float(sigma_t), corrector=False, order_c=0)
+        if i > 0 and (i - 1) not in self.disable_corrector and self._has_last:  # :759-761
+            p = self.this_order
+            A, K, E, rks, rhos = self._bh_coefficients(i, i - 1, [i - 1 - k for k in range(1, p)], p, True)
+            c.update(corrector=True, order_c=p, A_c=float(A), K_c=float(K), E_c=float(E), rc=[float(v) for v in rhos[:-1]],
+                     rk_c=[float(v) for v in rks], rc_last=float(rhos[-1]))
+        order = min(self.solver_order, n - i) if self.lower_order_final else self.solver_order  # :779-785
+        self.this_order = min(order, self.lower_order_nums + 1)
+        A, K, E, rks, rhos = self._bh_coefficients(i + 1, i, [i - k for k in range(1, self.this_order)], self.this_order,
+                                                   False)
+        c.update(order_p=self.this_order, A_p=float(A), K_p=float(K), E_p=float(E), rp=[float(v) for v in rhos],
+                 rk_p=[float(v) for v in rks])
+        self._has_last = True
+        if self.lower_order_nums < self.solver_order:
+            self.lower_order_nums += 1
+        self._step_index += 1
+        return c
+
+    def step(self, model_output, timestep, sample, model_output_cond=None, guidance_scale=0.0, out=None):
+        """sample / result: fp32 CUDA tensors (out may be sample); model_output (and model_output_cond, same dtype, for
+        the fused CFG combine) bf16 / fp32 with sample's element count."""
+        import torch
+
+        from .. import ops
+        c = self.step_scalars(timestep)
+        if self._bufs is None:
+            self._bufs = [torch.empty_like(sample, dtype=torch.float32) for _ in range(self.solver_order + 2)]
+        bufs, hist = self._bufs, self._hist
+        slot = next(j for j in range(self.solver_order + 1) if j not in hist)
+        last = bufs[-1]
+        corr = c["corrector"]
+        res = ops.unipc_step(model_output, model_output_cond, guidance_scale, sample, c, bufs[slot], last,
+                             last_sample=last if corr else None, m_prev=bufs[hist[-1]] if corr else None,
+                             hist_c=[bufs[hist[-1 - k]] for k in range(1, c["order_c"])],
+                             hist_p=[bufs[hist[-k]] for k in range(1, c["order_p"])],
+                             prediction_type=self.prediction_type, out=out)
+        hist.append(slot)
+        if len(hist) > self.solver_order:
+            hist.pop(0)
+        return res
