@@ -406,6 +406,42 @@ int b200mix_dpmpp_2m_step(const void* eps_u, const void* eps_c, int32_t eps_fp32
                           const float* m_prev, float* x_next, float* m_out, int64_t n, float sigma_cur, float alpha_cur,
                           float A, float C, float halfC, float inv_r0, void* stream);
 
+/* The ancestral noise z of b200mix_ddim_eta_step and b200mix_dpmpp_2m_sde_step is noise[i] (fp32, x's element count)
+ * or, with noise NULL, the Philox stream of b200mix_iddpm_step and b200mix_euler_ancestral_step keyed by
+ * (seed, step): element group g = elements 4g .. 4g+3 takes the four normals of
+ * philox4x32_10(counter = (step, g mod 2^32, g div 2^32, 0), key = (seed mod 2^32, seed div 2^32)), fp64 Box-Muller as
+ * written at b200mix_iddpm_step. */
+
+/* DDIMScheduler.step with eta > 0 (scheduling_ddim.py:410-475), fused with the CFG combine, fp32 state, one rounding
+ * per operation in this order:
+ *   m = m_u + g*(m_c - m_u)   (m_c NULL => m = m_u); m_u, m_c bf16 or fp32 (m_fp32)
+ *   x0, eps from m as in b200mix_ddim_step_ex (prediction_type 0 epsilon, 1 sample, 2 v_prediction)
+ *   clip_sample_range > 0: x0 = clip(x0, -range, range)                                  (:446-452)
+ *   use_clipped_model_output != 0: eps = (x - sa_t*x0)/sb_t, from the clipped x0          (:449-451)
+ *   x_prev = (sa_p*x0 + sb_p*eps) + std_dev_t*z                                           (:454-472)
+ * The host computes in fp32, in the reference's order, std_dev_t = eta * variance^0.5 and
+ * sb_p = (1 - alpha_prod_t_prev - std_dev_t^2)^0.5. z: see above. x_prev may alias x. */
+int b200mix_ddim_eta_step(const void* m_u, const void* m_c, int32_t m_fp32, float guidance, const float* x,
+                          const float* noise, float* x_prev, int64_t n, float sqrt_alpha_t, float sqrt_beta_t,
+                          float sqrt_alpha_prev, float sqrt_beta_prev, float std_dev_t, int32_t prediction_type,
+                          float clip_sample_range, int32_t use_clipped_model_output, uint64_t seed, int64_t step,
+                          void* stream);
+
+/* DPMSolverMultistepScheduler.step for "sde-dpmsolver++" / midpoint / epsilon prediction ("DPM-Solver++ 2M SDE",
+ * scheduling_dpmsolver_multistep.py:802-880), fused with the CFG combine, fp32 state, one rounding per operation in
+ * this order:
+ *   x0 = (x - sigma_cur*eps) / alpha_cur                                   (convert_model_output, :446-453)
+ *   x_next = A*x + B*x0                                                     (first order, :561-567)
+ *   m_prev != NULL: x_next = x_next + halfB*(inv_r0*(x0 - m_prev))          (second order midpoint, :666-674)
+ *   x_next = x_next + N*z
+ * with A = sigma_t/sigma_s0*exp(-h), B = alpha_t*(1 - exp(-2h)), halfB = 0.5*B, inv_r0 = 1/r0 and
+ * N = sigma_t*sqrt(1 - exp(-2h)) computed on the host in fp32 like the reference's 0-d tensors. m_out receives x0 (the
+ * next step's m_prev). z: see above. x_next may alias x; m_out aliases none of the inputs. */
+int b200mix_dpmpp_2m_sde_step(const void* eps_u, const void* eps_c, int32_t eps_fp32, float guidance, const float* x,
+                              const float* noise, const float* m_prev, float* x_next, float* m_out, int64_t n,
+                              float sigma_cur, float alpha_cur, float A, float B, float halfB, float inv_r0, float N,
+                              uint64_t seed, int64_t step, void* stream);
+
 /* SD3 / DiT patchify: x NCHW [B,C,H,W] (fp32|bf16) -> rows [B*(H/p)*(W/p), C*p*p] bf16 with the column order
  * (c, ph, pw) of a flattened Conv2D weight [D,C,p,p] (PatchEmbed.proj, embeddings.py:143-150), and its inverse for
  * the output head: rows [B*h*w, p*p*C] in (ph, pw, c) order -> NCHW [B,C,h*p,w*p] (transformer_sd3.py:350-356). */

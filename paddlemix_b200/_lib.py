@@ -123,6 +123,10 @@ SIGNATURES = {
                                      c_float, c_float, c_float, c_float, c_float, c_uint64, c_int64, c_void_p],
     "b200mix_unipc_step": [c_void_p, c_void_p, c_int32, c_float] + [c_void_p] * 10 + [c_int64, c_int32,
                                                                                      POINTER(UnipcCoeffs), c_void_p],
+    "b200mix_ddim_eta_step": [c_void_p, c_void_p, c_int32, c_float, c_void_p, c_void_p, c_void_p, c_int64, c_float,
+                              c_float, c_float, c_float, c_float, c_int32, c_float, c_int32, c_uint64, c_int64, c_void_p],
+    "b200mix_dpmpp_2m_sde_step": [c_void_p, c_void_p, c_int32, c_float] + [c_void_p] * 5 + [c_int64] + [c_float] * 7 +
+                                 [c_uint64, c_int64, c_void_p],
     "b200mix_scale_model_input": [c_void_p, c_void_p, c_int64, c_float, c_void_p],
     "b200mix_dpmpp_2m_step": [c_void_p, c_void_p, c_int32, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_float,
                               c_float, c_float, c_float, c_float, c_float, c_void_p],

@@ -1017,6 +1017,94 @@ extern "C" int b200mix_dpmpp_2m_step(const void* eps_u, const void* eps_c, int32
   return 0;
 }
 
+// The two stochastic steps below take one thread per group of 4 consecutive elements, which is one Philox call
+// (philox_normal4) when noise is NULL, as euler_ancestral_step_kernel does; the minimum of 4 CTAs per SM gives ptxas
+// the registers to keep the fp64 Box-Muller out of local memory. x / x_prev may alias, so they are not __restrict__.
+
+// DDIMScheduler.step with eta > 0 (scheduling_ddim.py:410-475) in the order documented at b200mix_ddim_eta_step.
+__global__ void __launch_bounds__(256, 4) ddim_eta_step_kernel(
+    const void* __restrict__ m_u, const void* __restrict__ m_c, int m_fp32, float guidance, const float* x,
+    const float* __restrict__ noise, float* x_prev, long long n, float sa_t, float sb_t, float sa_p, float sb_p,
+    float std_dev_t, int pred_type, float clip, int clipped_eps, unsigned long long seed, uint32_t step) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const long long groups = (n + 3) >> 2;
+  for (long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x; g < groups; g += (long long)gridDim.x * blockDim.x) {
+    float z[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+    if (!noise) philox_normal4(seed, step, (unsigned long long)g, z);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const long long i = 4 * g + k;
+      if (i >= n) break;
+      const float xi = x[i];
+      float x0, e;
+      predict_x0_eps(pred_type, load_guided(m_u, m_c, i, m_fp32, guidance), xi, sa_t, sb_t, x0, e);
+      if (clip > 0.0f) x0 = fminf(fmaxf(x0, -clip), clip);
+      if (clipped_eps) e = __fdiv_rn(__fsub_rn(xi, __fmul_rn(sa_t, x0)), sb_t);
+      const float mean = __fadd_rn(__fmul_rn(sa_p, x0), __fmul_rn(sb_p, e));
+      x_prev[i] = __fadd_rn(mean, __fmul_rn(std_dev_t, noise ? noise[i] : z[k]));
+    }
+  }
+}
+
+// DPM-Solver++ 2M SDE step (scheduling_dpmsolver_multistep.py:446-453, :561-567, :666-674) in the order documented at
+// b200mix_dpmpp_2m_sde_step.
+__global__ void __launch_bounds__(256, 4) dpmpp_2m_sde_step_kernel(
+    const void* __restrict__ eps_u, const void* __restrict__ eps_c, int eps_fp32, float guidance, const float* x,
+    const float* __restrict__ noise, const float* __restrict__ m_prev, float* x_next, float* __restrict__ m_out,
+    long long n, float sigma_cur, float alpha_cur, float A, float B, float halfB, float inv_r0, float N,
+    unsigned long long seed, uint32_t step) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const long long groups = (n + 3) >> 2;
+  for (long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x; g < groups; g += (long long)gridDim.x * blockDim.x) {
+    float z[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+    if (!noise) philox_normal4(seed, step, (unsigned long long)g, z);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const long long i = 4 * g + k;
+      if (i >= n) break;
+      const float xv = x[i];
+      const float m0 = __fdiv_rn(__fsub_rn(xv, __fmul_rn(sigma_cur, load_guided(eps_u, eps_c, i, eps_fp32, guidance))),
+                                 alpha_cur);
+      float r = __fadd_rn(__fmul_rn(A, xv), __fmul_rn(B, m0));
+      if (m_prev) r = __fadd_rn(r, __fmul_rn(halfB, __fmul_rn(inv_r0, __fsub_rn(m0, m_prev[i]))));
+      m_out[i] = m0;
+      x_next[i] = __fadd_rn(r, __fmul_rn(N, noise ? noise[i] : z[k]));
+    }
+  }
+}
+
+extern "C" int b200mix_ddim_eta_step(const void* m_u, const void* m_c, int32_t m_fp32, float guidance, const float* x,
+                                     const float* noise, float* x_prev, int64_t n, float sqrt_alpha_t, float sqrt_beta_t,
+                                     float sqrt_alpha_prev, float sqrt_beta_prev, float std_dev_t,
+                                     int32_t prediction_type, float clip_sample_range, int32_t use_clipped_model_output,
+                                     uint64_t seed, int64_t step, void* stream) {
+  if (int rc = ensure_device()) return rc;
+  B200_CHECK_ARG(m_u && x && x_prev && n > 0, "ddim_eta_step: bad arguments");
+  B200_CHECK_ARG(prediction_type >= 0 && prediction_type <= 2, "ddim_eta_step: prediction_type must be 0 (epsilon), 1 "
+                 "(sample) or 2 (v_prediction)");
+  B200_CHECK_ARG(step >= 0 && step <= 0xFFFFFFFFll, "ddim_eta_step: step must fit 32 bits");
+  B200_CUDA(launch_pdl(ddim_eta_step_kernel, dim3(ew_grid((n + 3) / 4, 256)), dim3(256), 0, ST(stream), 1, m_u, m_c,
+                       (int)m_fp32, guidance, x, noise, x_prev, (long long)n, sqrt_alpha_t, sqrt_beta_t, sqrt_alpha_prev,
+                       sqrt_beta_prev, std_dev_t, (int)prediction_type, clip_sample_range,
+                       (int)(use_clipped_model_output ? 1 : 0), (unsigned long long)seed, (uint32_t)step));
+  return 0;
+}
+
+extern "C" int b200mix_dpmpp_2m_sde_step(const void* eps_u, const void* eps_c, int32_t eps_fp32, float guidance,
+                                         const float* x, const float* noise, const float* m_prev, float* x_next,
+                                         float* m_out, int64_t n, float sigma_cur, float alpha_cur, float A, float B,
+                                         float halfB, float inv_r0, float N, uint64_t seed, int64_t step, void* stream) {
+  if (int rc = ensure_device()) return rc;
+  B200_CHECK_ARG(eps_u && x && x_next && m_out && n > 0 && alpha_cur != 0.0f, "dpmpp_2m_sde_step: bad arguments");
+  B200_CHECK_ARG(step >= 0 && step <= 0xFFFFFFFFll, "dpmpp_2m_sde_step: step must fit 32 bits");
+  B200_CUDA(launch_pdl(dpmpp_2m_sde_step_kernel, dim3(ew_grid((n + 3) / 4, 256)), dim3(256), 0, ST(stream), 1, eps_u,
+                       eps_c, (int)eps_fp32, guidance, x, noise, m_prev, x_next, m_out, (long long)n, sigma_cur,
+                       alpha_cur, A, B, halfB, inv_r0, N, (unsigned long long)seed, (uint32_t)step));
+  return 0;
+}
+
 extern "C" int b200mix_scale_model_input(const float* x, float* y, int64_t n, float denom, void* stream) {
   if (int rc = ensure_device()) return rc;
   B200_CHECK_ARG(x && y && n > 0 && denom > 0.0f, "scale_model_input: bad arguments");

@@ -877,6 +877,30 @@ def dpmpp_2m_step(eps_u, eps_c, guidance, x, m_prev, m_out, sigma_cur, alpha_cur
     return out
 
 
+def ddim_eta_step(m_u, m_c, guidance, x, noise, sa_t, sb_t, sa_p, sb_p, std_dev_t, prediction_type="epsilon",
+                  clip_sample_range=0.0, use_clipped_model_output=False, seed=0, step=0, out=None):
+    """DDIMScheduler.step with eta > 0 (b200mix_ddim_eta_step, see include/b200mix.h): sb_p is the direction coefficient
+    (1 - a_prev - std_dev_t^2)^0.5; noise fp32 like x, or None for Philox normals keyed by (seed, step). out may be x."""
+    fp32, out = _step_tensors("ddim_eta_step", x, m_u, m_c, out, noise=noise)
+    _launch("b200mix_ddim_eta_step", m_u, m_c, fp32, float(guidance), x, noise, out, x.numel(), float(sa_t), float(sb_t),
+            float(sa_p), float(sb_p), float(std_dev_t), PRED_TYPES[prediction_type], float(clip_sample_range),
+            1 if use_clipped_model_output else 0, int(seed) & 0xFFFFFFFFFFFFFFFF, int(step))
+    return out
+
+
+def dpmpp_2m_sde_step(eps_u, eps_c, guidance, x, noise, m_prev, m_out, sigma_cur, alpha_cur, A, B, halfB, inv_r0, N,
+                      seed=0, step=0, out=None):
+    """DPM-Solver++ 2M SDE update (b200mix_dpmpp_2m_sde_step, see include/b200mix.h); m_prev None = first-order step;
+    m_out receives x0; noise fp32 like x, or None for Philox normals keyed by (seed, step). out may be x."""
+    if m_out is None:
+        raise ValueError("dpmpp_2m_sde_step: m_out (the x0 history entry) is required")
+    fp32, out = _step_tensors("dpmpp_2m_sde_step", x, eps_u, eps_c, out, noise=noise, m_prev=m_prev, m_out=m_out)
+    _launch("b200mix_dpmpp_2m_sde_step", eps_u, eps_c, fp32, float(guidance), x, noise, m_prev, out, m_out, x.numel(),
+            float(sigma_cur), float(alpha_cur), float(A), float(B), float(halfB), float(inv_r0), float(N),
+            int(seed) & 0xFFFFFFFFFFFFFFFF, int(step))
+    return out
+
+
 def euler_ancestral_step(m_u, m_c, guidance, x, noise, sigma, c_out, s2p1, dt, sigma_up, prediction_type="epsilon",
                          seed=0, step=0, out=None):
     """EulerAncestralDiscreteScheduler.step (b200mix_euler_ancestral_step, see include/b200mix.h): noise fp32 like x,

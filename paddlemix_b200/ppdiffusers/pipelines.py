@@ -19,7 +19,7 @@ import torch
 
 from .adapter import MultiAdapter
 from .controlnet import MultiControlNetModel, controlnet_keep
-from .schedulers import DDIMScheduler, EulerAncestralDiscreteScheduler
+from .schedulers import DDIMScheduler
 from .unet_2d_condition import UNet2DConditionModel
 
 bf16 = torch.bfloat16
@@ -188,8 +188,6 @@ class StableDiffusionPipeline:
             raise ValueError("Provide either `prompt` or `prompt_embeds`. Cannot leave both `prompt` and `prompt_embeds` undefined.")
         if output_type not in ("latent", "pt"):
             raise NotImplementedError("output_type must be 'latent' or 'pt' (PIL / numpy conversion is the caller's)")
-        if eta != 0.0:
-            raise NotImplementedError("eta > 0 (stochastic DDIM) is outside the hot path")
         from .. import ops
         dev = self.unet.device
         B = prompt_embeds.shape[0]
@@ -201,9 +199,12 @@ class StableDiffusionPipeline:
             if height is None or width is None:
                 raise ValueError("height/width (or latents) are required")
             latents = torch.randn(B, self.unet.config.in_channels, height // 8, width // 8, generator=g)
-        # prepare_extra_step_kwargs (pipeline_stable_diffusion.py:466-483): the stochastic Euler-ancestral step takes
-        # the call's generator (its Philox seed is drawn from it); every other scheduler's step is called as before
-        extra = {"generator": g} if isinstance(self.scheduler, EulerAncestralDiscreteScheduler) else {}
+        # prepare_extra_step_kwargs (pipeline_stable_diffusion.py:466-483): a scheduler whose step can draw noise (Euler
+        # a, DDIM with eta > 0, DPM-Solver++ 2M SDE) takes the call's generator, which seeds its Philox stream; eta
+        # goes to DDIM and, as in the reference, is ignored by every other scheduler
+        extra = {"generator": g} if getattr(self.scheduler, "takes_generator", False) else {}
+        if isinstance(self.scheduler, DDIMScheduler):
+            extra["eta"] = eta
         # timesteps first (pipeline_stable_diffusion.py:808-811), then prepare_latents scales the initial noise by the
         # scheduler's init_noise_sigma (:813-824, :583): for EulerDiscrete that value depends on the chosen timesteps
         self.scheduler.set_timesteps(num_inference_steps)

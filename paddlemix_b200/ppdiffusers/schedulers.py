@@ -100,10 +100,21 @@ def _multistep_schedule(ac, num_inference_steps, timestep_spacing, steps_offset,
 
 
 class DDIMScheduler:
-    """ppdiffusers.DDIMScheduler (scheduling_ddim.py:131) restricted to the deterministic sampling path."""
+    """ppdiffusers.DDIMScheduler (scheduling_ddim.py:131) without dynamic thresholding. eta = 0 (the deterministic
+    sampler) runs b200mix_ddim_step_ex; eta > 0 runs b200mix_ddim_eta_step, which adds std_dev_t * z to the same mean.
+
+    The noise z of a stochastic step is a standard normal per element. `step(..., variance_noise=...)` uses the given
+    fp32 tensor; otherwise the first such step after set_timesteps draws one 63-bit seed from `generator` (torch's
+    default generator when None), and every step takes counter-based Philox normals keyed by (seed, index of the step
+    call since set_timesteps), drawn inside the kernel, exactly as EulerAncestralDiscreteScheduler does. One generator
+    state therefore gives one result, on any GPU and with or without CUDA graphs, but not Paddle's draws. In a
+    data-parallel run every rank steps its own slice of the batch with its own scheduler: the noise is keyed by that
+    rank's generator and by the element's index within the rank's latents, not by the image's global index, so ranks
+    given equal generator states draw equal noise for their slices."""
 
     order = 1
     init_noise_sigma = 1.0
+    takes_generator = True  # step(..., generator=) seeds the noise of eta > 0 (see the class docstring)
 
     def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.0001, beta_end: float = 0.02,
                  beta_schedule: str = "linear", clip_sample: bool = True, set_alpha_to_one: bool = True,
@@ -125,11 +136,13 @@ class DDIMScheduler:
         self.timestep_spacing = timestep_spacing
         self.num_inference_steps: Optional[int] = None
         self.timesteps = np.arange(0, num_train_timesteps)[::-1].copy().astype(np.int64)
+        self._step, self._seed = 0, None  # the Philox key of the stochastic steps (eta > 0)
 
     def scale_model_input(self, sample, timestep=None):
         return sample
 
     def set_timesteps(self, num_inference_steps: int):
+        self._step, self._seed = 0, None
         if num_inference_steps > self.num_train_timesteps:
             raise ValueError(
                 f"`num_inference_steps`: {num_inference_steps} cannot be larger than `self.config.train_timesteps`:"
@@ -159,6 +172,11 @@ class DDIMScheduler:
 
     def step_scalars(self, timestep: int):
         """(sqrt(a_t), sqrt(1-a_t), sqrt(a_prev), sqrt(1-a_prev-std^2)) as fp32, eta = 0 (:410-457)."""
+        return self.eta_step_scalars(timestep, 0.0)[:4]
+
+    def eta_step_scalars(self, timestep: int, eta: float):
+        """(sqrt(a_t), sqrt(1-a_t), sqrt(a_prev), sqrt(1-a_prev-std^2), std) as fp32 with std = eta * variance^0.5
+        (:410-457), each computed as the reference computes its 0-d fp32 tensor."""
         if self.num_inference_steps is None:
             raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after creating the "
                              "scheduler")
@@ -168,21 +186,36 @@ class DDIMScheduler:
         a_p = self.alphas_cumprod[prev_timestep] if prev_timestep >= 0 else self.final_alpha_cumprod
         b_t = f32(f32(1) - a_t)
         var = self._get_variance(timestep, prev_timestep)
-        std = f32(f32(0.0) * np.sqrt(var, dtype=f32))
+        std = f32(f32(eta) * np.sqrt(var, dtype=f32))
         dir_coef = np.sqrt(f32(f32(f32(1) - a_p) - f32(std * std)), dtype=f32)
-        return float(np.sqrt(a_t, dtype=f32)), float(np.sqrt(b_t, dtype=f32)), float(np.sqrt(a_p, dtype=f32)), float(dir_coef)
+        return (float(np.sqrt(a_t, dtype=f32)), float(np.sqrt(b_t, dtype=f32)), float(np.sqrt(a_p, dtype=f32)),
+                float(dir_coef), float(std))
 
     def step(self, model_output, timestep, sample, eta: float = 0.0, model_output_cond=None, guidance_scale=0.0,
-             out=None):
-        """sample, result: fp32 CUDA tensors; model_output: contiguous bf16/fp32 CUDA tensor with sample's element
-        count, read in sample's element order. With model_output_cond (same dtype) the CFG combine is fused into the same
-        kernel."""
-        if eta != 0.0:
-            raise NotImplementedError("b200mix DDIM step covers eta = 0 (the deterministic sampler the pipelines use)")
+             out=None, use_clipped_model_output: bool = False, generator=None, variance_noise=None):
+        """sample, result: fp32 CUDA tensors (out may be sample); model_output: contiguous bf16/fp32 CUDA tensor with
+        sample's element count, read in sample's element order. With model_output_cond (same dtype) the CFG combine is
+        fused into the same kernel. eta > 0 adds std_dev_t * z (see the class docstring): variance_noise is z as an fp32
+        tensor like sample, or None for the Philox stream seeded from `generator`."""
         from .. import ops
-        sa_t, sb_t, sa_p, sb_p = self.step_scalars(timestep)
-        return ops.ddim_step(model_output, model_output_cond, guidance_scale, sample, sa_t, sb_t, sa_p, sb_p,
-                             self.prediction_type, self.clip_sample_range if self.clip_sample else 0.0, out=out)
+        if eta == 0.0 and not use_clipped_model_output:
+            sa_t, sb_t, sa_p, sb_p = self.step_scalars(timestep)
+            self._step += 1
+            return ops.ddim_step(model_output, model_output_cond, guidance_scale, sample, sa_t, sb_t, sa_p, sb_p,
+                                 self.prediction_type, self.clip_sample_range if self.clip_sample else 0.0, out=out)
+        if eta < 0.0:
+            raise ValueError(f"eta must be >= 0, got {eta}")
+        if eta > 0.0 and variance_noise is not None and generator is not None:  # :459-464
+            raise ValueError("Cannot pass both generator and variance_noise. Please make sure that either `generator` or"
+                             " `variance_noise` stays `None`.")
+        sa_t, sb_t, sa_p, sb_p, std = self.eta_step_scalars(timestep, eta)
+        if eta > 0.0 and variance_noise is None and self._seed is None:
+            from ..sampling import seed_from
+            self._seed = seed_from(generator)
+        self._step += 1
+        return ops.ddim_eta_step(model_output, model_output_cond, guidance_scale, sample, variance_noise, sa_t, sb_t, sa_p,
+                                 sb_p, std, self.prediction_type, self.clip_sample_range if self.clip_sample else 0.0,
+                                 use_clipped_model_output, seed=self._seed or 0, step=self._step - 1, out=out)
 
 
 class LCMScheduler:
@@ -483,14 +516,25 @@ class EulerDiscreteScheduler:
 
 class DPMSolverMultistepScheduler:
     """ppdiffusers.DPMSolverMultistepScheduler (scheduling_dpmsolver_multistep.py:36-919) restricted to what has a device
-    step: algorithm "dpmsolver++", solver_type "midpoint", order 1 or 2, epsilon prediction (the "DPM-Solver++ 2M"
-    sampler of SD / SDXL), incl. Karras sigmas / Lu lambdas, lower_order_final, euler_at_final. The schedule and the
-    per-step scalars are computed on the host in numpy with the reference's dtypes; `step` runs ONE fused kernel
-    (`b200mix_dpmpp_2m_step`): CFG combine, x0 = (x - sigma_t*eps)/alpha_t, the first / second order update in the
-    reference's operation order, and the x0 history for the next step (kept on the device)."""
+    step: algorithm "dpmsolver++" (the "DPM-Solver++ 2M" sampler of SD / SDXL) or "sde-dpmsolver++" ("DPM-Solver++ 2M
+    SDE"), solver_type "midpoint", order 1 or 2, epsilon prediction, incl. Karras sigmas / Lu lambdas,
+    lower_order_final, euler_at_final. The schedule and the per-step scalars are computed on the host in numpy with the
+    reference's dtypes; `step` runs ONE fused kernel (`b200mix_dpmpp_2m_step`, `b200mix_dpmpp_2m_sde_step`): CFG
+    combine, x0 = (x - sigma_t*eps)/alpha_t, the first / second order update in the reference's operation order, and
+    the x0 history for the next step (kept on the device).
+
+    The SDE's noise is a standard normal per element. `step(..., noise=...)` uses the given fp32 tensor; otherwise the
+    first step after set_timesteps draws one 63-bit seed from `generator` (torch's default generator when None), and
+    every step takes counter-based Philox normals keyed by (seed, step index), drawn inside the kernel, exactly as
+    EulerAncestralDiscreteScheduler does. One generator state therefore gives one result, on any GPU and with or
+    without CUDA graphs, but not Paddle's draws. In a data-parallel run every rank steps its own slice of the batch with
+    its own scheduler: the noise is keyed by that rank's generator and by the element's index within the rank's
+    latents, not by the image's global index, so ranks given equal generator states draw equal noise for their
+    slices."""
 
     order = 1
     init_noise_sigma = 1.0
+    takes_generator = True  # step(..., generator=) seeds the SDE's noise (see the class docstring)
 
     def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.0001, beta_end: float = 0.02,
                  beta_schedule: str = "linear", solver_order: int = 2, prediction_type: str = "epsilon",
@@ -500,10 +544,11 @@ class DPMSolverMultistepScheduler:
                  variance_type: Optional[str] = None, timestep_spacing: str = "linspace", steps_offset: int = 0):
         self.betas, self.alphas, self.alphas_cumprod = _beta_tables(beta_schedule, beta_start, beta_end,
                                                                     num_train_timesteps, type(self))
-        if (algorithm_type != "dpmsolver++" or solver_type != "midpoint" or solver_order not in (1, 2) or thresholding or
-                prediction_type != "epsilon" or variance_type):
-            raise NotImplementedError("DPMSolverMultistepScheduler(b200): the device step covers dpmsolver++ / midpoint / "
-                                      "order 1-2 / epsilon prediction without thresholding")
+        if (algorithm_type not in ("dpmsolver++", "sde-dpmsolver++") or solver_type != "midpoint" or
+                solver_order not in (1, 2) or thresholding or prediction_type != "epsilon" or variance_type):
+            raise NotImplementedError("DPMSolverMultistepScheduler(b200): the device step covers dpmsolver++ / "
+                                      "sde-dpmsolver++ / midpoint / order 1-2 / epsilon prediction without thresholding")
+        self.algorithm_type = algorithm_type
         self.num_train_timesteps, self.solver_order = num_train_timesteps, solver_order
         self.lower_order_final, self.euler_at_final = lower_order_final, euler_at_final
         self.use_karras_sigmas, self.use_lu_lambdas = use_karras_sigmas, use_lu_lambdas
@@ -514,6 +559,7 @@ class DPMSolverMultistepScheduler:
         self.lower_order_nums = 0
         self._step_index: Optional[int] = None
         self._m_prev = None  # x0 prediction of the previous step (device fp32)
+        self._seed: Optional[int] = None  # the SDE's Philox key
 
     def scale_model_input(self, sample, timestep=None):
         return sample
@@ -532,6 +578,7 @@ class DPMSolverMultistepScheduler:
         self.lower_order_nums = 0
         self._step_index = None
         self._m_prev = None
+        self._seed = None
 
     @staticmethod
     def _alpha_sigma_lambda(sigma):
@@ -541,9 +588,9 @@ class DPMSolverMultistepScheduler:
         sigma_t = f32(sigma * alpha_t)
         return alpha_t, sigma_t, f32(np.log(alpha_t, dtype=f32) - np.log(sigma_t, dtype=f32))
 
-    def step_scalars(self, timestep):
-        """(order, sigma_cur, alpha_cur, A, C, halfC, inv_r0): x0 = (x - sigma_cur*eps)/alpha_cur;
-        order 1: x' = A*x - C*x0; order 2: x' = A*x - C*x0 - halfC*(inv_r0*(x0 - x0_prev))."""
+    def _advance(self, timestep):
+        """(first order?, alpha_s0, sigma_s0, alpha_t, sigma_t, h, inv_r0) of this step (the reference's control flow in
+        step, :802-880), advancing the step index and the lower-order count."""
         if self.num_inference_steps is None:
             raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after creating the scheduler")
         if self._step_index is None:
@@ -554,8 +601,6 @@ class DPMSolverMultistepScheduler:
         alpha_s0, sigma_s0, lam_s0 = self._alpha_sigma_lambda(self.sigmas[i])
         alpha_t, sigma_t, lam_t = self._alpha_sigma_lambda(self.sigmas[i + 1])
         h = f32(lam_t - lam_s0)
-        A = f32(sigma_t / sigma_s0)
-        C = f32(alpha_t * f32(np.exp(f32(-h), dtype=f32) - f32(1.0)))
         first = self.solver_order == 1 or self.lower_order_nums < 1 or lower_order_final
         inv_r0 = f32(0.0)
         if not first:
@@ -568,19 +613,58 @@ class DPMSolverMultistepScheduler:
         if self.lower_order_nums < self.solver_order:
             self.lower_order_nums += 1
         self._step_index += 1
+        return first, alpha_s0, sigma_s0, alpha_t, sigma_t, h, inv_r0
+
+    def step_scalars(self, timestep):
+        """(order, sigma_cur, alpha_cur, A, C, halfC, inv_r0): x0 = (x - sigma_cur*eps)/alpha_cur;
+        order 1: x' = A*x - C*x0; order 2: x' = A*x - C*x0 - halfC*(inv_r0*(x0 - x0_prev))."""
+        first, alpha_s0, sigma_s0, alpha_t, sigma_t, h, inv_r0 = self._advance(timestep)
+        A = f32(sigma_t / sigma_s0)
+        C = f32(alpha_t * f32(np.exp(f32(-h), dtype=f32) - f32(1.0)))
         return (1 if first else 2, float(sigma_s0), float(alpha_s0), float(A), float(C), float(f32(f32(0.5) * C)), float(inv_r0))
 
-    def step(self, model_output, timestep, sample, model_output_cond=None, guidance_scale=0.0, out=None):
+    def sde_step_scalars(self, timestep):
+        """(order, sigma_cur, alpha_cur, A, B, halfB, inv_r0, N) of an "sde-dpmsolver++" step (:561-567, :666-674):
+        x0 = (x - sigma_cur*eps)/alpha_cur; order 1: x' = A*x + B*x0 + N*z; order 2: x' = A*x + B*x0 +
+        halfB*(inv_r0*(x0 - x0_prev)) + N*z, with A = sigma_t/sigma_s0*exp(-h), B = alpha_t*(1 - exp(-2h)),
+        halfB = 0.5*B and N = sigma_t*sqrt(1 - exp(-2h))."""
+        first, alpha_s0, sigma_s0, alpha_t, sigma_t, h, inv_r0 = self._advance(timestep)
+        A = f32(f32(sigma_t / sigma_s0) * np.exp(f32(-h), dtype=f32))
+        one_minus = f32(f32(1.0) - np.exp(f32(f32(-2.0) * h), dtype=f32))
+        B = f32(alpha_t * one_minus)
+        N = f32(sigma_t * np.sqrt(one_minus, dtype=f32))
+        return (1 if first else 2, float(sigma_s0), float(alpha_s0), float(A), float(B), float(f32(f32(0.5) * B)),
+                float(inv_r0), float(N))
+
+    def step(self, model_output, timestep, sample, model_output_cond=None, guidance_scale=0.0, out=None, generator=None,
+             noise=None):
+        """sample / result: fp32 CUDA tensors (out may be sample); model_output (and model_output_cond, same dtype, for
+        the fused CFG combine) bf16 / fp32 with sample's element count. "sde-dpmsolver++" only: noise is fp32 standard
+        normals like sample, or None for the Philox stream described in the class docstring."""
         from .. import ops
-        order, sigma_cur, alpha_cur, A, C, halfC, inv_r0 = self.step_scalars(timestep)
+        sde = self.algorithm_type == "sde-dpmsolver++"
+        if noise is not None and not sde:
+            raise ValueError("DPMSolverMultistepScheduler: only algorithm_type='sde-dpmsolver++' takes noise")
+        if sde:
+            order, sigma_cur, alpha_cur, A, B, halfB, inv_r0, N = self.sde_step_scalars(timestep)
+        else:
+            order, sigma_cur, alpha_cur, A, C, halfC, inv_r0 = self.step_scalars(timestep)
         if self._m_prev is None:
             import torch
             self._m_prev = [torch.empty_like(sample), torch.empty_like(sample)]
             self._m_slot = 0
         m_out, m_prev = self._m_prev[self._m_slot], self._m_prev[self._m_slot ^ 1]
         self._m_slot ^= 1
-        return ops.dpmpp_2m_step(model_output, model_output_cond, guidance_scale, sample, m_prev if order == 2 else None,
-                                 m_out, sigma_cur, alpha_cur, A, C, halfC, inv_r0, out=out)
+        if not sde:
+            return ops.dpmpp_2m_step(model_output, model_output_cond, guidance_scale, sample,
+                                     m_prev if order == 2 else None, m_out, sigma_cur, alpha_cur, A, C, halfC, inv_r0,
+                                     out=out)
+        if noise is None and self._seed is None:
+            from ..sampling import seed_from
+            self._seed = seed_from(generator)
+        return ops.dpmpp_2m_sde_step(model_output, model_output_cond, guidance_scale, sample, noise,
+                                     m_prev if order == 2 else None, m_out, sigma_cur, alpha_cur, A, B, halfB, inv_r0, N,
+                                     seed=self._seed or 0, step=self._step_index - 1, out=out)
 
 
 class EulerAncestralDiscreteScheduler(EulerDiscreteScheduler):
@@ -594,7 +678,11 @@ class EulerAncestralDiscreteScheduler(EulerDiscreteScheduler):
     step after set_timesteps draws one 63-bit seed from `generator` (torch's default generator when None) and every step
     takes counter-based Philox normals keyed by (seed, step index), drawn inside the kernel. One generator state
     therefore gives one result, on any GPU and with or without CUDA graphs; the draws cannot reproduce Paddle's RNG,
-    so images differ from the reference's for the same seed, as between any two RNGs."""
+    so images differ from the reference's for the same seed, as between any two RNGs. In a data-parallel run every rank
+    steps its own slice of the batch with its own scheduler: the noise is keyed by that rank's generator and by the
+    element's index within the rank's latents, not by the image's global index."""
+
+    takes_generator = True  # step(..., generator=) seeds the noise
 
     def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.0001, beta_end: float = 0.02,
                  beta_schedule: str = "linear", trained_betas=None, prediction_type: str = "epsilon",

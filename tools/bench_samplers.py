@@ -1,12 +1,12 @@
-"""Cost of the Euler-ancestral and UniPC steps. Prints one JSON line:
+"""Cost of the Euler-ancestral, UniPC, stochastic DDIM and DPM-Solver++ 2M SDE steps. Prints one JSON line:
   * the GPU's name, power limit and max SM clock, read in the same run;
-  * the time of b200mix_euler_ancestral_step (in-kernel Philox noise) and of b200mix_unipc_step (order 3 with the
-    order-3 corrector: the most history it reads) at SDXL 1024^2 and SD1.5 512^2, B = 8 with CFG (bf16 model output
-    [2B, 4, h, w] into an fp32 [B, 4, h, w] state), with the bytes each reads and writes once and their share of the
-    H100 SXM data-sheet 3.35 TB/s;
+  * the time of b200mix_euler_ancestral_step, b200mix_ddim_eta_step and b200mix_dpmpp_2m_sde_step (order 2; all three
+    with in-kernel Philox noise) and of b200mix_unipc_step (order 3 with the order-3 corrector: the most history it
+    reads) at SDXL 1024^2 and SD1.5 512^2, B = 8 with CFG (bf16 model output [2B, 4, h, w] into an fp32 [B, 4, h, w]
+    state), with the bytes each reads and writes once and their share of the H100 SXM data-sheet 3.35 TB/s;
   * ms per denoising step (graph replay of the UNet + scale_model_input + scheduler step) of the SDXL 1024^2 B = 8 CFG
-    pipeline loop with synthetic weights, for Euler a and UniPC against Euler and DPM-Solver++ 2M, alternated over
-    `--repeats` rounds: median, min and max.
+    pipeline loop with synthetic weights, for Euler a, UniPC, DDIM with eta = 0.5 and DPM-Solver++ 2M SDE against
+    Euler, DDIM (eta = 0) and DPM-Solver++ 2M, alternated over `--repeats` rounds: median, min and max.
 Writes nothing to the tree.
 
     python tools/bench_samplers.py [--batch 8] [--steps 10] [--repeats 3]
@@ -52,10 +52,14 @@ def spread(v):
 
 
 def schedulers():
-    from paddlemix_b200.ppdiffusers.schedulers import (DPMSolverMultistepScheduler, EulerAncestralDiscreteScheduler,
-                                                       EulerDiscreteScheduler, UniPCMultistepScheduler)
+    from paddlemix_b200.ppdiffusers.schedulers import (DDIMScheduler, DPMSolverMultistepScheduler,
+                                                       EulerAncestralDiscreteScheduler, EulerDiscreteScheduler,
+                                                       UniPCMultistepScheduler)
     return {"euler_a": EulerAncestralDiscreteScheduler(**XL), "unipc": UniPCMultistepScheduler(**XL, solver_order=3),
-            "euler": EulerDiscreteScheduler(**XL), "dpmpp_2m": DPMSolverMultistepScheduler(**XL)}
+            "ddim_eta": DDIMScheduler(**XL, set_alpha_to_one=False),
+            "dpmpp_2m_sde": DPMSolverMultistepScheduler(**XL, algorithm_type="sde-dpmsolver++"),
+            "euler": EulerDiscreteScheduler(**XL), "ddim": DDIMScheduler(**XL, set_alpha_to_one=False),
+            "dpmpp_2m": DPMSolverMultistepScheduler(**XL)}
 
 
 def kernel_times(B, g):
@@ -82,6 +86,13 @@ def kernel_times(B, g):
             "unipc_step": (lambda i: ops.unipc_step(eps[:B], eps[B:], 5.0, x, coeffs, bufs[1], bufs[2],
                                                     last_sample=bufs[2], m_prev=bufs[3], hist_c=[bufs[4], bufs[5]],
                                                     hist_p=[bufs[3], bufs[4]], out=bufs[0]), 36 * n),
+            # reads m_u, m_c (bf16) and x, writes x_prev: 2 + 2 + 4 + 4 bytes per element
+            "ddim_eta_step": (lambda i: ops.ddim_eta_step(eps[:B], eps[B:], 5.0, x, None, 0.9, 0.43, 0.95, 0.2, 0.25,
+                                                          seed=1234, step=i, out=bufs[0]), 12 * n),
+            # order 2: reads m_u, m_c, x and m_prev, writes x_next and m_out: 2 + 2 + 4 * 2 read, 4 * 2 written
+            "dpmpp_2m_sde_step": (lambda i: ops.dpmpp_2m_sde_step(eps[:B], eps[B:], 5.0, x, None, bufs[1], bufs[2], 0.9,
+                                                                  0.6, 0.8, 0.1, 0.05, 0.7, 0.3, seed=1234, step=i,
+                                                                  out=bufs[0]), 20 * n),
         }
         for name, (fn, nbytes) in runs.items():
             for i in range(20):
@@ -137,7 +148,9 @@ def main():
             st["model_in"][:B].copy_(scaled)
             st["model_in"][B:].copy_(scaled)
             eps = den(st["model_in"], float(t))
-            kw = {"generator": gen} if key == "euler_a" else {}
+            kw = {"generator": gen} if getattr(sch, "takes_generator", False) else {}  # the pipelines' rule
+            if key == "ddim_eta":
+                kw["eta"] = 0.5
             sch.step(eps[:B], t, st["x"], model_output_cond=eps[B:], guidance_scale=5.0, out=st["nxt"], **kw)
             st["x"], st["nxt"] = st["nxt"], st["x"]
         return step
