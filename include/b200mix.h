@@ -576,6 +576,37 @@ int b200mix_kv_reorder(void* const* layer_kv, int64_t n_layers, int64_t B, int64
                        int64_t row_elems, int64_t S, int64_t max_new, const int32_t* parents, const uint64_t* state,
                        const int32_t* done, void* stream);
 
+/* ---- LoRA weight update (LoRACompatibleLinear._fuse_lora / LoRACompatibleConv._fuse_lora,
+ * ppdiffusers/models/lora.py:117-165, :312-362) -------------------------------------------------------------------
+ * One target: a device-layout bf16 weight, or a row slice of a batched one. For n < N, k < K:
+ *   out[n, k] = bf16(base[n, k] + col_scale[k] * sum_j U[n, j] * D[j, k])     (col_scale null: 1)
+ *   colsum[n] = colsum_base[n] + sum_k (out[n, k] - base[n, k])                (only when colsum is set)
+ * base is the snapshot of the weight as loaded, so the result never depends on earlier LoRA states. An element (or a
+ * colsum) whose update is exactly zero is copied from base bit for bit. U, D: fp32, row-major, contiguous. */
+typedef struct b200mix_lora_item {
+  void* out;                /* bf16 [N, ld_out] */
+  const void* base;         /* bf16 [N, ld_base], must not overlap out */
+  const float* U;           /* [N, R] */
+  const float* D;           /* [R, K] */
+  const float* col_scale;   /* [K] or null */
+  float* colsum;            /* [N] or null */
+  const float* colsum_base; /* [N]; required exactly when colsum is set */
+  int64_t ld_out, ld_base, N, K, R;
+} b200mix_lora_item;
+
+#define B200MIX_LORA_MAX_RANK 512
+
+int b200mix_lora_workspace_size(int32_t n_items, int64_t* bytes);
+
+/* Rebuilds every item's target in one persistent launch over (item, 64-row tile) work units: U @ D on tensor cores
+ * (mma.sync m16n8k8 tf32, operands rounded to tf32 with rna, fp32 accumulation over j in order), then one fp32 add
+ * and one bf16 rounding per element. Each element and each colsum is produced by one thread / warp in a fixed order,
+ * so the result is deterministic. items: host array, copied into `workspace` (16-byte aligned, at least
+ * b200mix_lora_workspace_size bytes) on `stream`. Requires R a positive multiple of 8 and <= B200MIX_LORA_MAX_RANK,
+ * K a positive multiple of 8, ld_out / ld_base multiples of 8 and >= K, out / base / U / D 16-byte aligned. */
+int b200mix_lora_apply(const b200mix_lora_item* items, int32_t n_items, void* workspace, int64_t workspace_bytes,
+                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif

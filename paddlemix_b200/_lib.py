@@ -55,6 +55,15 @@ class UnipcCoeffs(Structure):
         ("rp", c_float * 2), ("rk_p", c_float * 2)]
 
 
+class LoraItem(Structure):
+    """Mirror of `b200mix_lora_item` (include/b200mix.h): device pointers and sizes of one LoRA target."""
+
+    _fields_ = [(name, c_void_p) for name in ("out", "base", "U", "D", "col_scale", "colsum", "colsum_base")] + [
+        (name, c_int64) for name in ("ld_out", "ld_base", "N", "K", "R")]
+
+
+LORA_MAX_RANK = 512  # B200MIX_LORA_MAX_RANK
+
 ACT_NONE, ACT_SILU, ACT_GELU_ERF, ACT_GELU_TANH, ACT_QUICK_GELU, ACT_RELU = 0, 1, 2, 3, 4, 5
 GEMM_ACTS = (ACT_NONE, ACT_SILU, ACT_GELU_ERF, ACT_GELU_TANH, ACT_QUICK_GELU)  # what the GEMM epilogues implement
 GLU_NONE, GLU_GEGLU, GLU_SWIGLU = 0, 1, 2
@@ -150,6 +159,8 @@ SIGNATURES = {
                                  c_int64, c_int64, c_int64, c_float, c_float, c_double, c_int32, c_void_p],
     "b200mix_kv_reorder": [c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p,
                            c_void_p, c_void_p],
+    "b200mix_lora_workspace_size": [c_int32, POINTER(c_int64)],
+    "b200mix_lora_apply": [POINTER(LoraItem), c_int32, c_void_p, c_int64, c_void_p],
 }
 STRING_GETTERS = ("b200mix_last_error", "b200mix_version")
 

@@ -456,6 +456,12 @@ def fold_upsample_conv_weight(w: torch.Tensor) -> torch.Tensor:
     """w: [Cout, 3, 3, Cin] (any float dtype; fold from the fp32 master weights when they exist) -> bf16 [Cout, 16, Cin],
     the per-output-parity 2x2 filters of nearest-2x-upsample + conv3x3 (b200mix_conv3x3_up2x). Row index =
     (py*2 + px)*4 + a*2 + b; taps that read the same low-resolution pixel are summed in fp32 and rounded once."""
+    return fold_upsample_taps(w).to(bf16).contiguous()
+
+
+def fold_upsample_taps(w: torch.Tensor) -> torch.Tensor:
+    """The fp32 tap sums of fold_upsample_conv_weight, before rounding: [O, 3, 3, I] -> fp32 [O, 16, I]. Linear in w,
+    so it also maps a LoRA down factor's taps [r, 3, 3, I] to its columns in the folded layout."""
     O, _, _, I = w.shape
     wf = w.float()
     groups = {0: ((0,), (1, 2)), 1: ((0, 1), (2,))}  # parity -> (taps folded into a = 0, taps folded into a = 1)
@@ -465,7 +471,7 @@ def fold_upsample_conv_weight(w: torch.Tensor) -> torch.Tensor:
             for a in range(2):
                 for b in range(2):
                     out[:, py, px, a, b] = sum(wf[:, ky, kx] for ky in groups[py][a] for kx in groups[px][b])
-    return out.reshape(O, 16, I).to(bf16).contiguous()
+    return out.reshape(O, 16, I)
 
 
 def conv3x3_up2x(x: torch.Tensor, w4: torch.Tensor, bias=None, *, row_add=None, residual=None, act=ACT_NONE,
@@ -759,6 +765,69 @@ def weighted_sum_rows(xs, weights, out: torch.Tensor) -> torch.Tensor:
                 lambda: f"wsum {n}x{out.shape[0]}x{row}"):
         _launch("b200mix_weighted_sum_rows", n, ptrs, rows, ws, out, out.shape[0], row)
     return out
+
+
+def _span(t: torch.Tensor):
+    """[first byte, last byte + 1) of a tensor whose last dimension is contiguous."""
+    n = 1 + sum((s - 1) * st for s, st in zip(t.shape, t.stride()))
+    return t.data_ptr(), t.data_ptr() + n * t.element_size()
+
+
+def lora_apply(items) -> None:
+    """Rebuilds LoRA targets in one launch (b200mix_lora_apply). items: sequence of dicts with
+      out  bf16 [N, K] (a weight or a row slice of one: last dimension contiguous, row stride a multiple of 8),
+      base bf16 [N, K] (the snapshot; same layout rules), U fp32 [N, R], D fp32 [R, K] (contiguous),
+      and optionally col_scale fp32 [K], colsum / colsum_base fp32 [N] (together).
+    out[n, k] = bf16(base[n, k] + col_scale[k] * (U @ D)[n, k]); colsum = colsum_base + row sums of (out - base).
+    R must be a multiple of 8 (pad with zero columns / rows) and at most 512; K a multiple of 8. Every item is checked
+    before anything is launched; outputs must not overlap each other or any input."""
+    c = _Args("lora_apply")
+    items = list(items)
+    if not items:
+        raise ValueError("lora_apply: no items")
+    spans = []
+    for i, it in enumerate(items):
+        unknown = set(it) - {"out", "base", "U", "D", "col_scale", "colsum", "colsum_base"}
+        if unknown:
+            raise ValueError(f"lora_apply: item {i} has unknown fields {sorted(unknown)}")
+        N, K = c(f"items[{i}].out", it["out"], BF16, (None, None), ROWS)
+        R = c(f"items[{i}].U", it["U"], F32, (N, None))[1]
+        c(f"items[{i}].base", it["base"], BF16, (N, K), ROWS)
+        c(f"items[{i}].D", it["D"], F32, (R, K))
+        c(f"items[{i}].col_scale", it.get("col_scale"), F32, (K,))
+        c(f"items[{i}].colsum", it.get("colsum"), F32, (N,))
+        c(f"items[{i}].colsum_base", it.get("colsum_base"), F32, (N,))
+        if (it.get("colsum") is None) != (it.get("colsum_base") is None):
+            raise ValueError(f"lora_apply: items[{i}]: colsum and colsum_base go together")
+        if R == 0 or R % 8 or R > _lib.LORA_MAX_RANK or K % 8:
+            raise ValueError(f"lora_apply: items[{i}]: R = {R} must be a positive multiple of 8 up to "
+                             f"{_lib.LORA_MAX_RANK} and K = {K} a multiple of 8")
+        _aligned16("lora_apply", **{f"items[{i}].{k}": it[k] for k in ("out", "base", "U", "D")})
+        ins = [_span(it[k]) for k in ("base", "U", "D", "col_scale", "colsum_base") if it.get(k) is not None]
+        for k in ("out", "colsum"):
+            if it.get(k) is not None:
+                o0, o1 = _span(it[k])
+                if any(a < o1 and o0 < b for a, b in ins):
+                    raise ValueError(f"lora_apply: items[{i}].{k} overlaps one of the item's inputs")
+                spans.append((o0, o1, f"items[{i}].{k}"))
+    spans.sort()
+    for (a0, a1, na), (b0, b1, nb) in zip(spans, spans[1:]):
+        if b0 < a1:
+            raise ValueError(f"lora_apply: {na} and {nb} overlap")
+    c.on_cuda()
+    arr = (_lib.LoraItem * len(items))()
+    for i, it in enumerate(items):
+        o, b = it["out"], it["base"]
+        arr[i] = _lib.LoraItem(o.data_ptr(), b.data_ptr(), it["U"].data_ptr(), it["D"].data_ptr(),
+                               *(None if it.get(k) is None else it[k].data_ptr()
+                                 for k in ("col_scale", "colsum", "colsum_base")),
+                               o.stride(0), b.stride(0), o.shape[0], o.shape[1], it["U"].shape[1])
+    need = ctypes.c_int64()
+    check(lib.b200mix_lora_workspace_size(len(items), ctypes.byref(need)), "b200mix_lora_workspace_size")
+    ws = torch.empty(need.value, dtype=torch.uint8, device=items[0]["out"].device)
+    moved = sum(4.0 * it["out"].numel() + 4.0 * (it["U"].numel() + it["D"].numel()) for it in items)
+    with _Timed("lora", moved, "byte", lambda: f"lora {len(items)} items"):
+        _launch("b200mix_lora_apply", arr, len(items), ws, need.value)
 
 
 def zero_(t: torch.Tensor) -> torch.Tensor:

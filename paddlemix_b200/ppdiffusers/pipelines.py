@@ -143,6 +143,30 @@ class StableDiffusionPipeline:
     def __init__(self, unet: UNet2DConditionModel, scheduler: DDIMScheduler, use_cuda_graph: bool = True, vae=None):
         self.unet, self.scheduler, self.use_cuda_graph, self.vae = unet, scheduler, use_cuda_graph, vae
         self._graphed = {}
+        self._lora_scale = 1.0  # the LoRA call scale of the call in progress
+
+    # ---- LoRA (LoraLoaderMixin, loaders/lora.py:109-352; the weights live in self.unet) -------------------------------
+    def load_lora_weights(self, pretrained_model_name_or_path_or_dict, adapter_name=None, **kwargs):
+        """Loads a LoRA into the UNet (UNet2DConditionModel.load_attn_procs; text-encoder entries are skipped with a
+        warning). Captured CUDA graphs stay valid: the weights change in place."""
+        return self.unet.load_attn_procs(pretrained_model_name_or_path_or_dict, adapter_name=adapter_name, **kwargs)
+
+    def lora_state_dict(self, pretrained_model_name_or_path_or_dict, **kwargs):
+        """(state_dict, network_alphas, from_diffusers), text-encoder entries included (lora.lora_state_dict)."""
+        from .lora import lora_state_dict
+        return lora_state_dict(pretrained_model_name_or_path_or_dict, self.unet.config, **kwargs)
+
+    def fuse_lora(self, lora_scale: float = 1.0):
+        self.unet.fuse_lora(lora_scale)
+
+    def unfuse_lora(self):
+        self.unet.unfuse_lora()
+
+    def set_adapters(self, adapter_names, adapter_weights=None):
+        self.unet.set_adapters(adapter_names, adapter_weights)
+
+    def unload_lora_weights(self):
+        self.unet.unload_lora_weights()
 
     def decode_latents(self, latents):
         """pipeline_stable_diffusion.py:910-917 + VaeImageProcessor.postprocess(output_type="pt"): image =
@@ -172,7 +196,8 @@ class StableDiffusionPipeline:
         """The model output of step i for the NCHW fp32 model input (the static inputs are copied on the first step)."""
         if den is not None:
             return den(model_in, float(t), ctx if first else None, added if first else None)
-        return self.unet.forward(model_in, float(t), ctx, added_cond_kwargs=added, return_dict=False)[0]
+        return self.unet.forward(model_in, float(t), ctx, added_cond_kwargs=added,
+                                 cross_attention_kwargs={"scale": self._lora_scale}, return_dict=False)[0]
 
     @torch.no_grad()
     def __call__(self, prompt=None, height: Optional[int] = None, width: Optional[int] = None,
@@ -181,14 +206,24 @@ class StableDiffusionPipeline:
                  negative_prompt_embeds: Optional[torch.Tensor] = None, output_type: str = "latent",
                  added_cond_kwargs: Optional[Dict[str, torch.Tensor]] = None,
                  negative_added_cond_kwargs: Optional[Dict[str, torch.Tensor]] = None, callback_on_step_end=None,
-                 generator: Optional[torch.Generator] = None, guidance_rescale: float = 0.0):
+                 generator: Optional[torch.Generator] = None, guidance_rescale: float = 0.0,
+                 cross_attention_kwargs: Optional[Dict[str, Any]] = None):
+        """cross_attention_kwargs: {"scale": s} sets the LoRA call scale of the unfused adapters (default 1.0). It is
+        applied once, before the loop (one kernel launch when it changes the weights); other keys would need custom
+        attention processors, which the pipelines do not run."""
         if prompt is not None or negative_prompt is not None:
             raise NotImplementedError("text encoders are outside the hot path: pass prompt_embeds / negative_prompt_embeds")
         if prompt_embeds is None:
             raise ValueError("Provide either `prompt` or `prompt_embeds`. Cannot leave both `prompt` and `prompt_embeds` undefined.")
         if output_type not in ("latent", "pt"):
             raise NotImplementedError("output_type must be 'latent' or 'pt' (PIL / numpy conversion is the caller's)")
+        kw = dict(cross_attention_kwargs or {})
+        if set(kw) - {"scale"}:
+            raise NotImplementedError(f"cross_attention_kwargs {sorted(set(kw) - {'scale'})}: only 'scale' (the LoRA "
+                                      "scale) is supported by the pipelines")
         from .. import ops
+        self._lora_scale = float(kw.get("scale", 1.0))
+        self.unet._set_lora_scale(self._lora_scale)
         dev = self.unet.device
         B = prompt_embeds.shape[0]
         do_cfg = guidance_scale > 1.0  # pipeline_stable_diffusion.py:781
@@ -281,7 +316,8 @@ class StableDiffusionControlNetPipeline(StableDiffusionPipeline):
                  control_guidance_end: Union[float, List[float]] = 1.0,
                  added_cond_kwargs: Optional[Dict[str, torch.Tensor]] = None,
                  negative_added_cond_kwargs: Optional[Dict[str, torch.Tensor]] = None, callback_on_step_end=None,
-                 generator: Optional[torch.Generator] = None, guidance_rescale: float = 0.0):
+                 generator: Optional[torch.Generator] = None, guidance_rescale: float = 0.0,
+                 cross_attention_kwargs: Optional[Dict[str, Any]] = None):
         """`image`: the control image, fp32 [B | 1, C, H, W] in [0, 1] (a list of them, one per net, for
         Multi-ControlNet); loading and resizing images is the caller's job. Other arguments as
         StableDiffusionPipeline.__call__ and the reference (pipeline_controlnet.py:905-1003)."""
@@ -318,7 +354,7 @@ class StableDiffusionControlNetPipeline(StableDiffusionPipeline):
                                     added_cond_kwargs=added_cond_kwargs,
                                     negative_added_cond_kwargs=negative_added_cond_kwargs,
                                     callback_on_step_end=callback_on_step_end, generator=generator,
-                                    guidance_rescale=guidance_rescale)
+                                    guidance_rescale=guidance_rescale, cross_attention_kwargs=cross_attention_kwargs)
         finally:
             self._control = None
 
@@ -409,7 +445,8 @@ class StableDiffusionAdapterPipeline(StableDiffusionPipeline):
                  adapter_conditioning_scale: Union[float, List[float]] = 1.0, adapter_conditioning_factor: float = 1.0,
                  added_cond_kwargs: Optional[Dict[str, torch.Tensor]] = None,
                  negative_added_cond_kwargs: Optional[Dict[str, torch.Tensor]] = None, callback_on_step_end=None,
-                 generator: Optional[torch.Generator] = None, guidance_rescale: float = 0.0):
+                 generator: Optional[torch.Generator] = None, guidance_rescale: float = 0.0,
+                 cross_attention_kwargs: Optional[Dict[str, Any]] = None):
         """`image`: the adapter input, fp32 [B | 1, C, H, W] in [0, 1] (a list of them, one per adapter, for a
         MultiAdapter), with H and W 8x the latent size; loading and resizing images is the caller's job.
         `adapter_conditioning_scale`: a float, or for a MultiAdapter a list of one weight per adapter.
@@ -439,7 +476,7 @@ class StableDiffusionAdapterPipeline(StableDiffusionPipeline):
                                     added_cond_kwargs=added_cond_kwargs,
                                     negative_added_cond_kwargs=negative_added_cond_kwargs,
                                     callback_on_step_end=callback_on_step_end, generator=generator,
-                                    guidance_rescale=guidance_rescale)
+                                    guidance_rescale=guidance_rescale, cross_attention_kwargs=cross_attention_kwargs)
         finally:
             self._adapter = None
 

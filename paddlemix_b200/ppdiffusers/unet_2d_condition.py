@@ -22,6 +22,7 @@ import torch
 
 from ..modeling import (FrozenDict, bind, linear_bias, linear_weight, pad_head_cols, pad_head_rows, pad_head_width,
                         synthetic_state_dict, to_f32)
+from .lora import interleave_rows
 
 bf16 = torch.bfloat16
 
@@ -299,9 +300,7 @@ class _BasicTransformerBlock:
         # GEGLU: proj(x).chunk(2) = (value, gate) -> interleave rows so both land in the same accumulator tile
         w = linear_weight(P, self.name + ".ff.net.0.proj")  # [8C, C]
         b = linear_bias(P, self.name + ".ff.net.0.proj")
-        half = w.shape[0] // 2
-        w_il = torch.stack([w[:half], w[half:]], 1).reshape(2 * half, -1).contiguous()
-        b_il = torch.stack([b[:half], b[half:]], 1).reshape(2 * half).contiguous()
+        w_il, b_il = interleave_rows(w), interleave_rows(b)
         self.ff1_w = w_il.to(dev, bf16)
         self.ff1_b = b_il.to(dev)
         # norm3 folded into the GEGLU projection (W' = W * gamma, bias' = bias + W beta, column sums of W')
@@ -392,7 +391,8 @@ class _Transformer2D:
 
 
 class UNet2DConditionModel:
-    """Drop-in for ppdiffusers.UNet2DConditionModel on the denoising hot path (inference, no adapters)."""
+    """Drop-in for ppdiffusers.UNet2DConditionModel on the denoising hot path (inference; LoRA through
+    load_attn_procs)."""
 
     def __init__(self, sample_size: Optional[int] = None, in_channels: int = 4, out_channels: int = 4,
                  center_input_sample: bool = False, flip_sin_to_cos: bool = True, freq_shift: int = 0,
@@ -445,6 +445,7 @@ class UNet2DConditionModel:
         self.device = None
         self._build()
         self._graphs: Dict[Any, Any] = {}
+        self._lora = None  # lora.LoraState once a LoRA is loaded
 
     # ------------------------------------------------------------------------------------------------------------
     def _build(self):
@@ -575,8 +576,10 @@ class UNet2DConditionModel:
     def load_state_dict(self, state_dict: Dict[str, Any], device: Union[int, str] = 0):
         """Reference-named parameters (ppdiffusers state-dict keys, Paddle layouts). Every Linear is transposed once,
         convs go to [O,kh,kw,I], q/k/v (and cross k/v, time_emb_proj) are concatenated for batched GEMMs."""
-        P = state_dict
-        dev = bind(self, P, device)
+        return self._load_tensors(state_dict, bind(self, state_dict, device))
+
+    def _load_tensors(self, P, dev):
+        """The device layout of load_state_dict, built on `dev` (any torch device: the layout is plain torch)."""
         for m in self._leaves():
             m.load(P, dev)
         # batched time_emb_proj: one GEMM [B, ted] x [sum(cout), ted]^T per forward
@@ -603,7 +606,68 @@ class UNet2DConditionModel:
         for grp in self._kv_groups.values():
             grp["w"] = torch.cat(grp["w"], 0).to(dev, bf16).contiguous()
         self._graphs.clear()
+        self._lora = None  # new weights: every adapter and snapshot refers to the old ones
         return self
+
+    # ---- LoRA (loaders/unet.py:85-622; see lora.py) -----------------------------------------------------------------
+    def _lora_state(self):
+        from .lora import LoraState
+        if self.device is None:
+            raise RuntimeError("load_state_dict() must be called before loading a LoRA")
+        if self._lora is None:
+            self._lora = LoraState(self)
+        return self._lora
+
+    def load_attn_procs(self, pretrained_model_name_or_path_or_dict, network_alphas=None, adapter_name=None,
+                        from_diffusers=None):
+        """UNet2DConditionLoadersMixin.load_attn_procs (loaders/unet.py:85-421) for LoRA: a path (safetensors /
+        .pdparams) or a state dict in any format lora.lora_state_dict reads, with or without the 'unet.' prefix.
+        Text-encoder entries are skipped with one warning. The new adapter (default name default_<i>) becomes the
+        only active unfused one; the touched weights are rebuilt in place with one kernel launch, so captured CUDA
+        graphs keep working. Every check runs before any device work."""
+        from . import lora as L
+        sd, alphas, from_diffusers = L.lora_state_dict(pretrained_model_name_or_path_or_dict, self.config,
+                                                       from_diffusers)
+        if network_alphas:
+            alphas = {**(alphas or {}), **network_alphas}
+        sd, te = L.split_text_encoder(sd)
+        parsed = L.parse_lora(sd, alphas, from_diffusers, L.lora_layer_shapes(self.state_dict_shapes()))
+        L.warn_text_encoder(len(te))
+        if not parsed:
+            raise ValueError("the LoRA state dict has no UNet entries")
+        state = self._lora_state()
+        if adapter_name is None:
+            adapter_name = f"default_{len(state.adapters)}"
+        state.add(adapter_name, parsed)
+        return adapter_name
+
+    def fuse_lora(self, lora_scale: float = 1.0):
+        """loaders/unet.py:594-597: the active adapters are merged at lora_scale (times their set_adapters weight)
+        and no longer follow cross_attention_kwargs["scale"]."""
+        if self._lora is not None:
+            self._lora.fuse(lora_scale)
+
+    def unfuse_lora(self):
+        """loaders/unet.py:610-612: fused adapters return to the active unfused set."""
+        if self._lora is not None:
+            self._lora.unfuse()
+
+    def set_adapters(self, adapter_names, weights=None):
+        """Activate the named unfused adapters with per-adapter weights (a float, a list, or None for 1.0)."""
+        if self._lora is None:
+            raise ValueError("no LoRA is loaded")
+        self._lora.set_adapters(adapter_names, weights)
+
+    def unload_lora_weights(self):
+        """Drops the unfused adapters; the weights return to the loaded checkpoint plus any fused adapters."""
+        if self._lora is not None:
+            self._lora.unload()
+
+    def _set_lora_scale(self, scale: float):
+        """The call scale lambda of the unfused adapters (cross_attention_kwargs["scale"]): one kernel launch when it
+        differs from the scale the weights are realised at, none otherwise."""
+        if self._lora is not None:
+            self._lora.set_scale(scale)
 
     # ------------------------------------------------------------------------------------------------------------
     def _embeddings(self, timestep, B, added_cond_kwargs):
@@ -745,6 +809,11 @@ class UNet2DConditionModel:
         if self.device is None:
             raise RuntimeError("load_state_dict() must be called before forward()")
         dev = self.device
+        # unet_2d_condition.py:1073: "scale" is the LoRA call scale (default 1.0); it is consumed here, so a scale
+        # alone keeps the fused-processor fast path
+        kw = dict(cross_attention_kwargs or {})
+        self._set_lora_scale(kw.pop("scale", 1.0))
+        cross_attention_kwargs = kw or None
         sample = sample.to(dev)
         if sample.dtype not in (torch.float32, bf16):
             sample = sample.float()
