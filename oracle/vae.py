@@ -62,6 +62,47 @@ def vae_decoder_param_shapes(cfg) -> Dict[str, tuple]:
     return S
 
 
+def vae_decoder_layout(cfg, B, h, w):
+    """Every kernel call of AutoencoderKL.decode on a [B, latent_channels, h, w] latent, in execution order, as dicts
+    with keys name (the parameter prefix), op, B, H, W (the spatial size the op reads), cin, cout, groups and, for
+    conv3x3, residual (the resnet's conv2 adds the block input or its shortcut). op is one of small_cin (post_quant_conv,
+    conv_in), groupnorm (silu: whether SiLU follows), conv3x3, shortcut (the 1x1 GEMM), attention (the one-head mid
+    attention: cin = cout = head width) and up2x (nearest 2x + conv3x3)."""
+    boc, L, lc, G = cfg["block_out_channels"], cfg["layers_per_block"], cfg["latent_channels"], cfg["norm_num_groups"]
+    sites = []
+
+    def site(name, op, H, W, cin, cout, **kw):
+        sites.append(dict(name=name, op=op, B=B, H=H, W=W, cin=cin, cout=cout, groups=G, **kw))
+
+    def resnet(p, H, W, i, o):
+        site(p + ".norm1", "groupnorm", H, W, i, i, silu=True)
+        site(p + ".conv1", "conv3x3", H, W, i, o, residual=False)
+        site(p + ".norm2", "groupnorm", H, W, o, o, silu=True)
+        if i != o:
+            site(p + ".conv_shortcut", "shortcut", H, W, i, o)
+        site(p + ".conv2", "conv3x3", H, W, o, o, residual=True)
+
+    C = boc[-1]
+    site("post_quant_conv", "small_cin", h, w, lc, lc)
+    site("decoder.conv_in", "small_cin", h, w, lc, C)
+    resnet("decoder.mid_block.resnets.0", h, w, C, C)
+    site("decoder.mid_block.attentions.0.group_norm", "groupnorm", h, w, C, C, silu=False)
+    site("decoder.mid_block.attentions.0", "attention", h, w, C, C)
+    resnet("decoder.mid_block.resnets.1", h, w, C, C)
+    rev = list(reversed(boc))
+    out, H, W = rev[0], h, w
+    for i in range(len(boc)):
+        prev, out = out, rev[i]
+        for j in range(L + 1):
+            resnet(f"decoder.up_blocks.{i}.resnets.{j}", H, W, prev if j == 0 else out, out)
+        if i != len(boc) - 1:
+            site(f"decoder.up_blocks.{i}.upsamplers.0.conv", "up2x", H, W, out, out)
+            H, W = 2 * H, 2 * W
+    site("decoder.conv_norm_out", "groupnorm", H, W, boc[0], boc[0], silu=True)
+    site("decoder.conv_out", "conv3x3", H, W, boc[0], cfg["out_channels"], residual=False)
+    return sites
+
+
 def init_vae_params(cfg, seed=1) -> Params:
     g = torch.Generator().manual_seed(seed)
     P = {}

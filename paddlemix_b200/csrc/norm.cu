@@ -38,16 +38,27 @@ __device__ __forceinline__ float silu_f(float x) {
 // without atomics-ordering concerns) and off the FP64 pipe. The first version kept the partials in double; on this
 // part ~100 dependent DADDs per CTA (one warp, one group per lane) cost more than streaming the CTA's pixels
 // (FP64 issues at a fraction of the FP32 rate). Only the last three operations per
-// group (mean, variance from the int64 totals) are double. Block = PPB pixels x CV 8-channel vectors; each thread owns
+// group (mean, variance from the integer totals) are double. Block = PPB pixels x CV 8-channel vectors; each thread owns
 // a fixed channel vector, so every row is read with fully coalesced 16-byte loads.
+// The sums are of d = x - c, where the shift c is the group's mean over pixel 0 of the batch element (the same value in
+// every CTA), so that the variance E[d^2] - E[d]^2 does not cancel |mean| / std away in the fp32 per-thread chains (up
+// to ~3600 values at the VAE decoder's full resolution): summed about 0, the output at |mean| / std = 16 / 64 / 2^8 was
+// off by 0.005 / 0.13 / 4.8 of its RMS there. The last CTA adds the int64 partials into 128-bit totals: a group of
+// 8.4 M elements at RMS 1e4 sums to 2^66 in the 2^16 fixed point of the squares, which wrapped in int64. What must fit
+// is one CTA's partial: |sum d| < 2^39, sum d^2 < 2^47.
 // ------------------------------------------------------------------------------------------------------------
 constexpr float GN_FIX_SUM = 16777216.0f, GN_FIX_SQ = 65536.0f;
+__device__ __forceinline__ double i128_to_double(__int128 v) {
+  return static_cast<double>(static_cast<long long>(v >> 64)) * 18446744073709551616.0 +
+         static_cast<double>(static_cast<unsigned long long>(v));
+}
 __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x1, int C1, const __nv_bfloat16* __restrict__ x2,
                                 int C2, long long* __restrict__ partial, float* __restrict__ mr,  // n_per_group: 1 / elements per group
                                 unsigned int* __restrict__ counters, long long HW, int groups, int PPB, int pix_per_cta,
                                 double n_per_group, float eps) {
-  extern __shared__ float sm[];  // [PPB][2][C]
+  extern __shared__ __align__(16) float sm[];  // [PPB][2][C]
   __shared__ bool is_last;
+  __shared__ float shift[256];   // per group: the shift c
   pdl_wait();
   pdl_launch_dependents();
   const int C = C1 + C2;
@@ -56,20 +67,30 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x1, int C1, co
   const int pl = threadIdx.x / CV;
   const int b = blockIdx.y;
   const int c0 = cv * 8;
+  const int cpg = C / groups;
+  const __nv_bfloat16* x1b = x1 + static_cast<long long>(b) * HW * C1;
+  const __nv_bfloat16* x2b = x2 + static_cast<long long>(b) * HW * C2;
+  if (threadIdx.x < groups) {
+    float a = 0.0f;
+    for (int k = threadIdx.x * cpg; k < (threadIdx.x + 1) * cpg; ++k)
+      a += __bfloat162float(k < C1 ? x1b[k] : x2b[k - C1]);
+    shift[threadIdx.x] = a / static_cast<float>(cpg);
+  }
+  __syncthreads();
   const __nv_bfloat16* src;
   long long ld;
   int cc;
   if (c0 < C1) {
-    src = x1 + static_cast<long long>(b) * HW * C1, ld = C1, cc = c0;
+    src = x1b, ld = C1, cc = c0;
   } else {
-    src = x2 + static_cast<long long>(b) * HW * C2, ld = C2, cc = c0 - C1;
+    src = x2b, ld = C2, cc = c0 - C1;
   }
   const long long p_begin = static_cast<long long>(blockIdx.x) * pix_per_cta;
   const long long p_end = min(HW, p_begin + pix_per_cta);
   if (pl < PPB) {
-    float s[8], q[8];
+    float s[8], q[8], sh[8];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) s[i] = 0.0f, q[i] = 0.0f;
+    for (int i = 0; i < 8; ++i) s[i] = 0.0f, q[i] = 0.0f, sh[i] = shift[(c0 + i) / cpg];
     long long pix = p_begin + pl;
     for (; pix + 7LL * PPB < p_end; pix += 8LL * PPB) {  // 8 independent 16-byte loads in flight per thread
       uint4 w[8];
@@ -80,7 +101,7 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x1, int C1, co
         float f[8];
         unpack8(w[u], f);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) s[i] += f[i], q[i] += f[i] * f[i];
+        for (int i = 0; i < 8; ++i) f[i] -= sh[i], s[i] += f[i], q[i] += f[i] * f[i];
       }
     }
     for (; pix < p_end; pix += PPB) {
@@ -88,14 +109,13 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x1, int C1, co
       float f[8];
       unpack8(w, f);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) s[i] += f[i], q[i] += f[i] * f[i];
+      for (int i = 0; i < 8; ++i) f[i] -= sh[i], s[i] += f[i], q[i] += f[i] * f[i];
     }
     float* dst = sm + static_cast<size_t>(pl) * 2 * C;
 #pragma unroll
     for (int i = 0; i < 8; ++i) dst[c0 + i] = s[i], dst[C + c0 + i] = q[i];
   }
   __syncthreads();
-  const int cpg = C / groups;
   // `per` threads cooperate on one group (host guarantees blockDim >= groups): strided fp32 partial sums, combined in a
   // fixed order through shared memory
   const int per = blockDim.x / groups;
@@ -132,10 +152,10 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x1, int C1, co
   __syncthreads();
   if (!is_last) return;
   __threadfence();
-  long long* red = reinterpret_cast<long long*>(sm);  // [threads][2] (dynamic smem is at least threads * 16 bytes: host guarantees)
+  __int128* red = reinterpret_cast<__int128*>(sm);  // [threads][2] (dynamic smem is at least threads * 32 bytes: host guarantees)
   const int gx = gridDim.x;
   const int g = gq, j = jq;
-  long long su = 0, sq = 0;
+  __int128 su = 0, sq = 0;
   if (g < groups) {
     // L2 loads (the partials were published with __threadfence + the arrival counter), several in flight: a volatile
     // loop here would serialise one L2 round trip per partial
@@ -149,13 +169,13 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x1, int C1, co
   red[2 * threadIdx.x] = su, red[2 * threadIdx.x + 1] = sq;
   __syncthreads();
   if (g < groups && j == 0) {
-    long long ai = 0, ci = 0;
+    __int128 ai = 0, ci = 0;
     for (int t = 0; t < per; ++t) ai += red[2 * (threadIdx.x + t)], ci += red[2 * (threadIdx.x + t) + 1];
     // n_per_group arrives as its reciprocal: a double division is ~30 FP64 instructions on the kernel's critical tail
-    const double mean = static_cast<double>(ai) * (1.0 / GN_FIX_SUM) * n_per_group;
-    double var = static_cast<double>(ci) * (1.0 / GN_FIX_SQ) * n_per_group - mean * mean;
+    const double dmean = i128_to_double(ai) * (1.0 / GN_FIX_SUM) * n_per_group;  // E[x - c]
+    double var = i128_to_double(ci) * (1.0 / GN_FIX_SQ) * n_per_group - dmean * dmean;
     if (var < 0.0) var = 0.0;
-    mr[(b * groups + g) * 2 + 0] = static_cast<float>(mean);
+    mr[(b * groups + g) * 2 + 0] = static_cast<float>(static_cast<double>(shift[g]) + dmean);
     mr[(b * groups + g) * 2 + 1] = rsqrtf(static_cast<float>(var) + eps);
   }
 }
@@ -450,7 +470,7 @@ extern "C" int b200mix_groupnorm_nhwc(const void* x1, int64_t C1, const void* x2
   pix_per_cta = ((pix_per_cta + PPB - 1) / PPB) * PPB;
   if (pix_per_cta < PPB) pix_per_cta = PPB;
   const unsigned gx = (unsigned)((HW + pix_per_cta - 1) / pix_per_cta);
-  // scratch layout: [1024] uint32 arrival counters at a FIXED offset | [gx*B*groups*2] double partials | [B*groups*2]
+  // scratch layout: [1024] uint32 arrival counters at a FIXED offset | [gx*B*groups*2] int64 partials | [B*groups*2]
   // float (mean, rstd). The counters must be ZERO before the first call and are left at zero by every call (the caller
   // zero-fills the scratch once when it allocates it); they sit in front because gx - and with it the size of the
   // partial region - changes from call to call.
@@ -462,7 +482,7 @@ extern "C" int b200mix_groupnorm_nhwc(const void* x1, int64_t C1, const void* x2
   B200_CHECK_ARG(groups <= 256 && groups <= threads, "groupnorm: at most min(256, block size) groups");
   float* mr = reinterpret_cast<float*>(dstats + (long long)gx * B * groups * 2);
   dim3 grid(gx, (unsigned)B);
-  const size_t smem = std::max((size_t)PPB * 2 * C * sizeof(float), (size_t)threads * 2 * sizeof(double));
+  const size_t smem = std::max((size_t)PPB * 2 * C * sizeof(float), (size_t)threads * 2 * sizeof(__int128));
   B200_CUDA(launch_pdl(gn_stats_kernel, grid, dim3(threads), smem, st, 1, reinterpret_cast<const __nv_bfloat16*>(x1),
                        (int)C1, reinterpret_cast<const __nv_bfloat16*>(x2), (int)C2, dstats, mr, counters, (long long)HW,
                        (int)groups, PPB, (int)pix_per_cta, 1.0 / (static_cast<double>(HW) * (double)(C / groups)), eps));
